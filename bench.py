@@ -5,8 +5,8 @@
     python bench.py --impl reference --gpus 1 --steps 2 --warmup 1   # CPU arm: the oracle port
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ... # one rank per GPU (NCCL)
 
-Workload (BASELINE.json configs[1]): VQ-8192 tokenizer training, bf16 autocast, per-GPU batch 256,
-256x256 synthetic images, random-init ViT-B encoder/decoder.  One step = VQModel forward
+Workload: VQ-8192 tokenizer training, bf16 autocast, per-GPU batch 128 (the reference recipe's global batch 1024
+over 8 processes; it fits the 80 GB of an H100), 256x256 synthetic images, random-init ViT-B encoder/decoder.  One step = VQModel forward
 (encode -> quantize -> latent perturbation -> decode) + L2 reconstruction/vq/commit losses + backward
 + AdamW (+ DDP gradient all-reduce for N > 1): the body of xqgan_train.py:448-462 restricted to the
 in-scope path (no LPIPS / discriminator / frozen teacher, whose weights cannot be downloaded here --
@@ -17,6 +17,7 @@ Prints ONE JSON line (rank 0).
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -39,14 +40,17 @@ def parse():
     p.add_argument("--steps", type=int, default=6)
     p.add_argument("--warmup", type=int, default=3)
     p.add_argument("--impl", type=str, default="ours", choices=["ours", "reference", "eager"],
-                   help="ours: libxqb200 path; reference: CPU oracle port (the contract's reference arm); eager: the "
+                   help="ours: libxqb200 path; reference: CPU oracle port (the host-core reference arm); eager: the "
                         "reference's way of computing the path in plain PyTorch on the SAME GPU (extra, informative)")
     p.add_argument("--workload", type=str, default=WORKLOAD)
-    p.add_argument("--batch", type=int, default=256, help="per-GPU batch")
+    p.add_argument("--batch", type=int, default=128, help="per-GPU batch")
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--no-extra", action="store_true", help="skip the MSVR10P2-4096 ours-vs-eager extra measurement")
     p.add_argument("--fp32-grads", action="store_true", help="multi-GPU: all-reduce fp32 gradient buckets (stock DDP) instead of bf16")
     p.add_argument("--cpu-sample", type=int, default=0, help="images per CPU-baseline step (0 = auto)")
+    p.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                   help="write what the last timed step computed (losses, a fixed sample of the reconstruction, the token "
+                        "indices, a fixed sample of the updated parameters) as DIR/<name>.npy, to compare two builds")
     return p.parse_args()
 
 
@@ -64,7 +68,7 @@ def build_model(workload: str, device):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -76,6 +80,7 @@ class ClockSampler:
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits",
                                           "-i", str(self.index), "-lms", "200"], stdout=subprocess.PIPE, text=True)
+            atexit.register(self.proc.terminate)        # never outlive the benchmark, whatever ends it
             threading.Thread(target=self._read, daemon=True).start()
         except Exception:
             self.proc = None
@@ -148,14 +153,15 @@ def _safe(fn):
 
 def peaks():
     """(HBM GB/s, dense bf16 TFLOP/s, source).  Every kernel bench.py times sits inside a long training step, so the tensor
-    roof is the SUSTAINED cuBLAS figure of MEASURED_PEAKS.json (the burst one is for a kernel timed alone)."""
+    roof is the SUSTAINED cuBLAS figure of MEASURED_PEAKS.json (the burst one is for a kernel timed alone).  Without that file:
+    the H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16 at 700 W), which a power-limited card does not reach."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
         if "bf16_tflops_sustained" in d:
-            return d.get("hbm_gbs", 6650.0), d["bf16_tflops_sustained"], "measured (MEASURED_PEAKS.json: hbm_gbs, bf16_tflops_sustained)"
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured (MEASURED_PEAKS.json: hbm_gbs, bf16_tflops)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+            return d.get("hbm_gbs", 3350.0), d["bf16_tflops_sustained"], "measured (MEASURED_PEAKS.json: hbm_gbs, bf16_tflops_sustained)"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), "measured (MEASURED_PEAKS.json: hbm_gbs, bf16_tflops)"
+    return 3350.0, 989.0, "fallback (H100 SXM data sheet, not a measured peak)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -220,6 +226,7 @@ def make_step(ctx, workload, B, impl):
         opt.zero_grad(set_to_none=True)
         loss.backward()
         opt.step()
+        step.last = {"loss": loss, "vq_loss": vq, "commit_loss": commit, "entropy_loss": ent, "reconstruction": dec}
         return loss
 
     g = torch.Generator(device=ctx.dev).manual_seed(1234 * ctx.world + ctx.rank)
@@ -303,23 +310,20 @@ def quantizer_roofline(workload, margs, B, kern_ms, entry, hbm, tf, src):
     tfs = flops_alg / (kern_ms * 1e-3) / 1e12
     if multi:
         name = "ms_forward_kernel (fused 10-scale residual loop in shared memory, FP32 search); timed = one xq_ms_forward call (one PQ branch)"
+        tkey = f"ms_forward_kernel/{workload}/B{B}"
         note = ("10 DEPENDENT scales per image: latency x 10 bounds the kernel; the per-scale searches are CUDA-core FP32 "
                 "(DESIGN.md section 9), so the tensor fraction is reported against the contraction's roof, not achieved on tensor cores")
-        tkey = f"ms_forward_kernel/{workload}/B{B}"
     else:
         tc = (C in (32, 64)) and os.environ.get("XQ_VQ_ALGO", "auto")[0] != "e"
-        name = ("vq_search_tc_kernel (tcgen05 TF32 screening + exact fp32 rescoring)" if tc else
+        name = ("vq_search_tc_kernel (wgmma TF32 screening + exact fp32 rescoring)" if tc else
                 "vq_search_kernel (exact fp32 CUDA-core)") + "; timed = the xq_vq_forward call (codebook prep + search + loss finalize)"
         note = "contraction-bound, not HBM-bound (arithmetic intensity ~1900 FLOP/B, DESIGN.md section 5)"
         tkey = f"vq_search_tc_kernel/N{rows_branch}/V{V}/C{C}"
     out = {"bound": "tensor", "kernel": name, "achieved": tfs, "peak": tf, "unit": "TFLOP/s", "frac": tfs / tf,
-           "traffic": traffic.get(tkey), "peak_source": src + " (dense bf16 cuBLAS; no TF32 peak is measured on this pool)",
+           "traffic": traffic.get(tkey), "peak_source": src + " (dense bf16; no TF32 peak is measured)",
            "kernel_ms": kern_ms, "algorithmic_flops": flops_alg, "algorithmic_bytes": bytes_alg, "hbm_gbs": gbs,
            "hbm_frac": gbs / hbm, "note": note + "; traffic = dram bytes/launch from the committed ncu capture of this "
            "kernel + shape (profiles/ncu_traffic.json), null when that shape was not captured"}
-    if not multi:
-        # TMEM -> register read floor of the tcgen05 path: every approximate score (N*V fp32) crosses the tcgen05.ld port once
-        out["tmem_read_floor_ms"] = rows_branch * V * 4 / (125.0 * 148 * 1.9e9) * 1e3
     return out
 
 
@@ -437,6 +441,8 @@ def run_ours(a):
 
     ms, ms_e2e = ctx.max_over_ranks(ms, ms_e2e)
     peak_mem = torch.cuda.max_memory_allocated() / 2 ** 30
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, model, step.last)
 
     extra = None
     if a.impl == "ours" and not a.no_extra:
@@ -487,14 +493,42 @@ def run_ours(a):
         ctx.dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, model, last, n_sample=1 << 20):
+    """What the last timed step computed, as DIR/<name>.npy: its losses (float64), the token indices of every quantizer
+    (float64, exact), and float32 samples of the reconstruction and of the updated parameters -- the same n_sample element
+    positions on every run (seeded), so that two builds of the project can be compared output for output (~9 MB in all)."""
+    import numpy as np
+
+    def sample(t):
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() <= n_sample:
+            return flat
+        g = torch.Generator().manual_seed(0)
+        return flat[torch.randint(0, flat.numel(), (n_sample,), generator=g).to(flat.device)]
+
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.array([float(torch.as_tensor(last[k]).detach())], dtype=np.float64) for k in ("loss", "vq_loss", "commit_loss", "entropy_loss")}
+    arrays["reconstruction_sample"] = sample(last["reconstruction"]).cpu().numpy()
+    idx = []
+    for m in model.modules():
+        if getattr(m, "last_idx", None) is not None:
+            idx.append(m.last_idx.reshape(-1))
+        elif getattr(m, "last_idx_Bl", None) is not None:
+            idx.extend(t.reshape(-1) for t in m.last_idx_Bl)
+    if idx:
+        arrays["tokens"] = torch.cat([t.to(torch.float64) for t in idx]).cpu().numpy()
+    arrays["params_sample"] = sample(torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])).cpu().numpy()
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+
+
 # ----------------------------------------------------------------------------------------------
 def cpu_arm(a, steps, warmup, state=None, margs=None, budget_s=14.0):
     """the oracle port of the same training step on the host cores (bounded sample: about `budget_s` seconds of
     CPU work per timed step, so the whole arm ends within minutes whatever --steps is)."""
     from oracle import vit_ref, xq_oracle as xo
     import torch.nn.functional as F  # noqa: F401
-    # measured on the B200 host (128-core Xeon 8562Y+, tools/cpu_probe.py): 16 threads 1.10 img/s, 32 -> 1.05,
-    # 64 -> 0.53, 128 -> pathological (> 90 s/step): the step's small GEMMs do not scale past ~16-32 threads
+    # the step's small GEMMs do not scale past ~16-32 host threads (tools/cpu_probe.py measures it on a given host)
     cores = min(os.cpu_count() or 1, 16)
     torch.set_num_threads(cores)
     xo.set_num_threads(cores)
@@ -534,7 +568,7 @@ def workload_config(a, world):
                         "fwd+bwd+AdamW, L2+vq+commit loss (no LPIPS/GAN/teacher)",
             "global_batch": world * B, "parallelism": f"dp{world}",
             "grad_allreduce": ("none (1 GPU)" if world == 1 else ("fp32 buckets" if a.fp32_grads else "bf16-compressed buckets (fp32 master weights)")),
-            "l2_policy": "inputs (201 MB/step) + activations exceed the 126 MB L2"}
+            "l2_policy": "inputs (201 MB/step) + activations exceed the 50 MB L2"}
 
 
 def run_reference(a):

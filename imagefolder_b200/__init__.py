@@ -1,4 +1,4 @@
-"""imagefolder_b200 -- B200-native (sm_100a) hot path of the XQ-GAN / ImageFolder image tokenizer.
+"""imagefolder_b200 -- H100-native (sm_90a) hot path of the XQ-GAN / ImageFolder image tokenizer.
 
 Public surface mirrors the reference modules (SURVEY.md section 8b):
     VectorQuantizer, VectorQuantizer2, LFQ, add_perturbation / add_perturb, VQModel, ModelArgs,

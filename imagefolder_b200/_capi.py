@@ -45,7 +45,7 @@ def lib() -> ctypes.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise XqError(
-            f"{LIB_PATH} not found: the sm_100a CUDA library is required (there is no CPU/PyTorch fallback). "
+            f"{LIB_PATH} not found: the sm_90a CUDA library is required (there is no CPU/PyTorch fallback). "
             "Build it with `python -c 'import __graft_entry__ as g; g.build()'` or imagefolder_b200/csrc/build.sh")
     L = ctypes.CDLL(LIB_PATH)
     vp, f32p, i64p = c_void_p, c_void_p, c_void_p  # device pointers are passed as integers

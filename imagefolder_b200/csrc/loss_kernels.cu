@@ -1,4 +1,4 @@
-// loss_kernels.cu -- SURVEY.md section 8 row f-1: the HBM-bound pieces of the training loss stack (sm_100a).
+// loss_kernels.cu -- SURVEY.md section 8 row f-1: the HBM-bound pieces of the training loss stack (sm_90a).
 //
 //   lpips_layer_*   tokenizer/tokenizer_image/lpips.py:79-90 -- per VGG stage: channel-normalise both feature maps,
 //                   squared difference, 1x1 `lin` conv (a per-channel weight), spatial mean.  The reference runs ~10

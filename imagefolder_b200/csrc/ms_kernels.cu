@@ -1,4 +1,4 @@
-// ms_kernels.cu -- fused multi-scale residual quantizers (sm_100a).
+// ms_kernels.cu -- fused multi-scale residual quantizers (sm_90a).
 //
 // Replaces the arithmetic of
 //   VectorQuantizer2.forward / f_to_idxBl_or_fhat / embed_to_fhat / idxBl_to_var_input

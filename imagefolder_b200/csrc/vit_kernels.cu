@@ -1,4 +1,4 @@
-// vit_kernels.cu -- HBM-bound glue kernels of the ViT encoder/decoder blocks (sm_100a).
+// vit_kernels.cu -- HBM-bound glue kernels of the ViT encoder/decoder blocks (sm_90a).
 //
 // The reference block (dino_enc/vision_transformer.py:336-339) is
 //     x = x + drop_path(ls1(attn(norm1(x))));   x = x + drop_path(ls2(mlp(norm2(x))))
@@ -122,12 +122,10 @@ residual_ln_fwd_kernel(const float *__restrict__ x, const __nv_bfloat16 *__restr
 }
 
 // ---- TMA-bulk staged streaming skeleton -------------------------------------------------------------------------
-// tools/mb/stream_mb.cu (B200): a persistent 1-CTA-per-SM kernel whose producer warp stages row tiles into shared memory
-// with cp.async.bulk (1-D TMA, mbarrier complete_tx) and whose consumer warps each own one row of the tile, with tiles
-// handed out by an atomic counter, streams at 6.7-6.8 TB/s INCLUDING register-resident column sums -- the same rate as a
-// flat copy -- where the best register-load loop (grid-stride, software-pipelined) reaches 5.7-6.0 and the previous
-// warp-per-row LayerNorm backward 4.5.  No registers are spent on loads in flight and the memory system always has
-// NST-1 tiles outstanding.
+// A persistent 1-CTA-per-SM kernel whose producer warp stages row tiles into shared memory with cp.async.bulk (1-D TMA,
+// mbarrier complete_tx) and whose consumer warps each own one row of the tile, with tiles handed out by an atomic counter:
+// no registers are spent on loads in flight and the memory system always has NST-1 tiles outstanding, so the register-
+// resident column sums ride along with a flat-copy-like stream (tools/mb/stream_mb.cu compares the skeletons).
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -379,8 +377,8 @@ __device__ __forceinline__ void load_bias8(const float *bias, int c, float (&bb)
 }
 __global__ void gelu_fwd_kernel(const uint4 *__restrict__ x, const float *__restrict__ bias, uint4 *__restrict__ y,
                                 int M, int C8) {
-    // NON-persistent: one CTA per GELU_RU rows.  tools/mb/stream_mb.cu on B200: fresh small CTAs stream at 6.1 TB/s where
-    // the persistent grid-stride form of the same loop reaches 5.4 (lock-step load/store phases + SM imbalance).
+    // NON-persistent: one CTA per GELU_RU rows.  Fresh small CTAs avoid the lock-step load/store phases and SM imbalance of
+    // the persistent grid-stride form of the same loop (tools/mb/stream_mb.cu compares the two).
     const int row0 = blockIdx.x * GELU_RU;
     for (int c = threadIdx.x; c < C8; c += blockDim.x) {
         float bb[8];

@@ -1,4 +1,4 @@
-// vq_kernels.cu -- single-scale VectorQuantizer + latent perturbation kernels (sm_100a).
+// vq_kernels.cu -- single-scale VectorQuantizer + latent perturbation kernels (sm_90a).
 //
 // Replaces the arithmetic of
 //   VectorQuantizer.forward / f_to_idxBl_or_fhat   tokenizer/tokenizer_image/xqgan_model.py:745-833
@@ -530,7 +530,7 @@ int xq_vq_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     cudaStream_t stream = (cudaStream_t)stream_;
     const int algo = vq_algo();
     if (algo != 1 && vq_tc_supported(C, V, codebook_norm)) {
-        // tcgen05 screening + exact rescoring (bit-identical to the CUDA-core kernel below)
+        // TF32 wgmma screening + exact rescoring (bit-identical to the CUDA-core kernel below)
         int rc = vq_tc_forward(z, E, B, C, HW, V, ste_value, beta, idx, out, loss, hist, workspace, workspace_bytes, stream);
         if (rc != XQ_ERR_UNSUPPORTED) return rc;
         if (algo == 2) return rc;

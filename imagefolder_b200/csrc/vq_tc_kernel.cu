@@ -1,13 +1,12 @@
-// vq_tc_kernel.cu -- tcgen05 / TMEM / TMA version of the fused VQ search (sm_100a).
+// vq_tc_kernel.cu -- wgmma / TMA version of the fused VQ search (sm_90a).
 //
 // Same contract and same BIT-EXACT results as vq_search_kernel (vq_kernels.cu), reached differently:
 //
-//   screening   the -2<z,c> inner products of a 128-row x 256-code tile are computed by ONE thread issuing
-//               tcgen05.mma.kind::tf32 (operands in 128B-swizzled shared memory: rows written by the CTA,
-//               code tiles streamed by TMA), accumulators in TMEM (2 x 256 columns, double buffered);
-//   epilogue    4 warps read their TMEM lanes with tcgen05.ld (32 columns at a time), take the maximum of each
-//               32-code group with FMNMX3 trees and remember, per row, the few groups whose maximum is
-//               within W of the running maximum (a push is ~10 instructions; no per-element scan);
+//   screening   the -2<z,c> inner products of a 128-row x 128-code tile are computed by two warpgroups issuing
+//               wgmma.m64n128k8.tf32 (A = the CTA's rows, B = code tiles streamed by TMA, both 128B-swizzled shared
+//               memory), accumulators in registers, handed to the epilogue warpgroup through a shared-memory score tile;
+//   epilogue    one thread per row takes the maximum of each 32-code group and remembers, per row, the few groups
+//               whose maximum is within W of the running maximum (a push is ~10 instructions; no per-element scan);
 //   rescoring   only the codes of those groups (1.1 groups per row on average) are re-scored with the
 //               canonical fp32 arithmetic (fmaf chain, d = (zz+ee) - 2 dot, first index on ties) -> the index
 //               equals the exact kernel's and the oracle's: the true argmin provably lies in a kept group.
@@ -16,107 +15,41 @@
 // each, so |dot_tf32 - dot| <= 2^-9 * sum|z_k c_k| <= 1.96e-3.  We use eps = 2.5e-3 and keep every code with
 // score >= running_max - (2 eps + 2e-6)  (the 2e-6 covers the fp32 rounding of zz + ee in the canonical key).
 //
-// Roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2-5 = epilogue
-// (TMEM lane quadrant = warp_id % 4).  Pipelines: full/empty mbarriers per smem stage (TMA <-> MMA),
-// tmem_full/tmem_empty per accumulator stage (MMA <-> epilogue).
+// Roles (416 threads): warpgroups 0-1 = MMA (rows 64 wg .. 64 wg + 63), warpgroup 2 = epilogue (thread = row),
+// warp 12 = TMA producer.  Pipelines: full/empty mbarriers per smem stage (TMA <-> MMA), s_full/s_empty for the score
+// tile (MMA <-> epilogue).
 #include <cuda.h>
 #include <mutex>
 
 #include "xq_common.cuh"
+#include "xq_tc.cuh"
 
 namespace xq {
 
 static long long *g_vq_tc_trace = nullptr;     // in-kernel clock trace buffer (development builds only)
 
-constexpr int TC_BM = 128;       // rows per CTA  (UMMA M)
-constexpr int TC_BN = 128;       // codes per tile (UMMA N); 2 accumulator stages = 256 TMEM columns -> 2 CTAs / SM
-constexpr int TC_THREADS = 192;
+constexpr int TC_BM = 128;       // rows per CTA  (two wgmma M = 64 halves)
+constexpr int TC_BN = 128;       // codes per tile (wgmma N)
+constexpr int TC_THREADS = 416;
+constexpr int TC_SLD = TC_BN + 1;   // score tile row pitch (floats): one row per epilogue thread, conflict-free columns
 constexpr int TC_CAP = 16;       // candidate-group slots per row
 constexpr float TC_EPS = 2.5e-3f;
 constexpr float TC_W = 2.0f * TC_EPS + 2e-6f;
 
-// ---- PTX wrappers ----------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+using xqtc::desc_k_sw128;
+using xqtc::elect_one;
+using xqtc::fence_async_smem;
+using xqtc::mbar_arrive;
+using xqtc::mbar_expect_tx;
+using xqtc::mbar_init;
+using xqtc::mbar_wait;
+using xqtc::smem_u32;
 
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.b32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-    } while (!done);
-}
 __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int x, int y, uint64_t *bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
         : "memory");
-}
-// one lane of a CONVERGED warp: single-thread tcgen05 / TMA instructions issued under `if (lane == 0)` are wrapped by the
-// compiler in an ELECT / BRA.U.ANY serialisation loop (~112 clk per tcgen05.mma measured, tools/umma_probe.cu); issued under
-// elect.sync by a warp that runs the control flow uniformly they are plain predicated instructions (tensor-pipe rate)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// UMMA shared-memory descriptor: K-major operand, SWIZZLE_128B, 8-row atoms 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address >> 4            bits [0,14)
-    d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset = 1024 B   bits [32,46)
-    d |= (uint64_t)1 << 46;                         // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                         // layout type: SWIZZLE_128B
-    return d;
-}
-// instruction descriptor: D = F32, A = B = TF32, both K-major, M = 128, N = 256
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // byte offset of element (row, k) inside a K-major SWIZZLE_128B operand made of 32-float (128 B) K chunks
@@ -141,34 +74,36 @@ __device__ __forceinline__ void cand_push(float m1, float m2, int code, float *c
 
 struct TcSmem {
     float *A;        // [C/32][128][32]  swizzled
-    float *B;        // [NSTAGE][C/32][256][32] swizzled (TMA)
+    float *B;        // [NSTAGE][C/32][128][32] swizzled (TMA)
+    float *S;        // [128][TC_SLD] approximate scores of the current code tile
     float *cand_s;   // [128][CAP] best score of the group
     float *cand_s2;  // [128][CAP] runner-up score of the group
     int *cand_v;     // [128][CAP] code with the best score (group = code >> 5)
     float *zz, *red;
     int *idx;
-    uint64_t *full, *empty, *tfull, *tempty;
-    uint32_t *tmem_ptr;
+    uint64_t *full, *empty, *sfull, *sempty;
 };
 
 static size_t tc_smem_bytes(int C, int nstage) {
     size_t b = 1024;                                        // alignment slack
     b += (size_t)TC_BM * C * 4;                             // A
     b += (size_t)nstage * TC_BN * C * 4;                    // B
+    b += (size_t)TC_BM * TC_SLD * 4;                        // S
     b += (size_t)TC_BM * TC_CAP * 12;                       // candidates
     b += (size_t)TC_BM * 4 * 2 + 32 * 4;                    // zz, idx, red
-    b += 8 * (2 * 8 + 4) + 16;                              // barriers + tmem ptr
+    b += 8 * (2 * 8 + 2);                                   // barriers
     return b;
 }
 
-__global__ void __launch_bounds__(TC_THREADS, 2)
+template <int KC>   // 128-byte K chunks: C / 32
+__global__ void __launch_bounds__(TC_THREADS, 1)
 vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__restrict__ z, const float *__restrict__ E,
                     const float *__restrict__ En, const float *__restrict__ ee, int N, int C, int HW, int V, int Vpad,
                     int nstage, int ste_value, int64_t *__restrict__ idx_out, float *__restrict__ out,
                     float *__restrict__ partial, float *__restrict__ hist, long long *__restrict__ dbg) {
     extern __shared__ uint8_t smem_raw[];
-    // dbg (optional, CTA 0 only): [0] start, [1] after prologue; per tile t: [8+4t+0] mma waited tempty,
-    // [+1] mma waited full, [+2] mma issued+committed, [+3] epilogue warp 2 done with tile
+    // dbg (optional, CTA 0 only): [0] start, [1] after prologue; per tile t: [8+4t+1] MMA warp 0 waited full,
+    // [+2] its MMAs retired, [+3] epilogue warp 8 done with tile
     const bool trace = dbg && blockIdx.x == 0;
     if (trace && threadIdx.x == 0) dbg[0] = clock64();
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -176,6 +111,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
     s.A = (float *)base;
     s.B = (float *)(base + (size_t)TC_BM * C * 4);
     uint8_t *p = base + (size_t)TC_BM * C * 4 + (size_t)nstage * TC_BN * C * 4;
+    s.S = (float *)p; p += (size_t)TC_BM * TC_SLD * 4;
     s.cand_s = (float *)p; p += (size_t)TC_BM * TC_CAP * 4;
     s.cand_s2 = (float *)p; p += (size_t)TC_BM * TC_CAP * 4;
     s.cand_v = (int *)p; p += (size_t)TC_BM * TC_CAP * 4;
@@ -184,24 +120,20 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
     s.red = (float *)p; p += 32 * 4;
     s.full = (uint64_t *)p; p += 8 * 8;
     s.empty = (uint64_t *)p; p += 8 * 8;
-    s.tfull = (uint64_t *)p; p += 2 * 8;
-    s.tempty = (uint64_t *)p; p += 2 * 8;
-    s.tmem_ptr = (uint32_t *)p;
+    s.sfull = (uint64_t *)p; p += 8;
+    s.sempty = (uint64_t *)p;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int row0 = blockIdx.x * TC_BM;
-    const int KC = C >> 5;                       // 128-byte K chunks
     const int T = Vpad / TC_BN;
     const uint32_t stage_bytes = (uint32_t)TC_BN * C * 4;
 
     if (tid == 0) {
-        for (int i = 0; i < nstage; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&s.tfull[i], 1); mbar_init(&s.tempty[i], 4); }
+        // empty: one arrival per MMA warp; sfull: every MMA thread (its score stores); sempty: every epilogue thread
+        for (int i = 0; i < nstage; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 8); }
+        mbar_init(s.sfull, 256);
+        mbar_init(s.sempty, 128);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s.tmem_ptr)), "r"(2 * TC_BN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
     }
     // rows: coalesced load of the raw NCHW tile into the swizzled A operand (consecutive threads = consecutive
     // rows of one channel), then one thread per row normalises in place with the canonical chain
@@ -228,14 +160,11 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
         }
         s.zz[tid] = zz;
     }
-    fence_async_smem();            // generic-proxy stores to A -> visible to the async proxy (tcgen05.mma)
-    tc_fence_before();
+    fence_async_smem();            // generic-proxy stores to A -> visible to the async proxy (wgmma)
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *s.tmem_ptr;
     if (trace && threadIdx.x == 0) dbg[1] = clock64();
 
-    if (warp == 0) {
+    if (warp == 12) {
         // ===== TMA producer (whole warp runs the loop, one elected lane issues) =====
         for (int t = 0; t < T; ++t) {
             const int st = t % nstage;
@@ -248,36 +177,44 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
             }
             __syncwarp();
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (whole warp runs the control flow, one elected lane issues) =====
-        const uint32_t idesc = umma_idesc_tf32(TC_BM, TC_BN);
-        const uint32_t a_addr = smem_u32(s.A);
+    } else if (warp < 8) {
+        // ===== MMA warpgroup wg: rows 64 wg .. 64 wg + 63; accumulator -> score tile once the epilogue has read the last one =====
+        const int wg = warp >> 2;
+        const int rq = wg * 64 + (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
+        const uint32_t a_addr = smem_u32(s.A) + wg * 64 * 128;
         for (int t = 0; t < T; ++t) {
-            const int st = t % nstage, as = t & 1;
-            mbar_wait(&s.tempty[as], ((t >> 1) & 1) ^ 1);
-            if (trace && lane == 0 && t < 60) dbg[8 + 4 * t + 0] = clock64();
+            const int st = t % nstage;
             mbar_wait(&s.full[st], (t / nstage) & 1);
-            if (trace && lane == 0 && t < 60) dbg[8 + 4 * t + 1] = clock64();
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t b_addr = smem_u32(s.B + (size_t)st * TC_BN * C);
-                const uint32_t d_tmem = tmem_base + (uint32_t)(as * TC_BN);
-                for (int kc = 0; kc < KC; ++kc) {
+            if (trace && tid == 0 && t < 60) dbg[8 + 4 * t + 1] = clock64();
+            const uint32_t b_addr = smem_u32(s.B + (size_t)st * TC_BN * C);
+            float acc[64];
+            xqtc::wgmma_fence();
 #pragma unroll
-                    for (int k4 = 0; k4 < 4; ++k4) {
-                        uint64_t ad = umma_desc_sw128(a_addr + kc * TC_BM * 128 + k4 * 32);
-                        uint64_t bd = umma_desc_sw128(b_addr + kc * TC_BN * 128 + k4 * 32);
-                        umma_tf32(d_tmem, ad, bd, idesc, (kc | k4) ? 1u : 0u);
-                    }
-                }
-                umma_commit(&s.empty[st]);    // smem stage free once these MMAs retire
-                umma_commit(&s.tfull[as]);    // accumulator ready
+            for (int kc = 0; kc < KC; ++kc) {
+#pragma unroll
+                for (int k4 = 0; k4 < 4; ++k4)
+                    xqtc::wgmma_m64n128k8_tf32(acc, desc_k_sw128(a_addr + kc * TC_BM * 128 + k4 * 32),
+                                               desc_k_sw128(b_addr + kc * TC_BN * 128 + k4 * 32), (kc | k4) ? 1u : 0u);
             }
+            xqtc::wgmma_commit();
+            xqtc::wgmma_wait<0>();
+            xqtc::fence_regs(acc);
             __syncwarp();
-            if (trace && lane == 0 && t < 60) dbg[8 + 4 * t + 2] = clock64();
+            if (lane == 0) mbar_arrive(&s.empty[st]);       // smem stage free
+            if (trace && tid == 0 && t < 60) dbg[8 + 4 * t + 2] = clock64();
+            mbar_wait(s.sempty, (t & 1) ^ 1);               // the epilogue has read the previous tile's scores
+            float *r0 = s.S + (size_t)rq * TC_SLD, *r1 = r0 + 8 * TC_SLD;
+#pragma unroll
+            for (int j = 0; j < TC_BN / 8; ++j) {
+                r0[8 * j + cq] = acc[4 * j];
+                r0[8 * j + cq + 1] = acc[4 * j + 1];
+                r1[8 * j + cq] = acc[4 * j + 2];
+                r1[8 * j + cq + 1] = acc[4 * j + 3];
+            }
+            mbar_arrive(s.sfull);
         }
-    } else {
-        // ===== epilogue: one thread per row (TMEM lane) =====
+    } else if (warp < 12) {
+        // ===== epilogue: one thread per row =====
         const int q = warp & 3;
         const int row = q * 32 + lane;
         float runmax = -CUDART_INF_F, thr = -CUDART_INF_F;
@@ -286,23 +223,18 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
         float *cs2 = s.cand_s2 + row * TC_CAP;
         int *cv = s.cand_v + row * TC_CAP;
         for (int t = 0; t < T; ++t) {
-            const int as = t & 1;
-            mbar_wait(&s.tfull[as], (t >> 1) & 1);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * TC_BN);
+            mbar_wait(s.sfull, t & 1);
             const int vt = t * TC_BN;
-            float v[TC_BN / 32][32];
-#pragma unroll
-            for (int g = 0; g < TC_BN / 32; ++g) tmem_ld32(taddr + g * 32, v[g]);   // issue all loads, wait once
-            tmem_wait_ld();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s.tempty[as]);     // the accumulator stage is free as soon as it is in registers
+            const float *srow = s.S + (size_t)row * TC_SLD;
 #pragma unroll
             for (int g = 0; g < TC_BN / 32; ++g) {
-                float m = v[g][0];
+                float vg[32];
 #pragma unroll
-                for (int j = 1; j < 32; ++j) m = fmaxf(m, v[g][j]);
+                for (int j = 0; j < 32; ++j) vg[j] = srow[g * 32 + j];
+                if (g == TC_BN / 32 - 1) mbar_arrive(s.sempty);   // the score tile is free once its last group is in registers
+                float m = vg[0];
+#pragma unroll
+                for (int j = 1; j < 32; ++j) m = fmaxf(m, vg[j]);
                 if (m >= thr) {          // rare per row (~ln(#groups) times); branch-free, ILP-friendly body
                     const int cbase = vt + g * 32;
                     float m1 = m;
@@ -310,8 +242,8 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
                         m1 = -CUDART_INF_F;
 #pragma unroll
                         for (int j = 0; j < 32; ++j) {
-                            if (cbase + j >= V) v[g][j] = -CUDART_INF_F;
-                            m1 = fmaxf(m1, v[g][j]);
+                            if (cbase + j >= V) vg[j] = -CUDART_INF_F;
+                            m1 = fmaxf(m1, vg[j]);
                         }
                     }
                     if (m1 >= thr) {
@@ -322,14 +254,14 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
                         int na = 0, nb = 0, nc = 0, nd = 0;
 #pragma unroll
                         for (int j = 0; j < 32; j += 4) {
-                            ia = min(ia, v[g][j + 0] == m1 ? j + 0 : 32);
-                            ib = min(ib, v[g][j + 1] == m1 ? j + 1 : 32);
-                            ic = min(ic, v[g][j + 2] == m1 ? j + 2 : 32);
-                            id = min(id, v[g][j + 3] == m1 ? j + 3 : 32);
-                            na += v[g][j + 0] >= lo;
-                            nb += v[g][j + 1] >= lo;
-                            nc += v[g][j + 2] >= lo;
-                            nd += v[g][j + 3] >= lo;
+                            ia = min(ia, vg[j + 0] == m1 ? j + 0 : 32);
+                            ib = min(ib, vg[j + 1] == m1 ? j + 1 : 32);
+                            ic = min(ic, vg[j + 2] == m1 ? j + 2 : 32);
+                            id = min(id, vg[j + 3] == m1 ? j + 3 : 32);
+                            na += vg[j + 0] >= lo;
+                            nb += vg[j + 1] >= lo;
+                            nc += vg[j + 2] >= lo;
+                            nd += vg[j + 3] >= lo;
                         }
                         const int i1 = min(min(ia, ib), min(ic, id));
                         const int nW = (na + nb) + (nc + nd);
@@ -340,9 +272,9 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
                 }
             }
 
-            if (trace && warp == 2 && lane == 0 && t < 60) dbg[8 + 4 * t + 3] = clock64();
+            if (trace && warp == 8 && lane == 0 && t < 60) dbg[8 + 4 * t + 3] = clock64();
         }
-        if (trace && warp == 2 && lane == 0) dbg[2] = clock64();
+        if (trace && warp == 8 && lane == 0) dbg[2] = clock64();
         // exact canonical rescoring, warp-cooperative: for every (row, candidate group) of this warp, lane j
         // scores code j of the group against the row (row values broadcast from smem, the 32 code rows are one
         // contiguous 32*C*4-byte block of En), then a (d, code) lexicographic warp-argmin picks the winner.
@@ -401,15 +333,9 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
             if (lane == r) { best_d = rb_d; best_v = rb_v; }
         }
         s.idx[row] = best_v;
-        if (trace && warp == 2 && lane == 0) dbg[4] = clock64();
+        if (trace && warp == 8 && lane == 0) dbg[4] = clock64();
     }
-    __syncwarp();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * TC_BN));
-    }
     // ---- common epilogue: z_q = normalised code (xqgan_model.py:769-771).  En[v] (prep kernel) holds exactly
     // E[v] / max(|E[v]|, eps) computed with the canonical chain, i.e. the bits the exact kernel recomputes here.
     float sq = 0.f;
@@ -471,22 +397,6 @@ __global__ void finalize_mse_tc_kernel(const float *__restrict__ partial, int n,
     }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                    const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode_fn() {
-    static PFN_encodeTiled fn = nullptr;   // resolved once per process (a function pointer, not kernel state)
-    if (!fn) {
-        void *p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = (PFN_encodeTiled)p;
-    }
-    return fn;
-}
-
 size_t vq_tc_workspace_bytes(int B, int C, int HW, int V) {
     size_t Vp = ((size_t)V + TC_BN - 1) / TC_BN * TC_BN;
     size_t ctas = ((size_t)B * HW + TC_BM - 1) / TC_BM;
@@ -503,7 +413,7 @@ int vq_tc_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     if (!vq_tc_supported(C, V, 1)) return XQ_ERR_UNSUPPORTED;
     if (workspace_bytes < vq_tc_workspace_bytes(B, C, HW, V)) return XQ_ERR_WORKSPACE;
     if (((uintptr_t)workspace & 127) != 0) return XQ_ERR_UNSUPPORTED;   // TMA global address alignment
-    PFN_encodeTiled enc = get_encode_fn();
+    xqtc::PFN_encodeTiled enc = xqtc::get_encode_fn();
     if (!enc) return XQ_ERR_UNSUPPORTED;
     const int Vp = (V + TC_BN - 1) / TC_BN * TC_BN;
     const int N = B * HW;
@@ -545,11 +455,12 @@ int vq_tc_forward(const float *z, const float *E, int B, int C, int HW, int V, i
 
     codebook_prep_rowmajor_kernel<<<(Vp + 127) / 128, 128, 0, stream>>>(E, V, C, Vp, En, ee);
     XQ_LAUNCH_CHECK("codebook_prep_rowmajor_kernel");
-    XQ_CUDA_TRY(cudaFuncSetAttribute(vq_search_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int ctas = (N + TC_BM - 1) / TC_BM;
     long long *dbg = g_vq_tc_trace;          // nullptr unless a development build set it (xq_dev_set_vq_trace, -DXQ_VQ_TC_TRACE)
-    vq_search_tc_kernel<<<ctas, TC_THREADS, smem, stream>>>(tm, z, E, En, ee, N, C, HW, V, Vp, nstage, ste_value, idx, out,
-                                                           loss ? partial : nullptr, hist, dbg);
+    auto kern = C == 32 ? vq_search_tc_kernel<1> : vq_search_tc_kernel<2>;
+    XQ_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<ctas, TC_THREADS, smem, stream>>>(tm, z, E, En, ee, N, C, HW, V, Vp, nstage, ste_value, idx, out,
+                                             loss ? partial : nullptr, hist, dbg);
     XQ_LAUNCH_CHECK("vq_search_tc_kernel");
     if (loss) {
         finalize_mse_tc_kernel<<<1, 32, 0, stream>>>(partial, ctas, 1.0 / ((double)N * (double)C), beta, loss);

@@ -1,4 +1,4 @@
-// xq_common.cuh -- shared device helpers for libxqb200 (sm_100a only).
+// xq_common.cuh -- shared device helpers for libxqb200 (sm_90a).
 //
 // CANONICAL ARITHMETIC (DESIGN.md): every value that feeds an index decision is IEEE fp32,
 // round-to-nearest, fixed operation order, fused multiply-add only where written as fmaf().

@@ -40,54 +40,4 @@ __device__ __forceinline__ float dgelu_f(float x) {
     return fmaf(x * 0.3989422804014327f, e, 0.5f + copysignf(half, x));
 }
 
-
-// ---- two elements per instruction: Blackwell executes packed fp32 pairs (FFMA2 / FMUL2 / FADD2).  The fused GEMM epilogues are
-// bound by instruction issue, so they use these; every lane performs exactly the operation sequence of the scalar functions above
-// (same fma / mul / add, same order, IEEE rounding per lane), i.e. the same bits.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) { f32x2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void up2(f32x2 v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { f32x2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 dup2(float c) { return pk2(c, c); }
-
-// (gelu_f(x0), gelu_f(x1))
-__device__ __forceinline__ f32x2 gelu_f2(float x0, float x1) {
-    const f32x2 A = pk2(fabsf(x0), fabsf(x1));
-    f32x2 P = fma2(A, dup2(5.382975000e-06f), dup2(4.889063564e-05f));
-    P = fma2(P, A, dup2(3.800357500e-05f));
-    P = fma2(P, A, dup2(3.277626324e-03f));
-    P = fma2(P, A, dup2(2.114100615e-02f));
-    P = fma2(P, A, dup2(4.986734697e-02f));
-    P = fma2(P, A, dup2(1.0f));
-    P = mul2(P, P); P = mul2(P, P); P = mul2(P, P); P = mul2(P, P);
-    float p0, p1, h0, h1;
-    up2(P, p0, p1);
-    const f32x2 H = mul2(dup2(0.5f), pk2(x0, x1));
-    up2(H, h0, h1);
-    const f32x2 AH = pk2(fabsf(h0), fabsf(h1));
-    // -|h| * r + (h + |h|)  ==  |h| * rcp(-p) + (h + |h|): the reciprocal is odd, the product's sign symmetric
-    return fma2(AH, pk2(rcp_fast(-p0), rcp_fast(-p1)), add2(H, AH));
-}
-// (dgelu_f(x0), dgelu_f(x1))
-__device__ __forceinline__ f32x2 dgelu_f2(float x0, float x1) {
-    const f32x2 X = pk2(x0, x1);
-    float u0, u1;
-    up2(fma2(pk2(fabsf(x0), fabsf(x1)), dup2(0.23164189f), dup2(1.0f)), u0, u1);
-    const f32x2 T = pk2(rcp_fast(u0), rcp_fast(u1));
-    f32x2 Q = fma2(T, dup2(1.061405429f), dup2(-1.453152027f));
-    Q = fma2(Q, T, dup2(1.421413741f));
-    Q = fma2(Q, T, dup2(-0.284496736f));
-    Q = fma2(Q, T, dup2(0.254829592f));
-    float s0, s1;
-    up2(mul2(mul2(X, X), dup2(-0.72134752044448170f)), s0, s1);
-    const f32x2 E = pk2(ex2_fast(s0), ex2_fast(s1));
-    const f32x2 PE = mul2(mul2(Q, T), E);
-    float hf0, hf1;
-    up2(fma2(dup2(-0.5f), PE, dup2(0.5f)), hf0, hf1);
-    const f32x2 S = add2(dup2(0.5f), pk2(copysignf(hf0, x0), copysignf(hf1, x1)));
-    return fma2(mul2(X, dup2(0.3989422804014327f)), E, S);
-}
-
 }  // namespace xqv

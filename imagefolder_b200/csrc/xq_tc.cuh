@@ -1,13 +1,15 @@
-// xq_tc.cuh -- PTX wrappers for the bf16 tcgen05 / TMEM / TMA kernels of libxqb200 (sm_100a only).
+// xq_tc.cuh -- PTX wrappers for the bf16 / tf32 wgmma + TMA + mbarrier kernels of libxqb200 (sm_90a).
 //
-// Shared-memory operand layouts used by the attention kernels (all SWIZZLE_128B, 1024-byte aligned tiles):
+// Shared-memory operand layouts used by the attention and GEMM kernels (all SWIZZLE_128B, 1024-byte aligned tiles):
 //   "row tile"  [R rows][64 bf16]  = what one TMA box {64, R, 1} of a [.., rows, 64*k] tensor lands as:
 //               byte(r, c) = r*128 + (((c >> 3) ^ (r & 7)) << 4) + (c & 7)*2
 //     * as a K-major operand   (MMA K runs along the 64 columns): rows are M (or N), descriptor SBO = 1024
 //     * as an MN-major operand (MMA K runs along the ROWS, M/N along the 64 columns): 8 rows = one swizzle atom,
-//       SBO = 1024 (next 8 K), LBO = distance to the next 64 M/N elements (a second row tile)
-// Descriptor field meanings follow the sm_100 shared-memory matrix descriptor (start >> 4, LBO >> 4 at bit 16,
-// SBO >> 4 at bit 32, version 1 at bit 46, layout type at bit 61; SWIZZLE_128B = 2).
+//       SBO = 1024 (next 8 K), LBO = distance to the next 64 M/N elements (unused: every MN-major operand here is 64 wide)
+// Descriptor fields follow the sm_90 wgmma shared-memory matrix descriptor (start >> 4, LBO >> 4 at bit 16, SBO >> 4 at
+// bit 32, layout type at bit 62; SWIZZLE_128B = 1).
+// Accumulator fragment of wgmma.m64nN (per warpgroup, warp w = warp % 4, lane l): d[4j + e] holds row 16w + l/4 (+8 for
+// e >= 2), column 8j + 2(l%4) + (e & 1).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -84,150 +86,84 @@ template <int N>
 __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ---- fences ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- TMEM allocation (one warp, power-of-two columns >= 32) -------------------------------------------------
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_holder) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "n"(COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS));
-}
-
-// ---- descriptors ------------------------------------------------------------------------------------------
-// K-major SWIZZLE_128B operand: rows 128 B apart, 8-row atoms 1024 B apart
+// ---- wgmma ------------------------------------------------------------------------------------------------
+// K-major SWIZZLE_128B operand: rows 128 B apart, 8-row atoms 1024 B apart; the K offset inside the 128-byte row is added to
+// the start address (desc_adv)
 __device__ __forceinline__ uint64_t desc_k_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)1 << 16;                 // LBO: unused for a swizzled K-major operand one atom wide
     d |= (uint64_t)(1024 >> 4) << 32;       // SBO
-    d |= (uint64_t)1 << 46;                 // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                 // SWIZZLE_128B
     return d;
 }
-// MN-major SWIZZLE_128B operand: 64 M/N elements per 128-byte row, 8 K-rows per atom (SBO), next 64 M/N at LBO
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// MN-major SWIZZLE_128B operand: 64 M/N elements per 128-byte row, 8 K-rows per atom (SBO = 1024), the next 64 M/N at LBO
+__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// instruction descriptor, kind::f16: D = F32, A = B = BF16
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// advance a shared-memory matrix descriptor by `bytes` (start-address field is in 16-byte units; never carries out of it)
+__device__ __forceinline__ uint64_t desc_adv(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins accumulator registers in program order around wgmma_wait: without it the compiler may move reads of an accumulator
+// above the wait that makes it valid
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- MMA ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
+// D[64 x 64] (+)= A[64 x 16] B[16 x 64], A and B from shared memory (descriptors); TA / TB: operand is MN-major
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-// A operand from TMEM (lane = M row, 2 bf16 per 32-bit column, K-major)
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
 
-// ---- TMEM <-> registers (32 lanes x 32-bit, N consecutive columns per thread) ----------------------------
-#define XQTC_R8(r, o) "=r"(r[o + 0]), "=r"(r[o + 1]), "=r"(r[o + 2]), "=r"(r[o + 3]), "=r"(r[o + 4]), "=r"(r[o + 5]), "=r"(r[o + 6]), "=r"(r[o + 7])
-#define XQTC_I8(r, o) "r"(r[o + 0]), "r"(r[o + 1]), "r"(r[o + 2]), "r"(r[o + 3]), "r"(r[o + 4]), "r"(r[o + 5]), "r"(r[o + 6]), "r"(r[o + 7])
+// D[64 x 128] (+)= A[64 x 16] B[16 x 128], A and B from shared memory (descriptors); TA / TB: operand is MN-major
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// D[64 x 64] (+)= A[64 x 16] B[16 x 64], A from registers (accumulator fragment layout, bf16 pairs), B from shared memory
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : XQTC_R8(r, 0), XQTC_R8(r, 8), XQTC_R8(r, 16), XQTC_R8(r, 24)
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : XQTC_R8(r, 0), XQTC_R8(r, 8)
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : XQTC_R8(r, 0)
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-        ::XQTC_I8(r, 0), XQTC_I8(r, 8), XQTC_I8(r, 16), XQTC_I8(r, 24), "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-        ::XQTC_I8(r, 0), XQTC_I8(r, 8), "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// ---- explicit shared-memory accesses (pointers derived from the aligned dynamic-smem base are GENERIC to the compiler:
-// without these it emits ST.E / LD.E generic instructions instead of STS / LDS) ------------------------------------
-// ---- CTA pair (cta_group::2): two CTAs of a 2-cluster (same TPC) issue ONE MMA with M = 256 (128 accumulator rows in each
-// CTA's TMEM) and N <= 256 (each CTA stages half of the B tile).  PTX forms as in the vendored CUTLASS headers
-// (cute/arch/copy_sm100_tma.hpp, cutlass/arch/barrier.h, cute/arch/tmem_allocator_sm100.hpp); verified on hardware by
-// tools/gemm_probe.cu (bit-identical to cuBLAS at 131328 x 3072 x 768).
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// executed by BOTH CTAs: the bytes land in the executing CTA's shared memory and complete on the LEADER's (rank 0) barrier --
-// the mbarrier address with the pair's peer bit cleared
-__device__ __forceinline__ void tma_load_3d_2sm(void *dst, const CUtensorMap *map, int c0, int c1, int c2, uint64_t *leader_bar) {
-    asm volatile("cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(leader_bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cta(uint64_t *bar, uint32_t cta) {       // arrive on `bar` of cluster CTA `cta`
-    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-                 ::"r"(smem_u32(bar)), "r"(cta) : "memory");
-}
-__device__ __forceinline__ void umma_ss2(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void umma_commit2(uint64_t *bar) {                         // arrives on `bar` in BOTH CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc2(uint32_t *smem_holder) {                  // same warp id in both CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "r"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(COLS) : "memory");
+// D[64 x 128] (+)= A[64 x 8] B[8 x 128], TF32 operands (both K-major) from shared memory
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(acc));
 }
 
 __device__ __forceinline__ void sts128(uint32_t saddr, uint4 v) {
@@ -238,13 +174,9 @@ __device__ __forceinline__ float4 lds128f(uint32_t saddr) {
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr) : "memory");
     return v;
 }
-// advance a shared-memory matrix descriptor by `bytes` (start-address field is in 16-byte units; never carries out of it)
-__device__ __forceinline__ uint64_t desc_adv(uint64_t d, uint32_t bytes) { return d + (uint64_t)(bytes >> 4); }
 
-// one lane of a CONVERGED warp.  The single-thread tcgen05 / TMA instructions take uniform-register operands: issued
-// under `if (lane == 0)` (a divergent region) the compiler wraps each one in an ELECT / BRA.U.ANY serialisation loop,
-// measured at ~112 clk per tcgen05.mma whatever its shape; issued under elect.sync by a warp that runs the surrounding
-// control flow uniformly they are plain predicated instructions (64 clk for M128 N128 K16 = the tensor-pipe rate).
+// one lane of a CONVERGED warp, for the single-thread TMA / mbarrier instructions of a warp that runs the surrounding
+// control flow uniformly
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));

@@ -12,7 +12,7 @@ Parameter names (= checkpoint keys) are identical to timm's: patch_embed.proj, c
 pos_embed, blocks.{i}.{norm1,attn.qkv,attn.proj,ls1.gamma,norm2,mlp.fc1,mlp.fc2,ls2.gamma}, norm.
 
 GEMMs run on cuBLAS and attention on the fused SDPA library kernel (plain library calls); the
-elementwise / normalisation glue is what imagefolder_b200.vit_ops replaces with sm_100a kernels.
+elementwise / normalisation glue is what imagefolder_b200.vit_ops replaces with sm_90a kernels.
 """
 from __future__ import annotations
 

@@ -3,7 +3,7 @@
 `run_blocks(vit, x)` walks `vit.blocks` + `vit.norm` exactly like the reference
 (dino_enc/dinov2.py:183-190 -> vision_transformer.py:336-339) but replaces every chain
    [+ residual] -> LayerScale -> DropPath -> add -> LayerNorm -> cast-to-bf16
-by ONE kernel (`xq_vit_residual_ln_fwd`), GELU by one bf16 kernel and attention by the tcgen05 / TMEM / TMA flash
+by ONE kernel (`xq_vit_residual_ln_fwd`), GELU by one bf16 kernel and attention by the wgmma / TMA flash
 kernels of csrc/attn_kernel.cu (`xq_vit_attn_fwd/bwd`, reading the packed qkv projection in place and writing d(qkv)
 in the packed layout); the projection GEMMs stay on cuBLAS.  Attention dropout > 0 (no shipped config) and head
 dims other than 64 use the SDPA library kernel.  The residual stream is fp32 and the GEMM operands bf16,
@@ -120,7 +120,7 @@ def gelu_bias(x, bias=None):
     return _GeluBias.apply(x, bias)
 
 
-MLP_TC_ENABLED = [True]       # the tcgen05 GEMMs with fused GELU / GELU' epilogues (csrc/gemm_kernel.cu)
+MLP_TC_ENABLED = [True]       # the wgmma GEMMs with fused GELU / GELU' epilogues (csrc/gemm_kernel.cu)
 
 
 def mlp_tc_ok(y, fc1, fc2) -> bool:
@@ -181,7 +181,7 @@ class _FusedMLP(torch.autograd.Function):
 
 
 def mlp_forward(mlp, y):
-    """timm Mlp (fc1 -> GELU -> fc2, drop = 0) without the fc2 bias; fused tcgen05 path when the shapes allow, else library GEMMs +
+    """timm Mlp (fc1 -> GELU -> fc2, drop = 0) without the fc2 bias; fused wgmma path when the shapes allow, else library GEMMs +
     the stand-alone bias / GELU kernel."""
     if mlp_tc_ok(y, mlp.fc1, mlp.fc2):
         return _FusedMLP.apply(y, mlp.fc1.weight, mlp.fc1.bias, mlp.fc2.weight)
@@ -189,7 +189,7 @@ def mlp_forward(mlp, y):
     return F.linear(h, mlp.fc2.weight)
 
 
-ATTN_TC_ENABLED = [True]      # the tcgen05 attention kernels (csrc/attn_kernel.cu); tools flip it to time the library path
+ATTN_TC_ENABLED = [True]      # the wgmma attention kernels (csrc/attn_kernel.cu); tools flip it to time the library path
 
 
 def attn_tc_ok(qkv, num_heads: int, dropout_p: float) -> bool:

@@ -1,5 +1,5 @@
 /*
- * xqb200.h -- C ABI of libxqb200.so: the B200 (sm_100a) quantizer hot path of the XQ-GAN /
+ * xqb200.h -- C ABI of libxqb200.so: the H100 (sm_90a) quantizer hot path of the XQ-GAN /
  * ImageFolder image tokenizer.
  *
  * The reference (lxa9867/ImageFolder) is pure Python; its "operator boundary" for this path is
@@ -240,7 +240,7 @@ int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, 
 
 /*   Flash attention of the ViT blocks, head_dim 64, no mask, no dropout (Attention.forward,
  *   tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197: F.scaled_dot_product_attention on
- *   qkv.reshape(B,N,3,H,hd).permute(2,0,3,1,4), then x.transpose(1,2).reshape(B,N,C)).  tcgen05 / TMEM / TMA kernel.
+ *   qkv.reshape(B,N,3,H,hd).permute(2,0,3,1,4), then x.transpose(1,2).reshape(B,N,C)).  wgmma / TMA kernel.
  *     qkv   bf16 [B,N,3,H,64]  the packed projection, read in place (no q/k/v copies)
  *     out   bf16 [B,N,H*64]    head-merged attention output (what `proj` consumes)
  *     lse2  fp32 [B,H,N]       base-2 log-sum-exp of the scaled scores (scale*log2(e)*q.k), saved for backward
@@ -249,7 +249,7 @@ int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
 
 /*   Backward of xq_vit_attn_fwd: d_out bf16 [B,N,H*64] -> dqkv bf16 [B,N,3,H,64] (the gradient of the packed projection,
  *   written in place of autograd's three permuted tensors + stack).  `out` and `lse2` are the forward's results.
- *   workspace (256-byte aligned, xq_vit_attn_bwd_workspace_bytes): fp32 dQ accumulator [B*H,N,64] (TMA reduce-add across
+ *   workspace (256-byte aligned, xq_vit_attn_bwd_workspace_bytes): fp32 dQ accumulator [B*H,N,64] (atomic adds across
  *   the key blocks) + the padded statistics.  g_bias fp32 [3*H*64] (may be NULL) receives the column sums of dqkv = the
  *   gradient of the qkv bias (nn.Linear's backward `sum(0)` pass, fused into the epilogues).  3 launches + memsets. */
 size_t xq_vit_attn_bwd_workspace_bytes(int B, int N, int H);
@@ -282,12 +282,13 @@ int xq_diffaug_forward(const float *x, const float *rand01, int B, int C, int H,
 int xq_diffaug_backward(const float *g, const float *rand01, int B, int C, int H, int W, int flags, int cut_h, int cut_w,
                         float *gx, float *sums, void *stream);
 
-/* ---- ViT MLP with the element-wise work fused into a hand-written tcgen05 GEMM (csrc/gemm_kernel.cu) --------------------
+/* ---- ViT MLP with the element-wise work fused into a hand-written wgmma GEMM (csrc/gemm_kernel.cu) ----------------------
  * Replaces, inside timm's Mlp as called by Block.forward (tokenizer/tokenizer_image/dino_enc/vision_transformer.py:336-339):
  *   forward   F.linear(y, W1) [cuBLAS] + GELU(. + b1) [xq_vit_gelu_fwd]            -> xq_vit_fc1_gelu_fwd
  *   backward  d_act = d_out W2 [cuBLAS] + d_act * GELU'(pre + b1), d_b1 [xq_vit_gelu_bwd] -> xq_vit_fc2_dgelu_bwd
- * All matrices row-major bf16; bias / d_bias fp32.  N % 256 == 0, K % 64 == 0 (else XQ_ERR_UNSUPPORTED: the caller keeps the
- * library GEMM + stand-alone kernel), any M.  Results are bit-identical to that two-call sequence.
+ * All matrices row-major bf16; bias / d_bias fp32.  N % 128 == 0, N / 128 <= SM count, K % 64 == 0 (else XQ_ERR_UNSUPPORTED),
+ * any M.  pre / act / d_pre apply the same device functions to the same rounded bf16 GEMM results as that two-call sequence
+ * (equal up to the GEMM's fp32 accumulation order); d_bias is summed with fp32 atomics, in no fixed order.
  *   x [M,K], w [N,K] (fc1.weight as bf16)  ->  pre [M,N] = x w^T ,  act [M,N] = GELU(pre + bias)                               */
 int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream);
 /*  d_out [M,K] (gradient of the fc2 output), w2t [N,K] (fc2.weight TRANSPOSED, bf16), pre [M,N] (saved by the forward)

@@ -3,7 +3,7 @@
     python oracle/build.py        -> oracle/libxq_oracle.so
 
 Flags: -ffp-contract=off so that only the fmaf() calls written in the source fuse
-(canonical arithmetic); -mfma -mavx2 (x86-64-v3, present on every B200 host CPU) so fmaf
+(canonical arithmetic); -mfma -mavx2 (x86-64-v3, present on every current x86 GPU host) so fmaf
 is a single instruction; OpenMP for the row-parallel loops.  The reference is pure Python,
 so there is no `oracle/_ref` to compile (DESIGN.md "Oracle").
 """

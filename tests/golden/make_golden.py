@@ -2,8 +2,8 @@
 
     python tests/golden/make_golden.py            # writes tests/golden/*.npz
 
-Runs only in the build container, where /root/reference exists (it does not exist on the
-GPU box; tests read the committed .npz files).  The reference ships no tests or golden
+Needs a checkout of the reference, named by the XQ_REFERENCE environment variable (the tests only
+read the committed .npz / .json files).  The reference ships no tests or golden
 vectors (SURVEY.md section 4), so these files are what pins the oracle -- and through it the
 CUDA path -- to the reference's behaviour.  Recipe: SURVEY.md section 8c (stub timm / peft /
 webdataset, 1-rank gloo group).
@@ -16,7 +16,7 @@ import numpy as np
 import torch
 import torch.distributed as tdist
 
-REF = os.environ.get("XQ_REFERENCE", "/root/reference")
+REF = os.environ.get("XQ_REFERENCE", "")    # a checkout of lxa9867/ImageFolder (the reference)
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -390,7 +390,29 @@ def main_round2():
     case_vq2_unscreened(VQ2, "msvr_unscreened")
 
 
+def write_config_golden():
+    """reference_configs.json: the values of the reference's configs/*.yaml that config.SHIPPED_CONFIGS restates"""
+    import glob
+    import json
+
+    import yaml
+    sys.path.insert(0, os.path.dirname(os.path.dirname(OUT)))
+    from imagefolder_b200 import config as xcfg
+    out = {}
+    for f in sorted(glob.glob(os.path.join(REF, "configs", "*.yaml"))):
+        y = yaml.safe_load(open(f))
+        name = os.path.basename(f)[:-5]
+        out[name] = {k: y[k] for k in xcfg.SHIPPED_CONFIGS.get(name, y) if k in y}
+    with open(os.path.join(OUT, "reference_configs.json"), "w") as fh:
+        fh.write("{\n" + ",\n".join(f"{json.dumps(k)}: {json.dumps(v, sort_keys=True)}" for k, v in sorted(out.items())) + "\n}\n")
+
+
 def main():
+    if not os.path.isdir(REF):
+        raise SystemExit("set XQ_REFERENCE to a checkout of the reference (lxa9867/ImageFolder)")
+    if "--configs-only" in sys.argv:
+        write_config_golden()
+        return
     if "--round2-only" in sys.argv:
         main_round2()
         return

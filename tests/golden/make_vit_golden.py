@@ -28,7 +28,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 from vit_det_init import apply_det_init, golden_inputs  # noqa: E402
 
-REF = os.environ.get("XQ_REFERENCE", "/root/reference")
+REF = os.environ.get("XQ_REFERENCE", "")    # a checkout of lxa9867/ImageFolder (the reference)
 
 
 # ---- functional stand-ins for timm (test infrastructure) -----------------------------------------------------------

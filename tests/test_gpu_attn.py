@@ -1,4 +1,4 @@
-"""tcgen05 flash attention (csrc/attn_kernel.cu, xq_vit_attn_fwd / xq_vit_attn_bwd through the C-ABI) against a plain
+"""wgmma flash attention (csrc/attn_kernel.cu, xq_vit_attn_fwd / xq_vit_attn_bwd through the C-ABI) against a plain
 PyTorch fp32 explicit-softmax reference of the same op: Attention.forward,
 tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197 (softmax(q k^T / sqrt(d)) v on the packed projection).
 
@@ -58,7 +58,7 @@ def test_attention_forward_backward_match_fp32_reference(B, N, H, amp):
 
 
 def test_attention_autograd_node_uses_the_tc_kernels_and_matches_sdpa():
-    """The autograd node the ViT blocks call (_QKVAttention) on the tcgen05 path vs the same node on the SDPA library path."""
+    """The autograd node the ViT blocks call (_QKVAttention) on the wgmma path vs the same node on the SDPA library path."""
     from imagefolder_b200 import _capi, vit_ops
     torch.manual_seed(0)
     dev = torch.device("cuda")

@@ -442,7 +442,7 @@ def test_msbr_full_size_properties():
 
 
 # ------------------------------------------------------------------------------------------
-# tcgen05 screening + exact rescoring == exact CUDA-core kernel == oracle (bit for bit)
+# TF32 wgmma screening + exact rescoring == exact CUDA-core kernel == oracle (bit for bit)
 # ------------------------------------------------------------------------------------------
 def _run_vq_algo(algo, z, E):
     import os
@@ -465,6 +465,8 @@ def _run_vq_algo(algo, z, E):
                                            (3, 32, 7, 300, "dup"), (64, 32, 16, 8192, "ref"), (256, 32, 16, 8192, "randn"),
                                            (128, 64, 16, 4096, "randn"), (128, 32, 16, 16384, "ref")])
 def test_vq_tcgen05_path_is_bit_identical(B, C, hw, V, init):
+    """The tensor-core search (TF32 wgmma screening + exact rescoring; the name predates the sm_90a port) against the exact
+    CUDA-core kernel and the oracle, bit for bit."""
     torch.manual_seed(B * 7 + V)
     z = torch.randn(B, C, hw, hw, device="cuda")
     if init == "ref":
@@ -581,7 +583,7 @@ def test_var_helpers_consistent_with_token_decode_and_errors():
 @pytest.mark.parametrize("name", ["vq8192_c32", "vq16384_c32"])
 def test_vq_baseline_shaped_reference_goldens(name):
     """V = 8192 / 16384, C = 32 (BASELINE configs #2 / #3): indices bit-exact against the REFERENCE's own output
-    (tests/golden/make_golden.py --round2-only), on both the tcgen05 path and the exact CUDA-core path."""
+    (tests/golden/make_golden.py --round2-only), on both the tensor-core path and the exact CUDA-core path."""
     import os
     from test_oracle_golden import big_vq_inputs
     g = load_golden(name)

@@ -297,7 +297,7 @@ def test_assemble_cabi_exact():
 
 @pytest.mark.parametrize("M,C,Hd", [(2 * 513, 384, 1536), (4 * 513, 768, 3072), (131, 768, 3072), (3 * 256, 384, 1536)])
 def test_fused_mlp_gemm_epilogues_equal_library_gemm_plus_gelu_kernels(M, C, Hd):
-    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd (tcgen05 cta_group::2 GEMMs with GELU / GELU' + bias-gradient epilogues) against the
+    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd (wgmma GEMMs with GELU / GELU' + bias-gradient epilogues) against the
     path they replace -- library GEMM + the stand-alone bias / GELU kernels -- for timm Mlp inside Block.forward
     (dino_enc/vision_transformer.py:336-339).  The epilogues apply the same device functions to the same rounded bf16 values, so the
     results agree to the last bit up to the accumulation order of the GEMMs (checked at bf16 resolution)."""

@@ -78,16 +78,16 @@ def test_yaml_contract(tmp_path):
     assert abs(al - 0.75) < 1e-12 and de == 75
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/configs"), reason="reference tree not present")
-def test_shipped_config_table_matches_reference_yamls():
-    import glob
-    files = sorted(glob.glob("/root/reference/configs/*.yaml"))
-    assert {os.path.basename(f)[:-5] for f in files} == set(xcfg.SHIPPED_CONFIGS)
-    for f in files:
-        y = yaml.safe_load(open(f))
-        for k, v in xcfg.SHIPPED_CONFIGS[os.path.basename(f)[:-5]].items():
+def test_shipped_config_table_matches_reference_yamls(golden_dir):
+    """against the values of the reference's configs/*.yaml, stored by tests/golden/make_golden.py --configs-only"""
+    import json
+    with open(os.path.join(golden_dir, "reference_configs.json")) as f:
+        ref_cfgs = json.load(f)
+    assert set(ref_cfgs) == set(xcfg.SHIPPED_CONFIGS)
+    for name, y in ref_cfgs.items():
+        for k, v in xcfg.SHIPPED_CONFIGS[name].items():
             ref = float(y[k]) if k == "lr" else y[k]
-            assert ref == v, (f, k)
+            assert ref == v, (name, k)
 
 
 def test_model_variants_build():

@@ -4,7 +4,7 @@ decode; only timm's PatchEmbed / Mlp / DropPath / resample_abs_pos_embed are sta
 
 CPU (fp32, tolerance 1e-3 relative as the north star states -- observed ~1e-5): the product's modules and the oracle
 restatement (oracle/vit_ref.py) both have to reproduce the reference's numbers from the same name-seeded weights.
-GPU: the fused bf16 path (libxqb200 glue + tcgen05 attention) against the same goldens at bf16 tolerance."""
+GPU: the fused bf16 path (libxqb200 glue + wgmma attention) against the same goldens at bf16 tolerance."""
 import ast
 import os
 import sys
@@ -79,7 +79,7 @@ def test_oracle_vit_matches_reference_golden(name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CASES)
 def test_fused_cuda_vit_matches_reference_golden(name):
-    """bf16 autocast through the fused path (residual+LN / GELU glue kernels, tcgen05 attention, library GEMMs).
+    """bf16 autocast through the fused path (residual+LN / GELU glue kernels, wgmma attention, library GEMMs).
     Tolerance: bf16 GEMM operands over 12 blocks -> a few 1e-2 absolute on O(1) activations."""
     g, cfg = load_case(name)
     model = build_ours(cfg).cuda()

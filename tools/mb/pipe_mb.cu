@@ -1,5 +1,5 @@
-// pipe_mb.cu -- dev tool: per-SM throughput of the instructions the attention softmax is made of (B200).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/mb/pipe_mb tools/mb/pipe_mb.cu
+// pipe_mb.cu -- dev tool: per-SM throughput of the instructions the attention softmax is made of (H100).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/mb/pipe_mb tools/mb/pipe_mb.cu
 #include <cstdio>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

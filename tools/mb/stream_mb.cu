@@ -1,5 +1,5 @@
 // dev microbenchmark: which streaming skeleton reaches HBM peak for the row-major bf16 glue kernels?
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/mb/stream_mb tools/mb/stream_mb.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/mb/stream_mb tools/mb/stream_mb.cu
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cstdio>

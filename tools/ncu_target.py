@@ -1,5 +1,5 @@
 """dev tool: one launch set of a hot kernel at its bench shape, for `ncu --set full` captures (profiles/README.md):
-     python tools/ncu_target.py attn [B N H]      tcgen05 attention forward + backward     (default 256 513 12 = VQ-8192, B=256)
+     python tools/ncu_target.py attn [B N H]      wgmma attention forward + backward       (default 256 513 12 = VQ-8192, B=256)
      python tools/ncu_target.py vq   [B V C]      single-scale search, 16x16 tokens/image  (default 256 8192 32)
      python tools/ncu_target.py ms   [B V]        MSVR10P2 fused 10-scale kernel, training  (default 128 4096)"""
 import os
