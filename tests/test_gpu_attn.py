@@ -4,7 +4,8 @@ tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197 (softmax(q k^T 
 
 Tolerances (bf16 operands and bf16 P / dS inside the kernel, fp32 statistics and accumulation): forward 8e-3, gradients
 1e-2, both relative to the largest reference magnitude of the tensor.  Sequence lengths are the ones the shipped
-configs produce (513 / 514 VQ, 769 VP2, 499 / 379 multi-scale) plus edge cases (1, 16, 128, 129, 1024)."""
+configs produce (513 / 514 VQ, 769 VP2, 499 / 379 multi-scale) plus edge cases (1, 16, 128, 129, 1024) and every
+trailing-key count of the backward pre-pass (N mod 128 = 1 .. 4, and 5, which goes back to the tensor cores)."""
 import math
 
 import pytest
@@ -24,9 +25,13 @@ def _ref(qkv32, H):
 
 @pytest.mark.parametrize("B,N,H", [(2, 513, 3), (2, 514, 2), (1, 769, 2), (2, 499, 2), (2, 379, 3), (3, 1, 1), (1, 16, 2),
                                    (2, 128, 2), (2, 129, 1), (1, 1024, 1), (1, 333, 12),
-                                   # more (batch*head, key block) items than SMs: every CTA of the persistent backward walks
-                                   # several items (K / V prefetch into the other buffer, epilogue pipelined into the next item)
-                                   (5, 513, 12), (7, 300, 12), (40, 130, 12), (13, 100, 12)])
+                                   # more backward CTAs (one per key block and batch*head) than SMs: several waves, and the
+                                   # fp32 dQ atomics of one (batch, head) come from CTAs of different waves
+                                   (5, 513, 12), (7, 300, 12), (40, 130, 12), (13, 100, 12),
+                                   # N mod 128 = 3 / 4: the trailing keys on CUDA cores in the backward pre-pass
+                                   # (attn_bwd_prep_kernel<3> / <4>); N mod 128 = 5: the first length that goes back to a
+                                   # tensor-core key block for them
+                                   (2, 131, 2), (1, 132, 12), (2, 133, 3), (1, 387, 12), (2, 388, 2)])
 @pytest.mark.parametrize("amp", [1.0, 2.5])
 def test_attention_forward_backward_match_fp32_reference(B, N, H, amp):
     from imagefolder_b200 import vit_ops

@@ -1,11 +1,35 @@
-"""Numerics of the ViT glue kernels against a plain PyTorch fp32 reference of the same op
-(floating-point kernels: tolerance set by the bf16 operands, written per assertion)."""
+"""Numerics of the ViT glue kernels against a plain PyTorch fp32 / fp64 reference of the same op
+(floating-point kernels: tolerance set by the bf16 operands, written per assertion).
+
+The persistent kernels (residual_ln_bwd, pack_qkv, gelu_bwd) hand out row tiles dynamically, so they are also run at row
+counts where every CTA takes several tiles (the training encoder has 128 x 513 rows), through the C ABI with every output
+buffer NaN-filled first: a tile that is never written fails, and column sums of integer-valued inputs are exact in fp32
+in any order, so they are compared by equality and a tile counted twice fails too."""
+import math
+
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
+
+TRAIN_ROWS = 128 * 513          # encoder rows at a per-GPU batch of 128: cls + 256 image + 256 latent tokens per sample
+
+
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _nan(shape, dtype=torch.float32):
+    return torch.full(shape, float("nan"), dtype=dtype, device="cuda")
+
+
+def _assert_within(a, ref, tol, what):
+    """|a - ref| <= tol elementwise (tol broadcasts against ref); a NaN in `a` (an output never written) fails."""
+    err = (a.double() - ref).abs()
+    ok = err <= tol
+    assert bool(ok.all()), f"{what}: {int((~ok).sum())} of {ok.numel()} elements out of tolerance, max err {err.max().item():.3e}"
 
 
 def ref_residual_ln(x, branch, gamma, rs, w, b, eps, S, bbias=None):
@@ -77,6 +101,107 @@ def test_residual_ln_none_grads():
     np.testing.assert_allclose(x.grad.cpu().numpy(), x2.grad.float().cpu().numpy(), rtol=1e-4, atol=1e-4 * float(x2.grad.abs().max()))
 
 
+def _ln_bwd_stages(D):
+    # residual_ln_bwd_kernel's ring: 3 stages of 8 rows (x_out, g_xout fp32; g_y, branch bf16; 128 B of row stats) when
+    # they fit in 225 KiB of shared memory, else 2 (D = 1024)
+    return 3 if 3 * (8 * D * 12 + 128) <= 225 * 1024 else 2
+
+
+# (D, row count).  The backward hands out 8-row tiles: CTA i takes tile i, then tiles from an atomic counter through its
+# ring of stages.  "tile_per_sm": 8 rows per SM, one tile per CTA, the grid not clamped (the partial-sum reduction reads
+# every SM's partials).  "ring_twice": every CTA takes ~2 x stages tiles, so each stage is refilled (mbarrier parity
+# flips) and most tiles come from the counter; +5 leaves a ragged last tile.  "training": the encoder at a batch of 128
+# (8,208 tiles), 513 rows per sample, so tiles straddle samples.
+_LN_ROWS = [(D, rows) for D in (384, 768, 1024) for rows in ("tile_per_sm", "ring_twice")] + [(768, "training")]
+
+
+@pytest.mark.parametrize("D,rows", _LN_ROWS)
+@pytest.mark.parametrize("call", ["norm1", "mid_block", "final_norm"])
+def test_residual_ln_cabi_multi_tile(D, rows, call):
+    """xq_vit_residual_ln_fwd / _bwd at row counts where the persistent backward's CTAs take several tiles, with the
+    argument sets run_blocks passes: a block's first norm1 (no branch), a mid-block norm (branch + bias + LayerScale +
+    per-sample rowscale) and the final norm (branch, but x_out unused: g_xout = NULL).  fp64 autograd reference."""
+    from imagefolder_b200 import _capi
+    L = _capi.lib()
+    sms = _sms()
+    M, S = {"tile_per_sm": (8 * sms, 37), "ring_twice": (8 * sms * 2 * _ln_bwd_stages(D) + 5, 37),
+            "training": (TRAIN_ROWS, 513)}[rows]
+    torch.manual_seed(M + D)
+    dev = "cuda"
+    eps = 1e-6
+    x = torch.randn(M, D, device=dev) + 0.5 * torch.randn(M, 1, device=dev)     # row offsets: the mean is not ~0
+    w = torch.rand(D, device=dev) + 0.5
+    b = torch.randn(D, device=dev)
+    branch = bbias = gamma = rs = None
+    if call != "norm1":
+        branch = (torch.randn(M, D, device=dev) * 2).to(torch.bfloat16)
+        bbias = torch.randn(D, device=dev)
+        gamma = torch.rand(D, device=dev) + 0.5
+        rs = torch.rand((M + S - 1) // S, device=dev) * 1.5 + 0.25      # a different DropPath scale for every sample ...
+        rs[::5] = 0.0                                                     # ... and dropped samples
+    g_xout = torch.randn(M, D, device=dev) if call != "final_norm" else None
+    g_y = torch.randint(-4, 5, (M, D), device=dev).to(torch.bfloat16)    # integer-valued: d ln_b = sum g_y is exact
+
+    x_out, y, mean, rstd = _nan((M, D)), _nan((M, D), torch.bfloat16), _nan((M,)), _nan((M,))
+    stream = _capi.stream_ptr(x.device)
+    p = _capi.ptr
+    _capi.check(L.xq_vit_residual_ln_fwd(p(x), p(branch), p(bbias), p(gamma), p(rs), S, p(w), p(b), eps, M, D, p(x_out),
+                                         p(y), p(mean), p(rstd), stream), "xq_vit_residual_ln_fwd")
+    g_x = _nan((M, D))
+    g_w, g_b = _nan((D,)), _nan((D,))
+    g_branch = _nan((M, D), torch.bfloat16) if branch is not None else None
+    g_gamma = _nan((D,)) if branch is not None else None
+    g_bbias = _nan((D,)) if branch is not None else None
+    ws = torch.full((int(L.xq_vit_ln_bwd_workspace_bytes(D)),), 0xFF, dtype=torch.uint8, device=dev)   # NaN partials
+    _capi.check(L.xq_vit_residual_ln_bwd(p(g_xout), p(g_y), p(x_out), p(mean), p(rstd), p(w), p(branch), p(bbias), p(gamma),
+                                         p(rs), S, M, D, p(g_x), p(g_branch), p(g_w), p(g_b), p(g_gamma), p(g_bbias), p(ws),
+                                         ws.numel(), stream), "xq_vit_residual_ln_bwd")
+
+    # fp64 reference: x_new = x + s[row // S] * gamma * (branch + bias);  y = LayerNorm(x_new)
+    x2 = x.double().requires_grad_(True)
+    w2, b2 = w.double().requires_grad_(True), b.double().requires_grad_(True)
+    xn = x2
+    if branch is not None:
+        br2, bb2, ga2 = (t.double().requires_grad_(True) for t in (branch, bbias, gamma))
+        s_row = rs.double()[torch.arange(M, device=dev) // S].unsqueeze(1)
+        xn = x2 + s_row * ga2 * (br2 + bb2)
+    y2 = F.layer_norm(xn, (D,), w2, b2, eps)
+    if g_xout is not None:
+        torch.autograd.backward((y2, xn), (g_y.double(), g_xout.double()))
+    else:
+        y2.backward(g_y.double())
+    with torch.no_grad():
+        xn = xn.detach()
+        mean2 = xn.mean(-1)
+        rstd2 = (xn.var(-1, unbiased=False) + eps).rsqrt()
+        xh = (xn - mean2.unsqueeze(1)) * rstd2.unsqueeze(1)
+
+        # forward.  fp32 values: 1e-5 relative (of the row's mean |x_new| for the mean, a sum of D terms); bf16 y: 2^-8
+        if branch is None:
+            assert torch.equal(x_out, x)
+        _assert_within(x_out, xn, 1e-5 * xn.abs().max(), "x_out")
+        _assert_within(mean, mean2, 1e-5 * xn.abs().mean(-1), "mean")
+        _assert_within(rstd, rstd2, 1e-5 * rstd2, "rstd")
+        _assert_within(y.float(), y2.detach(), 2 ** -8 * y2.detach().abs().max(), "y")
+        del y2
+        # backward.  G = d x_new (= g_x); fp32 g_x: 1e-5 of its max; bf16 g_branch: 2^-8 of its max
+        G = x2.grad
+        _assert_within(g_x, G, 1e-5 * G.abs().max(), "g_x")
+        # column sums over M rows in fp32: a lane sums its CTA's tiles (~60 at the training shape), then 8 warps, then
+        # the per-SM partials 8 x 17 -- about 100 additions deep, 100 x 2^-24 < 1e-5 of sum |terms| of the column
+        gy64 = g_y.double()
+        _assert_within(g_w, w2.grad, 1e-5 * (gy64 * xh).abs().sum(0), "d ln_w")
+        assert torch.equal(g_b, g_y.to(torch.int64).sum(0).to(torch.float32)), "d ln_b: a row counted twice or not at all"
+        del gy64, xh
+        if branch is not None:
+            _assert_within(g_branch.float(), br2.grad, 2 ** -8 * br2.grad.abs().max(), "g_branch")
+            Gs = G * s_row
+            # the kernel sums G s branch and G s separately: d gamma = sum(G s branch) + bias sum(G s), d bias = gamma sum(G s)
+            sum_gs = Gs.abs().sum(0)
+            _assert_within(g_gamma, ga2.grad, 1e-5 * ((Gs * br2.detach()).abs().sum(0) + bb2.detach().abs() * sum_gs), "d gamma")
+            _assert_within(g_bbias, bb2.grad, 1e-5 * ga2.detach().abs() * sum_gs, "d branch_bias")
+
+
 def test_gelu_bf16():
     from imagefolder_b200.vit_ops import gelu_bias
     for C in (3072, 1536, 64):
@@ -95,6 +220,34 @@ def test_gelu_bf16():
         np.testing.assert_allclose(bias.grad.cpu().numpy(), b2.grad.float().cpu().numpy(), rtol=2e-2, atol=0.15)
     y = gelu_bias((torch.randn(2, 8, device="cuda")).to(torch.bfloat16), None)
     assert y.shape == (2, 8)
+
+    # the backward at the training rows and the ViT-B MLP width: every CTA of the persistent kernel walks dozens of row
+    # groups with the next group's loads in flight.  C ABI, NaN-filled outputs, fp64 reference in row chunks.
+    from imagefolder_b200 import _capi
+    L = _capi.lib()
+    M, C = TRAIN_ROWS, 3072
+    x = (torch.randn(M, C, device="cuda") * 2).to(torch.bfloat16)
+    bias = torch.randn(C, device="cuda")
+    gy = torch.randn(M, C, device="cuda").to(torch.bfloat16)
+    gx, gb = _nan((M, C), torch.bfloat16), _nan((C,))
+    _capi.check(L.xq_vit_gelu_bwd(_capi.ptr(x), _capi.ptr(bias), _capi.ptr(gy), _capi.ptr(gx), _capi.ptr(gb), M, C,
+                                  _capi.stream_ptr(x.device)), "xq_vit_gelu_bwd")
+    gb_ref, gb_abs, gy_abs = (torch.zeros(C, dtype=torch.float64, device="cuda") for _ in range(3))
+    errs, maxs = [], []
+    for r0 in range(0, M, 8192):
+        u = x[r0:r0 + 8192].double() + bias.double()
+        g64 = gy[r0:r0 + 8192].double()
+        t = g64 * (0.5 * (1.0 + torch.erf(u / math.sqrt(2.0))) + u * torch.exp(-0.5 * u * u) / math.sqrt(2.0 * math.pi))
+        errs.append((gx[r0:r0 + 8192].double() - t).abs().max())
+        maxs.append(t.abs().max())
+        gb_ref += t.sum(0)
+        gb_abs += t.abs().sum(0)
+        gy_abs += g64.abs().sum(0)
+    err, tmax = torch.stack(errs).max(), torch.stack(maxs).max()
+    assert bool(err <= 2 ** -8 * tmax), f"gx: max err {err.item():.3e} vs max {tmax.item():.3e}"     # bf16 output
+    # d bias: fp32 sums of the unrounded terms (a thread's ~100 rows, then one atomicAdd per CTA): rounding well under 1e-5 of
+    # sum |terms| of the column; the A&S erf inside gelu' adds at most ~5e-7 |gy| per term
+    _assert_within(gb, gb_ref, 1e-5 * gb_abs + 5e-7 * gy_abs, "d bias")
 
 
 def test_fused_blocks_match_module_path():
@@ -173,20 +326,32 @@ def test_pack_qkv_cabi_ragged_rows_and_bias():
     from imagefolder_b200 import _capi
     L = _capi.lib()
     torch.manual_seed(6)
-    for M, C in [(1, 8), (7, 64), (1031, 768), (4099, 384), (2500, 1024)]:
-        dq, dk, dv = (torch.randn(M, C, device="cuda").to(torch.bfloat16) for _ in range(3))
-        out = torch.empty(M, 3 * C, device="cuda", dtype=torch.bfloat16)
-        gb = torch.full((3 * C,), 7.0, device="cuda")
+    sms = _sms()
+    # the last two: the training encoder's rows (8,208 tiles, ~60 per CTA) and ~8 tiles per CTA at the widest C the kernel
+    # takes -- every CTA's 4-stage ring wraps and most tiles come from the atomic counter
+    for M, C in [(1, 8), (7, 64), (1031, 768), (4099, 384), (2500, 1024), (TRAIN_ROWS, 768), (8 * sms * 8 + 3, 1024)]:
         ws = torch.empty(int(L.xq_vit_pack_workspace_bytes()), dtype=torch.uint8, device="cuda")
-        _capi.check(L.xq_vit_pack_qkv(_capi.ptr(dq), _capi.ptr(dk), _capi.ptr(dv), _capi.ptr(out), _capi.ptr(gb), M, C,
-                                      _capi.ptr(ws), ws.numel(), _capi.stream_ptr(out.device)), "xq_vit_pack_qkv")
+
+        def pack(dq, dk, dv, gb):
+            out = _nan((M, 3 * C), torch.bfloat16)
+            _capi.check(L.xq_vit_pack_qkv(_capi.ptr(dq), _capi.ptr(dk), _capi.ptr(dv), _capi.ptr(out), _capi.ptr(gb), M, C,
+                                          _capi.ptr(ws), ws.numel(), _capi.stream_ptr(out.device)), "xq_vit_pack_qkv")
+            return out
+
+        # integer-valued gradients: the fp32 column sums are exact in any order, so the bias gradient must equal the int64
+        # sums -- a row counted twice or not at all fails at any M
+        dq, dk, dv = (torch.randint(-4, 5, (M, C), device="cuda").to(torch.bfloat16) for _ in range(3))
+        gb = torch.full((3 * C,), 7.0, device="cuda")                   # the launcher zeroes it
         ref = torch.cat([dq, dk, dv], dim=1)
-        assert torch.equal(out, ref)
-        np.testing.assert_allclose(gb.cpu().numpy(), ref.float().sum(0).cpu().numpy(), rtol=1e-4, atol=1e-3)
-        out.zero_()
-        _capi.check(L.xq_vit_pack_qkv(_capi.ptr(dq), _capi.ptr(dk), _capi.ptr(dv), _capi.ptr(out), None, M, C,
-                                      _capi.ptr(ws), ws.numel(), _capi.stream_ptr(out.device)), "xq_vit_pack_qkv")
-        assert torch.equal(out, ref)
+        assert torch.equal(pack(dq, dk, dv, gb), ref)
+        assert torch.equal(gb, ref.to(torch.int64).sum(0).to(torch.float32))
+        # full-mantissa values for the copy, with and without the bias gradient
+        dq, dk, dv = (torch.randn(M, C, device="cuda").to(torch.bfloat16) for _ in range(3))
+        ref = torch.cat([dq, dk, dv], dim=1)
+        assert torch.equal(pack(dq, dk, dv, gb), ref)
+        # fp32 sums: a lane's tiles (<= ~60), 8 warps, one atomicAdd per CTA: ~200 additions deep, 200 x 2^-24 = 1.2e-5
+        _assert_within(gb, ref.double().sum(0), 1.2e-5 * ref.double().abs().sum(0), "g_bias")
+        assert torch.equal(pack(dq, dk, dv, None), ref)
     assert L.xq_vit_pack_qkv(None, None, None, None, None, 4, 8, None, 0, None) != 0
 
 
@@ -293,6 +458,23 @@ def test_assemble_cabi_exact():
         gs, gt = torch.autograd.grad(out, (src, table), g)
         assert gs.dtype == dt and torch.equal(gs, g[:, 3:10].to(dt))
         np.testing.assert_allclose(gt.cpu().numpy(), g.sum(0).cpu().numpy(), rtol=1e-6, atol=1e-6)
+    # the backward at the encoder's sequence shape (cls + 256 image rows from src at t0 = 1 + 256 latents, D = 768) with
+    # batches where assemble_bwd_kernel's 8-sample loop runs once exactly, once plus a ragged step, and 16 times.  C ABI,
+    # NaN-filled outputs.  g on a 2^-8 grid with |g| <= 16: the cast to bf16 still rounds, and every partial sum over the
+    # batch is a multiple of 2^-8 below 2^11, exact in fp32 in any order -> d_table must equal the integer sum.
+    from imagefolder_b200 import _capi
+    L = _capi.lib()
+    T, Ls, t0, D = 513, 256, 1, 768
+    for B in (8, 9, 128):
+        gi = torch.randint(-4096, 4097, (B, T, D), device="cuda")
+        g = gi.float() / 256
+        d_table_ref = gi.sum(0).float() / 256
+        for dt in (torch.float32, torch.bfloat16):
+            d_src, d_table = _nan((B, Ls, D), dt), _nan((T, D))
+            _capi.check(L.xq_vit_assemble_bwd(_capi.ptr(g), B, Ls, T, D, t0, _capi.ptr(d_src), int(dt == torch.bfloat16),
+                                              _capi.ptr(d_table), _capi.stream_ptr(g.device)), "xq_vit_assemble_bwd")
+            assert torch.equal(d_src, g[:, t0:t0 + Ls].to(dt)), (B, dt)
+            assert torch.equal(d_table, d_table_ref), (B, dt)
 
 
 @pytest.mark.parametrize("M,C,Hd", [(2 * 513, 384, 1536), (4 * 513, 768, 3072), (131, 768, 3072), (3 * 256, 384, 1536)])
