@@ -224,6 +224,8 @@ static int gm_launch(const void *a, const void *b, void *c, void *c2, const floa
     const int nM = (M + GM_BM - 1) / GM_BM;
     int per_col = ds->n_sms / nN;                         // CTAs per column block
     if (per_col > nM) per_col = nM;
+    // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
+    if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st));
     mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(m.tmA, m.tmB, (__nv_bfloat16 *)c, (__nv_bfloat16 *)c2, bias, dbias, M, N, K);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
     return XQ_OK;
@@ -242,9 +244,7 @@ int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, co
                          int N, int K, void *stream) {
     if (int rc = xq::gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
     if (!d_bias) return XQ_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    XQ_CUDA_TRY(cudaMemsetAsync(d_bias, 0, sizeof(float) * (size_t)N, st));
-    return xq::gm_launch<2>(d_out, w2t, d_pre, const_cast<void *>(pre), bias, d_bias, M, N, K, st);
+    return xq::gm_launch<2>(d_out, w2t, d_pre, const_cast<void *>(pre), bias, d_bias, M, N, K, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -121,13 +121,24 @@ def gelu_bias(x, bias=None):
 
 
 MLP_TC_ENABLED = [True]       # the wgmma GEMMs with fused GELU / GELU' epilogues (csrc/gemm_kernel.cu)
+_SM_COUNT = {}                # device index -> multiprocessor count
+
+
+def _sm_count(device) -> int:
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    n = _SM_COUNT.get(idx)
+    if n is None:
+        n = _SM_COUNT[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return n
 
 
 def mlp_tc_ok(y, fc1, fc2) -> bool:
-    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd cover the shipped widths: bf16 tokens, hidden % 256 == 0, embed % 64 == 0."""
+    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd cover the shipped widths: bf16 tokens, hidden % 256 == 0, embed % 64 == 0,
+    out % 64 == 0 (the K of the backward GEMM), and at most one CTA column per SM (hidden / 128 <= SM count)."""
     return (MLP_TC_ENABLED[0] and y.is_cuda and y.dtype == torch.bfloat16 and fc1.bias is not None
-            and fc1.weight.shape[0] % 256 == 0 and fc1.weight.shape[1] % 64 == 0 and fc1.weight.shape[0] // 256 <= 64
-            and fc2.weight.shape[1] == fc1.weight.shape[0] and fc2.weight.shape[0] % 8 == 0)
+            and fc1.weight.shape[0] % 256 == 0 and fc1.weight.shape[1] % 64 == 0
+            and fc2.weight.shape[1] == fc1.weight.shape[0] and fc2.weight.shape[0] % 64 == 0
+            and fc1.weight.shape[0] // 128 <= _sm_count(y.device))
 
 
 class _FusedMLP(torch.autograd.Function):

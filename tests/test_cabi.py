@@ -153,15 +153,16 @@ def test_attention_entry_points_validate_arguments_without_gpu():
 
 
 def test_fused_mlp_gemm_entry_points_validate_arguments_without_gpu():
-    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd (csrc/gemm_kernel.cu): NULL pointers, misaligned buffers and widths the CTA-pair
-    tile does not cover are refused before anything is launched (the host then keeps library GEMM + the stand-alone kernel)."""
+    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd (csrc/gemm_kernel.cu): NULL pointers, misaligned buffers and widths the
+    128 x 128 tile with 64-wide K steps does not cover are refused before anything is launched (vit_ops.mlp_tc_ok keeps such
+    shapes on library GEMM + the stand-alone kernel)."""
     import ctypes as C
     from imagefolder_b200 import _capi
     L = _capi.lib()
     f = C.cast(C.c_void_p(4096), C.POINTER(C.c_float))
     assert L.xq_vit_fc1_gelu_fwd(None, 4096, f, 4096, 4096, 128, 3072, 768, None) == -1
     assert L.xq_vit_fc1_gelu_fwd(4096, 4096, f, 4096, 4096, 0, 3072, 768, None) == -1            # M = 0
-    assert L.xq_vit_fc1_gelu_fwd(4096, 4096, f, 4096, 4096, 128, 3000, 768, None) == -4          # N % 256 != 0: unsupported
+    assert L.xq_vit_fc1_gelu_fwd(4096, 4096, f, 4096, 4096, 128, 3000, 768, None) == -4          # N % 128 != 0: unsupported
     assert L.xq_vit_fc1_gelu_fwd(4096, 4096, f, 4096, 4096, 128, 3072, 100, None) == -4          # K % 64 != 0: unsupported
     assert L.xq_vit_fc1_gelu_fwd(4100, 4096, f, 4096, 4096, 128, 3072, 768, None) == -1          # x not 16-byte aligned
     assert L.xq_vit_fc2_dgelu_bwd(4096, 4096, 4096, f, 4096, None, 128, 3072, 768, None) == -1   # no bias-gradient buffer
@@ -170,8 +171,8 @@ def test_fused_mlp_gemm_entry_points_validate_arguments_without_gpu():
 
 
 def test_fused_mlp_dispatch_conditions():
-    """vit_ops.mlp_tc_ok: the fused GEMMs take bf16 CUDA tokens with hidden % 256 == 0 and embed % 64 == 0; everything else stays on
-    library GEMM + stand-alone bias / GELU kernel (same results, tests/test_gpu_vit_ops.py)."""
+    """vit_ops.mlp_tc_ok: the fused GEMMs take bf16 CUDA tokens with hidden % 256 == 0, embed % 64 == 0, out % 64 == 0 and
+    hidden / 128 <= SM count; everything else stays on library GEMM + stand-alone bias / GELU kernel (tests/test_gpu_mlp_gemm.py)."""
     import torch
     from imagefolder_b200 import vit_ops
     fc1, fc2 = torch.nn.Linear(768, 3072), torch.nn.Linear(3072, 768)
