@@ -131,6 +131,13 @@ def lib() -> ctypes.CDLL:
     L.xq_diffaug_forward.argtypes = [f32p, f32p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, f32p, f32p, vp]
     L.xq_diffaug_backward.restype = c_int
     L.xq_diffaug_backward.argtypes = [f32p, f32p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, f32p, f32p, vp]
+    # image transforms (csrc/img_kernels.cu): src / offs / plan / out are device pointers, except plan_host / ws_off_host
+    L.xq_img_workspace_bytes.restype = c_size_t
+    L.xq_img_workspace_bytes.argtypes = [vp, c_int, c_int, vp]
+    L.xq_img_box_halve.restype = c_int
+    L.xq_img_box_halve.argtypes = [vp, c_size_t, vp, vp, c_int, c_int, c_int, c_int, c_int, vp, c_size_t, vp]
+    L.xq_img_resize_crop_normalize.restype = c_int
+    L.xq_img_resize_crop_normalize.argtypes = [vp, c_size_t, vp, vp, c_int, c_int, vp, c_size_t, f32p, vp]
     _lib = L
     return L
 
@@ -212,5 +219,5 @@ EXPORTED_SYMBOLS = [
     "xq_ms_decode", "xq_ms_embed", "xq_usage_ema", "xq_usage_ema_dev", "xq_vit_residual_ln_fwd", "xq_vit_ln_bwd_workspace_bytes",
     "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_pack_qkv", "xq_vit_pack_workspace_bytes", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
-    "xq_diffaug_backward",
+    "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
 ]

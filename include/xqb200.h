@@ -296,6 +296,37 @@ int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *p
 int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
                          int M, int N, int K, void *stream);
 
+/* ---- input pipeline: the training / validation image transforms (SURVEY.md section 8 row f-4, csrc/img_kernels.cu) ---------
+ * Replaces the per-image CPU transform of the reference's DataLoader workers:
+ *   train  Compose([random_crop_arr, RandomHorizontalFlip(), ToTensor(), Normalize(0.5, 0.5)])  xqgan_train.py:225-230
+ *   val    Compose([center_crop_arr, ToTensor(), Normalize(0.5, 0.5)])                          xqgan_train.py:250-254
+ *   random_crop_arr / center_crop_arr                                                  dataset/augmentation.py:29-50 / :8-26
+ * bit-identically (Pillow 8-bit Image.resize arithmetic for the BOX halvings and the BICUBIC resize).  The workers only decode
+ * (np.asarray(Image.open(f).convert('RGB'))) and draw the random numbers; imagefolder_b200/data.py makes the plan.
+ *   src     uint8, every image [h, w, 3] (HWC) packed back to back; src_bytes = its length
+ *   offs    int64 [B, 2]: {byte offset of image i in src, byte offset of its halving buffers in the workspace}
+ *   plan    int32 [B, XQ_IMG_PLAN_COLS]: {h, w, levels (BOX halvings, augmentation.py:37-40 / :13-16), rs_h, rs_w (BICUBIC size,
+ *           :42-45 / :18-21), crop_y, crop_x (:48-49 / :24-25), flip (RandomHorizontalFlip's torch.rand(1) < 0.5)}
+ *   out     fp32 [B, 3, S, S] = (u / 255 - 0.5) / 0.5 of the cropped (and flipped) uint8 pixels
+ * A plan row is valid when h, w >= 1, (h, w) >> levels >= 1, rs_h, rs_w >= S, the crop lies inside the resized image, flip is 0/1
+ * and the BICUBIC resize has at most XQ_IMG_MAX_TAPS taps per axis (a downscale by less than 4 after the halvings).  The kernels
+ * re-check every row and every buffer bound and leave the output of an invalid image unwritten.
+ * ------------------------------------------------------------------------------------------------------------------------------ */
+#define XQ_IMG_PLAN_COLS 8
+#define XQ_IMG_MAX_TAPS 17
+#define XQ_IMG_MAX_SIZE 4096   /* largest crop side S */
+/* host-side: validates the plan (a HOST copy) for crop side S and lays out the halving buffers: ws_off_host [B] (may be NULL)
+ * receives each image's workspace offset.  Returns the workspace bytes (>= 16), or 0 when an argument or a plan row is invalid. */
+size_t xq_img_workspace_bytes(const int32_t *plan_host, int B, int S, int64_t *ws_off_host);
+/* one BOX halving level (1-based) for every image with levels >= level: (h, w) >> (level-1) -> (h, w) >> level, into the
+ * workspace.  Call it for level = 1 .. max(levels); max_out_h / max_out_w (the largest output at this level) only size the grid. */
+int xq_img_box_halve(const uint8_t *src, size_t src_bytes, const int64_t *offs, const int32_t *plan, int B, int S, int level,
+                     int max_out_h, int max_out_w, void *workspace, size_t workspace_bytes, void *stream);
+/* the final BICUBIC resize, evaluated only on the crop window, then flip, ToTensor and Normalize.  workspace may be NULL when no
+ * image has levels > 0. */
+int xq_img_resize_crop_normalize(const uint8_t *src, size_t src_bytes, const int64_t *offs, const int32_t *plan, int B, int S,
+                                 const void *workspace, size_t workspace_bytes, float *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
