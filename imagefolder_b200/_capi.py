@@ -14,6 +14,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libxqb200.so")
 XQ_MAX_SCALES = 32
+XQ_EMA_MAX_TENSORS = 1020      # entries of one xq_ema_update launch (include/xqb200.h)
 
 XQ_MS_VQ_ZNORM, XQ_MS_VQ_L2, XQ_MS_BSQ = 0, 1, 2
 
@@ -138,6 +139,9 @@ def lib() -> ctypes.CDLL:
     L.xq_img_box_halve.argtypes = [vp, c_size_t, vp, vp, c_int, c_int, c_int, c_int, c_int, vp, c_size_t, vp]
     L.xq_img_resize_crop_normalize.restype = c_int
     L.xq_img_resize_crop_normalize.argtypes = [vp, c_size_t, vp, vp, c_int, c_int, vp, c_size_t, f32p, vp]
+    # weight EMA (csrc/ema_kernel.cu): ema / param / numel are HOST arrays of device pointers and sizes
+    L.xq_ema_update.restype = c_int
+    L.xq_ema_update.argtypes = [vp, vp, vp, c_int, c_float, c_float, vp]
     _lib = L
     return L
 
@@ -220,4 +224,5 @@ EXPORTED_SYMBOLS = [
     "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_pack_qkv", "xq_vit_pack_workspace_bytes", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
+    "xq_ema_update",
 ]

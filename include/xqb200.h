@@ -327,6 +327,19 @@ int xq_img_box_halve(const uint8_t *src, size_t src_bytes, const int64_t *offs, 
 int xq_img_resize_crop_normalize(const uint8_t *src, size_t src_bytes, const int64_t *offs, const int32_t *plan, int B, int S,
                                  const void *workspace, size_t workspace_bytes, float *out, void *stream);
 
+/* ---- weight EMA of the trainer (csrc/ema_kernel.cu) ------------------------------------------------------------------------
+ * Replaces update_ema (utils/ema.py:4-14, called after every optimizer step at xqgan_train.py:461-462): for i < n
+ *   ema[i][k] <- ema[i][k] * decay + one_minus_decay * param[i][k]      k < numel[i], fp32
+ * bit-identical to torch's `ema.mul_(decay); ema.add_(param, alpha=one_minus_decay)` on the same GPU (fma(param, a, ema * d)).
+ *   ema, param, numel   HOST arrays of n entries; the pointers in ema / param are device pointers (4-byte aligned)
+ * The table travels in the kernel's parameter space: one launch per XQ_EMA_MAX_TENSORS entries, in order, on `stream`.
+ * n == 0 is a no-op; entries with numel 0 are skipped (their pointers may be NULL).  Every entry is validated before the first
+ * launch, so XQ_ERR_ARG (n < 0, NULL arrays, a negative numel, a NULL or misaligned pointer) means nothing was written.
+ * ------------------------------------------------------------------------------------------------------------------------------ */
+#define XQ_EMA_MAX_TENSORS 1020
+int xq_ema_update(float *const *ema, const float *const *param, const int64_t *numel, int n, float decay, float one_minus_decay,
+                  void *stream);
+
 #ifdef __cplusplus
 }
 #endif
