@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_float, c_int, c_int64, c_size_t, c_void_p
+from ctypes import POINTER, c_double, c_float, c_int, c_int64, c_size_t, c_void_p
 
 import torch
 
@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libxqb200.so")
 XQ_MAX_SCALES = 32
 XQ_EMA_MAX_TENSORS = 1020      # entries of one xq_ema_update launch (include/xqb200.h)
+XQ_ADAMW_MAX_TENSORS = 584     # entries of one xq_adamw_step launch (include/xqb200.h)
 
 XQ_MS_VQ_ZNORM, XQ_MS_VQ_L2, XQ_MS_BSQ = 0, 1, 2
 
@@ -142,6 +143,9 @@ def lib() -> ctypes.CDLL:
     # weight EMA (csrc/ema_kernel.cu): ema / param / numel are HOST arrays of device pointers and sizes
     L.xq_ema_update.restype = c_int
     L.xq_ema_update.argtypes = [vp, vp, vp, c_int, c_float, c_float, vp]
+    # AdamW step (csrc/adamw_kernel.cu): every array is a HOST array (of device pointers, sizes or per-tensor doubles)
+    L.xq_adamw_step.restype = c_int
+    L.xq_adamw_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, c_int, c_double, c_double, c_double, c_double, c_double, vp]
     _lib = L
     return L
 
@@ -224,5 +228,5 @@ EXPORTED_SYMBOLS = [
     "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_pack_qkv", "xq_vit_pack_workspace_bytes", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
-    "xq_ema_update",
+    "xq_ema_update", "xq_adamw_step",
 ]

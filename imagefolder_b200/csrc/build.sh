@@ -13,11 +13,13 @@ nvcc $FLAGS -c "$HERE/vq_tc_kernel.cu" -o "$OUT/vq_tc_kernel.o" "$@" &
 nvcc $FLAGS -c "$HERE/img_kernels.cu" -o "$OUT/img_kernels.o" "$@" &
 # weight EMA: its arithmetic is written with intrinsics, so the -fmad flag does not change it
 nvcc $FLAGS -c "$HERE/ema_kernel.cu" -o "$OUT/ema_kernel.o" "$@" &
+# AdamW step: the same, intrinsics throughout
+nvcc $FLAGS -c "$HERE/adamw_kernel.cu" -o "$OUT/adamw_kernel.o" "$@" &
 # ViT glue kernels carry no index decisions: default contraction (-fmad=true)
 nvcc ${FLAGS/-fmad=false/} -c "$HERE/vit_kernels.cu" -o "$OUT/vit_kernels.o" "$@" &
 nvcc ${FLAGS/-fmad=false/} -c "$HERE/loss_kernels.cu" -o "$OUT/loss_kernels.o" "$@" &
 nvcc ${FLAGS/-fmad=false/} -c "$HERE/attn_kernel.cu" -o "$OUT/attn_kernel.o" "$@" &
 nvcc ${FLAGS/-fmad=false/} -c "$HERE/gemm_kernel.cu" -o "$OUT/gemm_kernel.o" "$@" &
 for job in $(jobs -p); do wait "$job"; done     # a failed compile stops the build (a bare `wait` would ignore it)
-nvcc $ARCH -shared -o "$OUT/libxqb200.so" "$OUT/vq_kernels.o" "$OUT/vq_tc_kernel.o" "$OUT/ms_kernels.o" "$OUT/vit_kernels.o" "$OUT/loss_kernels.o" "$OUT/attn_kernel.o" "$OUT/gemm_kernel.o" "$OUT/img_kernels.o" "$OUT/ema_kernel.o" -lcudart
+nvcc $ARCH -shared -o "$OUT/libxqb200.so" "$OUT/vq_kernels.o" "$OUT/vq_tc_kernel.o" "$OUT/ms_kernels.o" "$OUT/vit_kernels.o" "$OUT/loss_kernels.o" "$OUT/attn_kernel.o" "$OUT/gemm_kernel.o" "$OUT/img_kernels.o" "$OUT/ema_kernel.o" "$OUT/adamw_kernel.o" -lcudart
 echo "$OUT/libxqb200.so"

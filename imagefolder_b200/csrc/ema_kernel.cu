@@ -10,18 +10,17 @@
 // alpha evaluates `self + other * alpha` in fp32 and nvcc contracts it to one fma.  Both steps are written as
 // intrinsics so that the -fmad flag of this translation unit cannot change them.
 //
-// Work split: the tensor table travels in the kernel's parameter space (__grid_constant__, up to 32 764 bytes on
-// sm_90 with CUDA >= 12.1), so there is no host-to-device copy.  Every tensor is cut into 64 KiB chunks; a persistent
-// grid takes the chunks in a grid stride and finds each chunk's tensor by a binary search over the chunk prefix.
+// Work split: the tensor table travels in the kernel's parameter space and a persistent grid walks its 64 KiB chunks
+// (xq_chunks.cuh).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "xq_common.cuh"
+#include "xq_chunks.cuh"
 
 namespace xqe {
 
-constexpr int THREADS = 256;
-constexpr int CHUNK = 16384;                 // floats per chunk (64 KiB); a multiple of 4, so float4 alignment holds per chunk
+using xqc::CHUNK;
+using xqc::THREADS;
 constexpr int U4 = 4;                        // float4 pairs in flight per thread (2 x 64 B)
 constexpr int U1 = 8;                        // floats in flight per thread on the scalar path
 constexpr int TABLE = XQ_EMA_MAX_TENSORS;
@@ -34,7 +33,7 @@ struct EmaTable {
     int n;
     float d, a;
 };
-static_assert(sizeof(EmaTable) <= 32764, "the tensor table must fit in the kernel parameter space");
+static_assert(sizeof(EmaTable) <= xqc::PARAM_BYTES, "the tensor table must fit in the kernel parameter space");
 
 __device__ __forceinline__ float ema_op(float e, float p, float d, float a) {
     return __fmaf_rn(p, a, __fmul_rn(e, d));
@@ -49,18 +48,11 @@ __global__ void __launch_bounds__(THREADS) ema_update_kernel(const __grid_consta
     const int64_t nchunks = tab.chunk_end[tab.n - 1];
     const float d = tab.d, a = tab.a;
     for (int64_t c = blockIdx.x; c < nchunks; c += gridDim.x) {
-        int lo = 0, hi = tab.n - 1;          // first tensor whose chunk_end exceeds c
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (tab.chunk_end[mid] > c) hi = mid;
-            else lo = mid + 1;
-        }
-        const int64_t first = lo ? tab.chunk_end[lo - 1] : 0;
-        const int64_t start = (c - first) * CHUNK;
-        const int count = (int)min((int64_t)CHUNK, tab.numel[lo] - start);
-        float *e = tab.ema[lo] + start;
-        const float *p = tab.param[lo] + start;
-        if ((((uintptr_t)tab.ema[lo] | (uintptr_t)tab.param[lo]) & 15) == 0) {
+        const xqc::Chunk k = xqc::locate_chunk(tab.chunk_end, tab.numel, tab.n, c);
+        const int count = k.count;
+        float *e = tab.ema[k.t] + k.start;
+        const float *p = tab.param[k.t] + k.start;
+        if ((((uintptr_t)tab.ema[k.t] | (uintptr_t)tab.param[k.t]) & 15) == 0) {
             float4 *e4 = reinterpret_cast<float4 *>(e);
             const float4 *p4 = reinterpret_cast<const float4 *>(p);
             const int n4 = count >> 2;
@@ -121,24 +113,20 @@ int xq_ema_update(float *const *ema, const float *const *param, const int64_t *n
         any = true;
     }
     if (!any) return XQ_OK;
-    int dev = 0, sms = 0, per_sm = 0;
-    XQ_CUDA_TRY(cudaGetDevice(&dev));
-    XQ_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    XQ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ema_update_kernel, THREADS, 0));
-    const int64_t max_grid = (int64_t)sms * (per_sm > 0 ? per_sm : 1);
+    int64_t max_grid = 0;
+    const int rc = xqc::persistent_grid(ema_update_kernel, &max_grid);
+    if (rc != XQ_OK) return rc;
     EmaTable tab;
     tab.d = decay;
     tab.a = one_minus_decay;
     for (int i0 = 0; i0 < n; i0 += TABLE) {
         tab.n = n - i0 < TABLE ? n - i0 : TABLE;
-        int64_t chunks = 0;
         for (int j = 0; j < tab.n; ++j) {
             tab.ema[j] = ema[i0 + j];
             tab.param[j] = param[i0 + j];
             tab.numel[j] = numel[i0 + j];
-            chunks += (numel[i0 + j] + CHUNK - 1) / CHUNK;
-            tab.chunk_end[j] = chunks;
         }
+        const int64_t chunks = xqc::chunk_prefix(tab.numel, tab.n, tab.chunk_end);
         if (chunks == 0) continue;
         const unsigned grid = (unsigned)(chunks < max_grid ? chunks : max_grid);
         ema_update_kernel<<<grid, THREADS, 0, (cudaStream_t)stream>>>(tab);

@@ -340,6 +340,26 @@ int xq_img_resize_crop_normalize(const uint8_t *src, size_t src_bytes, const int
 int xq_ema_update(float *const *ema, const float *const *param, const int64_t *numel, int n, float decay, float one_minus_decay,
                   void *stream);
 
+/* ---- AdamW step of the trainer (csrc/adamw_kernel.cu) ----------------------------------------------------------------------
+ * Replaces optimizer.step() / optimizer_disc.step() (torch.optim.AdamW, xqgan_train.py:344-347, 459, 474): for i < n, k < numel[i]
+ *   p = p * wd_factor  (skipped when wd_factor == 1);  m = lerp(m, g, one_minus_beta1);  v = v * beta2 + one_minus_beta2 * g * g
+ *   p = p + step_size[i] * m / (sqrt(v) / bc2_sqrt[i] + eps)
+ * bit-identical to torch's foreach AdamW (_multi_tensor_adam) for a tensor at step t, with the host values
+ *   wd_factor = 1 - lr * weight_decay, one_minus_beta1 = 1 - beta1, one_minus_beta2 = 1 - beta2,
+ *   step_size[i] = -(lr / (1 - beta1 ** t_i)), bc2_sqrt[i] = (1 - beta2 ** t_i) ** 0.5          (all doubles, t_i after the increment)
+ * each rounded once to fp32 here, as torch rounds its Scalar and scalar-list arguments.
+ *   param, grad, exp_avg, exp_avg_sq, numel, step_size, bc2_sqrt   HOST arrays of n entries; the tensor pointers are fp32 device
+ *   pointers (4-byte aligned).  The table travels in the kernel's parameter space: one launch per XQ_ADAMW_MAX_TENSORS entries, in
+ *   order, on `stream`.
+ * n == 0 is a no-op; entries with numel 0 are skipped (their pointers may be NULL).  Every entry and scalar is validated before the
+ * first launch, so XQ_ERR_ARG (n < 0, NULL arrays, a negative numel, a NULL or misaligned pointer, a non-finite scalar) means
+ * nothing was written.
+ * ------------------------------------------------------------------------------------------------------------------------------ */
+#define XQ_ADAMW_MAX_TENSORS 584
+int xq_adamw_step(float *const *param, const float *const *grad, float *const *exp_avg, float *const *exp_avg_sq,
+                  const int64_t *numel, const double *step_size, const double *bc2_sqrt, int n, double wd_factor,
+                  double one_minus_beta1, double beta2, double one_minus_beta2, double eps, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
