@@ -192,8 +192,8 @@ int xq_adamw_step(float *const *param, const float *const *grad, float *const *e
         any = true;
     }
     if (!any) return XQ_OK;
-    int64_t max_grid = 0;
-    const int rc = xqc::persistent_grid(adamw_step_kernel, &max_grid);
+    int max_grid = 0;
+    const int rc = xq::persistent_grid(adamw_step_kernel, THREADS, &max_grid);
     if (rc != XQ_OK) return rc;
     AdamwTable tab;
     // each scalar rounded once to fp32, as the foreach kernels receive it

@@ -17,8 +17,6 @@
 #include "xq_common.cuh"
 #include "xq_tc.cuh"
 
-#include <mutex>
-
 namespace xq {
 using namespace xqtc;
 
@@ -265,46 +263,6 @@ attn_fwd_tail_kernel(const __nv_bfloat16 *__restrict__ qkv, __nv_bfloat16 *__res
     if (lane == 0) lse2[(size_t)bh * N + n] = M + log2f(l);
 }
 
-// ---- host side ------------------------------------------------------------------------------------------------------
-struct AttnMaps {
-    const void *qkv;
-    int B, N, H;
-    CUtensorMap tmQKV;
-};
-
-// per-device one-time setup (function attributes are per device; the SM count may differ between devices of one process)
-struct AttnDevState { bool fwd_attr = false, bwd_attr = false, prep_attr = false; };
-static int attn_dev_state(AttnDevState **out) {
-    static std::mutex mu;
-    static AttnDevState states[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return xq::record_cuda_error(e, "cudaGetDevice");
-    if (dev < 0 || dev >= 64) return XQ_ERR_UNSUPPORTED;
-    std::lock_guard<std::mutex> g(mu);
-    *out = &states[dev];
-    return XQ_OK;
-}
-
-static bool get_fwd_maps(const void *qkv, int B, int N, int H, AttnMaps &m) {
-    static std::mutex mu;
-    static AttnMaps cache[16];
-    static int n_cached = 0, next = 0;
-    std::lock_guard<std::mutex> g(mu);
-    for (int i = 0; i < n_cached; ++i)
-        if (cache[i].qkv == qkv && cache[i].B == B && cache[i].N == N && cache[i].H == H) { m = cache[i]; return true; }
-    AttnMaps e;
-    e.qkv = qkv; e.B = B; e.N = N; e.H = H;
-    const uint64_t W = (uint64_t)3 * H * AT_D;
-    if (!make_map_3d(&e.tmQKV, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(qkv), W, N, B, W * 2, (uint64_t)N * W * 2, AT_D, AT_BM)) return false;
-    cache[next] = e;
-    next = (next + 1) % 16;
-    if (n_cached < 16) ++n_cached;
-    m = e;
-    return true;
-}
-
-
 // =====================================================================================================================
 // Backward.  One CTA per (batch, head, 128-key block), 288 threads: warpgroup wg owns keys 64 wg .. 64 wg + 63 of the block,
 // warp 8 is the TMA producer.  The CTA loops over the 64-query blocks i (Q_i, dO_i and the statistics through an AB_QS-stage
@@ -332,12 +290,6 @@ struct AttnBwdSmem {
     static constexpr int BAR = STAT + AB_QS * 512;
     static constexpr int BYTES = BAR + 256;
 };
-
-__device__ __forceinline__ void bulk_load_1d(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
 
 // dV / dK epilogue: the thread's accumulator fragment (rows rq, rq + 8 of the warpgroup's keys) * mul -> bf16 -> the packed
 // gradient, and the column sums of the ROUNDED values of the warp's 16 rows -> qkv-bias gradient.  Rows beyond N hold zeros
@@ -412,8 +364,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
                 mbar_expect_tx(&q_full[st], 2 * AB_QTILE + 2 * AB_BQ * 4);
                 tma_load_3d(base + AttnBwdSmem::Q + st * AB_QTILE, &tmQKV, colQ, i * AB_BQ, b, &q_full[st]);
                 tma_load_3d(base + AttnBwdSmem::DO + st * AB_QTILE, &tmDO, h * AT_D, i * AB_BQ, b, &q_full[st]);
-                bulk_load_1d(s_lse + st * AB_BQ, lseP + (size_t)bh * Npad + i * AB_BQ, AB_BQ * 4, &q_full[st]);
-                bulk_load_1d(s_delta + st * AB_BQ, deltaP + (size_t)bh * Npad + i * AB_BQ, AB_BQ * 4, &q_full[st]);
+                bulk_g2s(s_lse + st * AB_BQ, lseP + (size_t)bh * Npad + i * AB_BQ, AB_BQ * 4, &q_full[st]);
+                bulk_g2s(s_delta + st * AB_BQ, deltaP + (size_t)bh * Npad + i * AB_BQ, AB_BQ * 4, &q_full[st]);
             }
             __syncwarp();
         }
@@ -758,32 +710,6 @@ attn_dq_convert_kernel(const float *__restrict__ dq_acc, const __nv_bfloat16 *__
     }
 }
 
-struct AttnBwdMaps {
-    const void *qkv, *dout;
-    int B, N, H;
-    CUtensorMap tmQKV, tmDO;
-};
-
-static bool get_bwd_maps(const void *qkv, const void *dout, int B, int N, int H, AttnBwdMaps &m) {
-    static std::mutex mu;
-    static AttnBwdMaps cache[16];
-    static int n_cached = 0, next = 0;
-    std::lock_guard<std::mutex> g(mu);
-    for (int i = 0; i < n_cached; ++i)
-        if (cache[i].qkv == qkv && cache[i].dout == dout && cache[i].B == B &&
-            cache[i].N == N && cache[i].H == H) { m = cache[i]; return true; }
-    AttnBwdMaps e;
-    e.qkv = qkv; e.dout = dout; e.B = B; e.N = N; e.H = H;
-    const uint64_t W = (uint64_t)3 * H * AT_D, Wo = (uint64_t)H * AT_D;
-    if (!make_map_3d(&e.tmQKV, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(qkv), W, N, B, W * 2, (uint64_t)N * W * 2, AT_D, AB_BQ)) return false;
-    if (!make_map_3d(&e.tmDO, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(dout), Wo, N, B, Wo * 2, (uint64_t)N * Wo * 2, AT_D, AB_BQ)) return false;
-    cache[next] = e;
-    next = (next + 1) % 16;
-    if (n_cached < 16) ++n_cached;
-    m = e;
-    return true;
-}
-
 // keys handled by attn_bwd_prep_kernel instead of a key block of attn_bwd_kernel (0 = none)
 static int attn_bwd_ktail(int N) {
     const int r = N % AT_BN;
@@ -824,43 +750,32 @@ int xq_vit_attn_bwd(const void *qkv, const void *out, const void *d_out, const f
     float *lseP = (float *)((char *)workspace + off_lse);
     float *deltaP = (float *)((char *)workspace + off_delta);
     float *dsT = (float *)((char *)workspace + off_dst);
-    AttnBwdMaps m;
-    if (!get_bwd_maps(qkv, d_out, B, N, H, m)) return XQ_ERR_UNSUPPORTED;
+    const uint64_t W = (uint64_t)3 * H * AT_D, Wo = (uint64_t)H * AT_D;
+    CUtensorMap tmQKV, tmDO;
+    if (!tensor_map_bf16_3d(&tmQKV, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AB_BQ) ||
+        !tensor_map_bf16_3d(&tmDO, d_out, Wo, N, B, Wo * 2, (uint64_t)N * Wo * 2, AB_BQ))
+        return XQ_ERR_UNSUPPORTED;
     const int nt = attn_bwd_ktail(N);                                     // few trailing keys: CUDA-core kernel, not a key block
     const int nK = nt ? N / AT_BN : (N + AT_BN - 1) / AT_BN;
     const int Npad = (N + AT_BM - 1) / AT_BM * AT_BM;
     if ((long long)B * H > 65535) return XQ_ERR_UNSUPPORTED;
     if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, (size_t)3 * H * AT_D * sizeof(float), st));
     const float c2 = scale * 1.4426950408889634f;
-    AttnDevState *ds = nullptr;
-    if (int rc = attn_dev_state(&ds)) return rc;
     {
         dim3 grid(nt ? 1u : (unsigned)(Npad / AB_PREP_ROWS), (unsigned)(B * H));
-        const __nv_bfloat16 *qp = (const __nv_bfloat16 *)qkv, *op = (const __nv_bfloat16 *)out, *gp = (const __nv_bfloat16 *)d_out;
-        __nv_bfloat16 *dp = (__nv_bfloat16 *)dqkv;
-        constexpr int PS = 2 * 3 * (AB_PREP_ROWS / 32) * 256 * 16;             // the NT > 0 variants' two-stage row buffer
-        if (!ds->prep_attr) {
-            XQ_CUDA_TRY(cudaFuncSetAttribute(attn_bwd_prep_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS));
-            XQ_CUDA_TRY(cudaFuncSetAttribute(attn_bwd_prep_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS));
-            XQ_CUDA_TRY(cudaFuncSetAttribute(attn_bwd_prep_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS));
-            XQ_CUDA_TRY(cudaFuncSetAttribute(attn_bwd_prep_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, PS));
-            ds->prep_attr = true;
-        }
-        switch (nt) {
-        case 0: attn_bwd_prep_kernel<0><<<grid, 256, 0, st>>>(qp, op, gp, lse2, lseP, deltaP, acc, dsT, dp, g_bias, N, H, Npad, c2, scale); break;
-        case 1: attn_bwd_prep_kernel<1><<<grid, 256, PS, st>>>(qp, op, gp, lse2, lseP, deltaP, acc, dsT, dp, g_bias, N, H, Npad, c2, scale); break;
-        case 2: attn_bwd_prep_kernel<2><<<grid, 256, PS, st>>>(qp, op, gp, lse2, lseP, deltaP, acc, dsT, dp, g_bias, N, H, Npad, c2, scale); break;
-        case 3: attn_bwd_prep_kernel<3><<<grid, 256, PS, st>>>(qp, op, gp, lse2, lseP, deltaP, acc, dsT, dp, g_bias, N, H, Npad, c2, scale); break;
-        default: attn_bwd_prep_kernel<4><<<grid, 256, PS, st>>>(qp, op, gp, lse2, lseP, deltaP, acc, dsT, dp, g_bias, N, H, Npad, c2, scale); break;
-        }
+        // the NT > 0 variants' two-stage row buffer
+        const size_t ps = nt ? (size_t)2 * 3 * (AB_PREP_ROWS / 32) * 256 * 16 : 0;
+        decltype(&attn_bwd_prep_kernel<0>) const preps[] = {attn_bwd_prep_kernel<0>, attn_bwd_prep_kernel<1>, attn_bwd_prep_kernel<2>,
+                                                            attn_bwd_prep_kernel<3>, attn_bwd_prep_kernel<4>};
+        const auto prep = preps[nt < 4 ? nt : 4];
+        if (int rc = smem_optin(prep, ps)) return rc;
+        prep<<<grid, 256, ps, st>>>((const __nv_bfloat16 *)qkv, (const __nv_bfloat16 *)out, (const __nv_bfloat16 *)d_out, lse2, lseP,
+                                    deltaP, acc, dsT, (__nv_bfloat16 *)dqkv, g_bias, N, H, Npad, c2, scale);
         XQ_LAUNCH_CHECK("attn_bwd_prep_kernel");
     }
     const size_t smem = AttnBwdSmem::BYTES + 1024;
-    if (!ds->bwd_attr) {
-        XQ_CUDA_TRY(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ds->bwd_attr = true;
-    }
-    attn_bwd_kernel<<<dim3((unsigned)nK, (unsigned)(B * H)), AB_THREADS, smem, st>>>(m.tmQKV, m.tmDO, lseP, deltaP, acc,
+    if (int rc = smem_optin(attn_bwd_kernel, smem)) return rc;
+    attn_bwd_kernel<<<dim3((unsigned)nK, (unsigned)(B * H)), AB_THREADS, smem, st>>>(tmQKV, tmDO, lseP, deltaP, acc,
                                                                                      (__nv_bfloat16 *)dqkv, g_bias, N, H, Npad, c2, scale);
     XQ_LAUNCH_CHECK("attn_bwd_kernel");
     {
@@ -876,22 +791,18 @@ int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
     if (!qkv || !out || !lse2 || B <= 0 || N <= 0 || H <= 0) return XQ_ERR_ARG;
     if (head_dim != AT_D) return XQ_ERR_UNSUPPORTED;
     if (((uintptr_t)qkv & 15) || ((uintptr_t)out & 15)) return XQ_ERR_ARG;
-    AttnMaps m;
-    if (!get_fwd_maps(qkv, B, N, H, m)) return XQ_ERR_UNSUPPORTED;
+    const uint64_t W = (uint64_t)3 * H * AT_D;
+    CUtensorMap tmQKV;
+    if (!tensor_map_bf16_3d(&tmQKV, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AT_BM)) return XQ_ERR_UNSUPPORTED;
     // query tiles: full 128-row tiles on the tensor cores; a short remainder (<= AT_TAIL_MAX rows) on the CUDA cores
     const int n_tail = (N % AT_BM != 0 && N % AT_BM <= AT_TAIL_MAX && N > AT_BM) ? N % AT_BM : 0;
     const int nQ = n_tail ? N / AT_BM : (N + AT_BM - 1) / AT_BM;
     const size_t smem = AttnFwdSmem::BYTES + 1024;
-    AttnDevState *ds = nullptr;
-    if (int rc = attn_dev_state(&ds)) return rc;
-    if (!ds->fwd_attr) {
-        XQ_CUDA_TRY(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ds->fwd_attr = true;
-    }
+    if (int rc = smem_optin(attn_fwd_kernel, smem)) return rc;
     const long long tiles = (long long)B * H * nQ;
     if (tiles > 0x7fffffffLL) return XQ_ERR_ARG;
     const float c = scale * 1.4426950408889634f;
-    attn_fwd_kernel<<<(unsigned)tiles, AT_THREADS, smem, (cudaStream_t)stream>>>(m.tmQKV, (__nv_bfloat16 *)out, lse2, N, H, nQ, c);
+    attn_fwd_kernel<<<(unsigned)tiles, AT_THREADS, smem, (cudaStream_t)stream>>>(tmQKV, (__nv_bfloat16 *)out, lse2, N, H, nQ, c);
     XQ_LAUNCH_CHECK("attn_fwd_kernel");
     if (n_tail) {
         const long long warps = (long long)B * H * n_tail;

@@ -113,8 +113,8 @@ int xq_ema_update(float *const *ema, const float *const *param, const int64_t *n
         any = true;
     }
     if (!any) return XQ_OK;
-    int64_t max_grid = 0;
-    const int rc = xqc::persistent_grid(ema_update_kernel, &max_grid);
+    int max_grid = 0;
+    const int rc = xq::persistent_grid(ema_update_kernel, THREADS, &max_grid);
     if (rc != XQ_OK) return rc;
     EmaTable tab;
     tab.d = decay;

@@ -16,8 +16,6 @@
 #include "xq_tc.cuh"
 #include "xq_gelu.cuh"
 
-#include <mutex>
-
 namespace xq {
 
 using namespace xqtc;
@@ -155,56 +153,6 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------
-struct GemmMaps {
-    const void *a, *b;
-    int M, N, K;
-    CUtensorMap tmA, tmB;
-};
-
-static bool gm_get_maps(const void *a, const void *b, int M, int N, int K, GemmMaps &m) {
-    static std::mutex mu;
-    static GemmMaps cache[32];
-    static int n_cached = 0, next = 0;
-    std::lock_guard<std::mutex> g(mu);
-    for (int i = 0; i < n_cached; ++i)
-        if (cache[i].a == a && cache[i].b == b && cache[i].M == M && cache[i].N == N && cache[i].K == K) { m = cache[i]; return true; }
-    GemmMaps e;
-    e.a = a; e.b = b; e.M = M; e.N = N; e.K = K;
-    if (!make_map_3d(&e.tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(a), K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BK, GM_BM))
-        return false;
-    if (!make_map_3d(&e.tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(b), K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BK, GM_BN))
-        return false;
-    cache[next] = e;
-    next = (next + 1) % 32;
-    if (n_cached < 32) ++n_cached;
-    m = e;
-    return true;
-}
-
-struct GemmDevState { bool attr = false; int n_sms = 0; };
-static int gm_dev_state(GemmDevState **out) {
-    static std::mutex mu;
-    static GemmDevState states[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return record_cuda_error(e, "cudaGetDevice");
-    if (dev < 0 || dev >= 64) return XQ_ERR_UNSUPPORTED;
-    std::lock_guard<std::mutex> g(mu);
-    GemmDevState &s = states[dev];
-    if (!s.n_sms) {
-        e = cudaDeviceGetAttribute(&s.n_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (e != cudaSuccess) return record_cuda_error(e, "cudaDeviceGetAttribute");
-    }
-    if (!s.attr) {
-        e = cudaFuncSetAttribute(mlp_gemm_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GM_SMEM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(mlp_gemm_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GM_SMEM);
-        if (e != cudaSuccess) return record_cuda_error(e, "cudaFuncSetAttribute(mlp_gemm_kernel)");
-        s.attr = true;
-    }
-    *out = &s;
-    return XQ_OK;
-}
-
 static int gm_check(const void *a, const void *b, const void *c, const void *c2, const float *bias, int M, int N, int K) {
     if (!a || !b || !c || !c2 || !bias || M <= 0 || N <= 0 || K <= 0) return XQ_ERR_ARG;
     if (N % GM_BN != 0 || K % GM_BK != 0) return XQ_ERR_UNSUPPORTED;            // the ViT widths are multiples of 128 / 64
@@ -215,18 +163,21 @@ static int gm_check(const void *a, const void *b, const void *c, const void *c2,
 template <int EPI>
 static int gm_launch(const void *a, const void *b, void *c, void *c2, const float *bias, float *dbias, int M, int N, int K,
                      cudaStream_t st) {
-    GemmDevState *ds = nullptr;
-    if (int rc = gm_dev_state(&ds)) return rc;
+    int sms = 0;
+    if (int rc = sm_count(&sms)) return rc;
     const int nN = N / GM_BN;
-    if (nN > ds->n_sms) return XQ_ERR_UNSUPPORTED;
-    GemmMaps m;
-    if (!gm_get_maps(a, b, M, N, K, m)) return XQ_ERR_UNSUPPORTED;
+    if (nN > sms) return XQ_ERR_UNSUPPORTED;
+    CUtensorMap tmA, tmB;
+    if (!tensor_map_bf16_3d(&tmA, a, K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BM) ||
+        !tensor_map_bf16_3d(&tmB, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BN))
+        return XQ_ERR_UNSUPPORTED;
+    if (int rc = smem_optin(mlp_gemm_kernel<EPI>, GM_SMEM)) return rc;
     const int nM = (M + GM_BM - 1) / GM_BM;
-    int per_col = ds->n_sms / nN;                         // CTAs per column block
+    int per_col = sms / nN;                               // CTAs per column block
     if (per_col > nM) per_col = nM;
     // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
     if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st));
-    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(m.tmA, m.tmB, (__nv_bfloat16 *)c, (__nv_bfloat16 *)c2, bias, dbias, M, N, K);
+    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, (__nv_bfloat16 *)c, (__nv_bfloat16 *)c2, bias, dbias, M, N, K);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
     return XQ_OK;
 }

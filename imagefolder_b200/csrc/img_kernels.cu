@@ -15,11 +15,9 @@
 //   img_resize_crop_kernel   the final BICUBIC resize evaluated only on the crop window.  A CTA owns (image, 16-row strip):
 //                            it runs the strip's horizontal pass for the crop columns into shared memory (uint8, as Pillow's
 //                            intermediate), then the vertical pass, flip and normalisation, and writes fp32 [3, 16, S].
-#include <cuda_runtime.h>
 #include <math.h>
-#include <stdint.h>
 
-#include "../../include/xqb200.h"
+#include "xq_common.cuh"
 
 namespace xqi {
 
@@ -280,18 +278,19 @@ int xq_img_box_halve(const uint8_t *src, size_t src_bytes, const int64_t *offs, 
     dim3 grid((unsigned)min((max_out_w + 31) / 32, 1024), (unsigned)min((max_out_h + 7) / 8, 1024), (unsigned)B);
     img_box_halve_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(src, src_bytes, offs, plan, S, level, (uint8_t *)workspace,
                                                                   workspace_bytes);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("img_box_halve_kernel");
+    return XQ_OK;
 }
 
 int xq_img_resize_crop_normalize(const uint8_t *src, size_t src_bytes, const int64_t *offs, const int32_t *plan, int B, int S,
                                  const void *workspace, size_t workspace_bytes, float *out, void *stream) {
     if (!src || !offs || !plan || !out || B <= 0 || B > 65535 || S <= 0 || S > XQ_IMG_MAX_SIZE) return XQ_ERR_ARG;
-    cudaError_t e = cudaFuncSetAttribute(img_resize_crop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RC_SMEM);
-    if (e != cudaSuccess) return XQ_ERR_CUDA;
+    if (int rc = xq::smem_optin(img_resize_crop_kernel, RC_SMEM)) return rc;
     dim3 grid((unsigned)((S + RC_ROWS - 1) / RC_ROWS), (unsigned)B);
     img_resize_crop_kernel<<<grid, RC_THREADS, RC_SMEM, (cudaStream_t)stream>>>(src, src_bytes, offs, plan, S,
                                                                                 (const uint8_t *)workspace, workspace_bytes, out);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("img_resize_crop_kernel");
+    return XQ_OK;
 }
 
 }  // extern "C"

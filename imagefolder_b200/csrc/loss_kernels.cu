@@ -12,10 +12,8 @@
 // (per 8-channel chunk) because the single-pass form  sum w (a/na - b/nb)^2 = Swaa/na^2 + Swbb/nb^2 - 2 Swab/(na nb)
 // cancels when the reconstruction is close to the input.
 #include <cuda_bf16.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
 
-#include "../../include/xqb200.h"
+#include "xq_common.cuh"
 
 namespace xql {
 
@@ -329,9 +327,10 @@ int xq_lpips_layer_forward(const void *f0, const void *f1, int is_bf16, const fl
     else
         lpips_layer_fwd_kernel<<<grid, LP_THREADS, 0, st>>>((const float *)f0, (const float *)f1, lin_w, C, HW, eps,
                                                             (double *)workspace);
-    if (cudaGetLastError() != cudaSuccess) return XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("lpips_layer_fwd_kernel");
     lpips_reduce_kernel<<<B, 256, 0, st>>>((const double *)workspace, nblk, HW, accumulate, out);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("lpips_reduce_kernel");
+    return XQ_OK;
 }
 
 int xq_lpips_layer_backward(const void *f0, const void *f1, int is_bf16, const float *lin_w, int B, int C, int HW, float eps,
@@ -346,7 +345,8 @@ int xq_lpips_layer_backward(const void *f0, const void *f1, int is_bf16, const f
     else
         lpips_layer_bwd_kernel<<<grid, LP_THREADS, 0, st>>>((const float *)f0, (const float *)f1, lin_w, C, HW, eps, g_out,
                                                             (float *)g_f1);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("lpips_layer_bwd_kernel");
+    return XQ_OK;
 }
 
 static int aug_check(const float *a, const float *r, const float *ws, const float *o, int B, int C, int H, int W, int flags) {
@@ -361,10 +361,14 @@ int xq_diffaug_forward(const float *x, const float *rand01, int B, int C, int H,
     int rc = aug_check(x, rand01, sums, y, B, C, H, W, flags);
     if (rc != XQ_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    if (flags & 2) diffaug_sum_kernel<<<B, 512, 0, st>>>(x, rand01, B, C, H, W, flags, cut_h, cut_w, 0, sums);
+    if (flags & 2) {
+        diffaug_sum_kernel<<<B, 512, 0, st>>>(x, rand01, B, C, H, W, flags, cut_h, cut_w, 0, sums);
+        XQ_LAUNCH_CHECK("diffaug_sum_kernel");
+    }
     dim3 grid((H * W + 255) / 256, B);
     diffaug_fwd_kernel<<<grid, 256, 0, st>>>(x, rand01, sums, B, C, H, W, flags, cut_h, cut_w, y);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("diffaug_fwd_kernel");
+    return XQ_OK;
 }
 
 int xq_diffaug_backward(const float *g, const float *rand01, int B, int C, int H, int W, int flags, int cut_h, int cut_w,
@@ -372,10 +376,14 @@ int xq_diffaug_backward(const float *g, const float *rand01, int B, int C, int H
     int rc = aug_check(g, rand01, sums, gx, B, C, H, W, flags);
     if (rc != XQ_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    if (flags & 2) diffaug_sum_kernel<<<B, 512, 0, st>>>(g, rand01, B, C, H, W, flags, cut_h, cut_w, 1, sums);
+    if (flags & 2) {
+        diffaug_sum_kernel<<<B, 512, 0, st>>>(g, rand01, B, C, H, W, flags, cut_h, cut_w, 1, sums);
+        XQ_LAUNCH_CHECK("diffaug_sum_kernel");
+    }
     dim3 grid((H * W + 255) / 256, B);
     diffaug_bwd_kernel<<<grid, 256, 0, st>>>(g, rand01, sums, B, C, H, W, flags, cut_h, cut_w, gx);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("diffaug_bwd_kernel");
+    return XQ_OK;
 }
 
 }  // extern "C"

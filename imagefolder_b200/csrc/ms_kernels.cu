@@ -18,12 +18,6 @@
 
 namespace xq {
 
-static long long *g_ms_trace = nullptr;     // per-scale clock trace buffer (development builds only)
-#ifdef XQ_MS_TRACE
-extern "C" int xq_dev_set_ms_trace(void *dev_ptr) { g_ms_trace = (long long *)dev_ptr; return 0; }   // tools/ms_trace.py
-#endif
-
-
 constexpr int MS_THREADS = 384;       // forward / decode: 12 warps; the search tiling uses the first 256 threads (16 x 16)
 constexpr int MS_BWD_THREADS = 512;   // backward: no search, only latency-bound conv / pooling work -> more warps
 constexpr int MS_TILE_V = 128;
@@ -47,7 +41,6 @@ struct MsArgs {
     float *partial;       // [B] per-image loss partial
     float *F_last;        // [B,CHW] saved masked f_hat
     float *Fprev01;       // [SN,2,CHW] (BSQ) f_hat before scale si for images 0,1
-    long long *dbg;       // optional clock trace of CTA 0 (dev tool): [4*si + {0: pooled, 1: searched, 2: upsampled, 3: phi}]
 };
 
 // ---- shared-memory carve-up ------------------------------------------------------------
@@ -504,7 +497,6 @@ ms_forward_kernel(const MsArgs a) {
         ms_area_pool(s.rest, s.rows, C, H, W, P, RP);
         if (P != H || P != W) ms_cubic_tables(s, P, H, W);
         __syncthreads();
-        if (a.dbg && b == 0 && tid == 0) a.dbg[4 * si + 0] = clock64();
         if (bsq) {
             for (int r = tid; r < R; r += blockDim.x) {
                 int code = 0;
@@ -517,7 +509,6 @@ ms_forward_kernel(const MsArgs a) {
             __syncthreads();
             ms_search(s, a, R, RP, zz_s);
         }
-        if (a.dbg && b == 0 && tid == 0) a.dbg[4 * si + 1] = clock64();
         // indices out + histogram
         for (int r = tid; r < R; r += blockDim.x) {
             int v = s.idx[r];
@@ -528,7 +519,6 @@ ms_forward_kernel(const MsArgs a) {
         __syncthreads();
         ms_bicubic_up(s, C, H, W, P, RP);
         __syncthreads();
-        if (a.dbg && b == 0 && tid == 0) a.dbg[4 * si + 2] = clock64();
         if (bsq && a.Fprev01 && b < 2) {
             float *dst = a.Fprev01 + ((size_t)si * 2 + b) * CHW;
             for (int i = tid; i < CHW; i += blockDim.x) dst[i] = s.fhat[i];
@@ -555,7 +545,6 @@ ms_forward_kernel(const MsArgs a) {
         if (a.with_losses && m) loss_acc += sq / s.ratio[si];
         off += (int64_t)d.B * R;
         __syncthreads();
-        if (a.dbg && b == 0 && tid == 0) a.dbg[4 * si + 3] = clock64();
     }
     // epilogue: out, saved F_last, loss partial
     for (int i = tid; i < CHW; i += blockDim.x) {
@@ -1160,9 +1149,7 @@ int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const flo
     a.EnT = ws.EnT;
     a.ee = ws.ee;
     if (!bsq) {
-        codebook_prep_kernel<<<(a.Vpad + 127) / 128, 128, 0, stream>>>(E, d->V, C, a.Vpad, d->mode == XQ_MS_VQ_ZNORM,
-                                                                      ws.EnT, ws.ee);
-        XQ_LAUNCH_CHECK("codebook_prep_kernel");
+        if ((rc = launch_codebook_prep(E, d->V, C, a.Vpad, d->mode == XQ_MS_VQ_ZNORM, ws.EnT, ws.ee, stream)) != XQ_OK) return rc;
     }
     a.phi_w = phi_w; a.phi_b = phi_b; a.nq = with_losses ? n_quantizers : nullptr;
     a.with_losses = with_losses;
@@ -1170,8 +1157,7 @@ int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const flo
     a.partial = with_losses ? ws.partial : nullptr;
     a.F_last = saved ? sv.F_last : nullptr;
     a.Fprev01 = (bsq && with_losses) ? sv.Fprev01 : nullptr;
-    a.dbg = g_ms_trace;          // nullptr unless a development build set it (xq_dev_set_ms_trace, -DXQ_MS_TRACE)
-    XQ_CUDA_TRY(cudaFuncSetAttribute(ms_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if ((rc = smem_optin(ms_forward_kernel, smem)) != XQ_OK) return rc;
     ms_forward_kernel<<<d->B, MS_THREADS, smem, stream>>>(a);
     XQ_LAUNCH_CHECK("ms_forward_kernel");
     if (with_losses) {
@@ -1228,7 +1214,7 @@ int xq_ms_backward(const xq_ms_desc *d, const float *f, const float *E, const fl
         XQ_CUDA_TRY(cudaMemsetAsync(ws.dWpart, 0, sizeof(float) * (size_t)d->B * d->K * C * C * 9, stream));
         XQ_CUDA_TRY(cudaMemsetAsync(ws.dbpart, 0, sizeof(float) * (size_t)d->B * d->K * C, stream));
     }
-    XQ_CUDA_TRY(cudaFuncSetAttribute(ms_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if ((rc = smem_optin(ms_backward_kernel, smem)) != XQ_OK) return rc;
     ms_backward_kernel<<<d->B, MS_BWD_THREADS, smem, stream>>>(a);
     XQ_LAUNCH_CHECK("ms_backward_kernel");
     if (d->K > 0) {
@@ -1257,7 +1243,7 @@ int xq_ms_decode(const xq_ms_desc *d, const int64_t *idx_all, const float *E, co
     a.out = out; a.fhat_scales = fhat_scales; a.var_input = var_input;
     a.L_var = 0;
     for (int si = 1; si < d->SN; ++si) a.L_var += d->patch_nums[si] * d->patch_nums[si];
-    XQ_CUDA_TRY(cudaFuncSetAttribute(ms_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if ((rc = smem_optin(ms_decode_kernel, smem)) != XQ_OK) return rc;
     ms_decode_kernel<<<d->B, MS_THREADS, smem, (cudaStream_t)stream_>>>(a);
     XQ_LAUNCH_CHECK("ms_decode_kernel");
     return XQ_OK;
@@ -1275,7 +1261,7 @@ int xq_ms_embed(const xq_ms_desc *d, int si0, int si1, const float *h_all, const
     a.d = *d; a.idx_all = nullptr; a.h_all = h_all; a.E = nullptr; a.phi_w = phi_w; a.phi_b = phi_b;
     a.fhat_in = fhat_in; a.next = next; a.si0 = si0; a.si1 = si1;
     a.out = out; a.fhat_scales = fhat_scales; a.var_input = nullptr; a.L_var = 0;
-    XQ_CUDA_TRY(cudaFuncSetAttribute(ms_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if ((rc = smem_optin(ms_decode_kernel, smem)) != XQ_OK) return rc;
     ms_decode_kernel<<<d->B, MS_THREADS, smem, (cudaStream_t)stream_>>>(a);
     XQ_LAUNCH_CHECK("ms_decode_kernel");
     return XQ_OK;

@@ -15,23 +15,17 @@
 // Algorithmic bytes per element (row x channel): fwd 4 (x) + 2 (branch) + 4 (x_new) + 2 (y) = 12 B;
 // bwd 4 (g_xnew) + 2 (g_y) + 4 (x_new) + 2 (branch) + 4 (G) + 2 (g_branch) = 18 B.
 // These TUs do not carry index decisions, so they are built with the default -fmad=true.
-#include <cuda_bf16.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
-
-#include "../../include/xqb200.h"
+#include "xq_common.cuh"
 #include "xq_gelu.cuh"
+#include "xq_tc.cuh"
 
 namespace xqv {
 
+using namespace xqtc;
+using xq::warp_sum;
+
 constexpr int WARPS = 8;
 constexpr int THREADS = WARPS * 32;
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 struct bf16x4 { __nv_bfloat162 a, b; };
 
@@ -122,30 +116,10 @@ residual_ln_fwd_kernel(const float *__restrict__ x, const __nv_bfloat16 *__restr
 }
 
 // ---- TMA-bulk staged streaming skeleton -------------------------------------------------------------------------
-// A persistent 1-CTA-per-SM kernel whose producer warp stages row tiles into shared memory with cp.async.bulk (1-D TMA,
+// A persistent 1-CTA-per-SM kernel whose producer warp stages row tiles into shared memory with 1-D bulk copies (bulk_g2s,
 // mbarrier complete_tx) and whose consumer warps each own one row of the tile, with tiles handed out by an atomic counter:
 // no registers are spent on loads in flight and the memory system always has NST-1 tiles outstanding, so the register-
 // resident column sums ride along with a flat-copy-like stream (tools/mb/stream_mb.cu compares the skeletons).
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tXQV_WAIT:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra XQV_DONE;\n\tbra XQV_WAIT;\n\tXQV_DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
 
 // Backward.  grid = #SMs, 1 CTA / SM, warp 0 = producer, LNB_TR consumer warps (one tile row each), LNB_NST stages.
 // Stage layout: x_out [TR][D] f32 | g_xout [TR][D] f32 | g_y [TR][D] bf16 | branch [TR][D] bf16 | mean, rstd, scale [TR].
@@ -182,7 +156,7 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
     auto st_sc = [&](int st) { return reinterpret_cast<float *>(smem + st * stage_bytes + (size_t)TR * D * 12); };
     if (threadIdx.x == 0) {
         for (int i = 0; i < nst; ++i) { mbar_init(&full[i], 2); mbar_init(&empty[i], TR); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     __syncthreads();
 
@@ -190,7 +164,7 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
         // ---------------- producer ----------------
         for (int it = 0;; ++it) {
             const int st = it % nst;
-            mbar_wait(&empty[st], ((it / nst) & 1) ^ 1);
+            mbar_wait_ptx(&empty[st], ((it / nst) & 1) ^ 1);
             int tile = 0;
             if (lane == 0) tile = it == 0 ? (int)blockIdx.x : (int)gridDim.x + atomicAdd(counter, 1);
             tile = __shfl_sync(0xffffffffu, tile, 0);
@@ -230,7 +204,7 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
         }
         for (int it = 0;; ++it) {
             const int st = it % nst;
-            mbar_wait(&full[st], (it / nst) & 1);
+            mbar_wait_ptx(&full[st], (it / nst) & 1);
             const int tile = tile_of[st];
             if (tile >= ntiles) break;
             const int row = tile * TR + cw;
@@ -470,14 +444,14 @@ pack_qkv_kernel(const uint4 *__restrict__ dq, const uint4 *__restrict__ dk, cons
     const size_t stage_bytes = (size_t)3 * TR * src_row;           // [3][TR][C8] uint4
     if (threadIdx.x == 0) {
         for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TR); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     __syncthreads();
     if (warp == 0) {
         if (lane == 0) {
             for (int it = 0;; ++it) {
                 const int st = it % NST;
-                mbar_wait(&empty[st], ((it / NST) & 1) ^ 1);
+                mbar_wait_ptx(&empty[st], ((it / NST) & 1) ^ 1);
                 const int tile = it == 0 ? (int)blockIdx.x : (int)gridDim.x + atomicAdd(counter, 1);
                 tile_of[st] = tile;
                 if (tile >= ntiles) { mbar_arrive(&full[st]); break; }
@@ -498,7 +472,7 @@ pack_qkv_kernel(const uint4 *__restrict__ dq, const uint4 *__restrict__ dk, cons
             for (int k = 0; k < 8; ++k) acc[j][k] = 0.f;
         for (int it = 0;; ++it) {
             const int st = it % NST;
-            mbar_wait(&full[st], (it / NST) & 1);
+            mbar_wait_ptx(&full[st], (it / NST) & 1);
             const int tile = tile_of[st];
             if (tile >= ntiles) break;
             const int row = tile * TR + cw;
@@ -571,16 +545,6 @@ __global__ void patchify_kernel(const float *__restrict__ x, __nv_bfloat16 *__re
     store_bf16x4(out + i * 4, v);
 }
 
-// persistent grids = (SM count) x (CTAs of this kernel that are actually co-resident on one SM)
-template <typename K>
-static int persistent_grid(K kernel, int threads, size_t smem = 0) {
-    int dev = 0, sms = 148, per_sm = 1;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    return sms * per_sm;
-}
-
 // Token assembly (dinov2.py:151-170 / 318-336): the encoder / decoder build their input sequence as
 //   [prefix | image tokens | latent tokens] + positional / level embeddings
 // with cat + add + cat + add over [B, T, D] fp32 tensors.  Everything except ONE block of rows (the patch tokens in the
@@ -636,13 +600,6 @@ __global__ void assemble_bwd_kernel(const float *__restrict__ g, int B, int Ls, 
     if (d_table) *reinterpret_cast<float4 *>(d_table + ((size_t)t * D4 + d4) * 4) = acc;
 }
 
-static int bwd_grid() {
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return sms;      // 1 CTA / SM (TMA-staged tiles fill the shared memory)
-}
-
 }  // namespace xqv
 
 using namespace xqv;
@@ -657,7 +614,12 @@ using namespace xqv;
 
 extern "C" {
 
-size_t xq_vit_ln_bwd_workspace_bytes(int D) { return sizeof(float) * (size_t)bwd_grid() * NACC * D + 256; }
+// the TMA-staged kernels run 1 CTA / SM (their tiles fill the shared memory)
+size_t xq_vit_ln_bwd_workspace_bytes(int D) {
+    int sms = 0;
+    if (xq::sm_count(&sms) != XQ_OK) return 0;
+    return sizeof(float) * (size_t)sms * NACC * D + 256;
+}
 
 int xq_vit_residual_ln_fwd(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
                            const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
@@ -669,7 +631,8 @@ int xq_vit_residual_ln_fwd(const float *x, const void *branch, const float *bran
     XQV_DISPATCH(D, (residual_ln_fwd_kernel<NV><<<grid, THREADS, 0, st>>>(
                         x, (const __nv_bfloat16 *)branch, branch_bias, ls_gamma, rowscale, rows_per_sample, ln_w, ln_b,
                         eps, M, x_out, (__nv_bfloat16 *)y, mean, rstd)));
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("residual_ln_fwd_kernel");
+    return XQ_OK;
 }
 
 int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_out, const float *mean,
@@ -680,28 +643,30 @@ int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_
     if (!x_out || !mean || !rstd || M <= 0 || !workspace) return XQ_ERR_ARG;
     if (g_y && !ln_w) return XQ_ERR_ARG;
     if (branch && rowscale && rows_per_sample <= 0) return XQ_ERR_ARG;
-    int grid = bwd_grid();
-    if (workspace_bytes < sizeof(float) * (size_t)grid * NACC * D + 256) return XQ_ERR_WORKSPACE;
+    int sms = 0;
+    if (int rc = xq::sm_count(&sms)) return rc;
+    const size_t part_bytes = sizeof(float) * (size_t)sms * NACC * D;
+    if (workspace_bytes < part_bytes + 256) return XQ_ERR_WORKSPACE;
     const int ntiles = (M + LNB_TR - 1) / LNB_TR;
-    if (grid > ntiles) grid = ntiles;
+    const int grid = sms < ntiles ? sms : ntiles;
     cudaStream_t st = (cudaStream_t)stream;
     float *part = (float *)workspace;
-    int *counter = (int *)((char *)workspace + sizeof(float) * (size_t)bwd_grid() * NACC * D);   // dynamic tile counter
-    if (cudaMemsetAsync(counter, 0, sizeof(int), st) != cudaSuccess) return XQ_ERR_CUDA;
+    int *counter = (int *)((char *)workspace + part_bytes);   // dynamic tile counter
+    XQ_CUDA_TRY(cudaMemsetAsync(counter, 0, sizeof(int), st));
     const int nst = lnb_stages(D);
     size_t smem = lnb_stage_bytes(D) * nst;
     if (smem < sizeof(float) * (size_t)LNB_TR * NACC * D) smem = sizeof(float) * (size_t)LNB_TR * NACC * D;
     XQV_DISPATCH(D, {
-        if (cudaFuncSetAttribute(residual_ln_bwd_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return XQ_ERR_CUDA;
+        if (int rc = xq::smem_optin(residual_ln_bwd_kernel<NV>, smem)) return rc;
         residual_ln_bwd_kernel<NV><<<grid, LNB_THREADS, smem, st>>>(
             g_xout, (const __nv_bfloat16 *)g_y, x_out, mean, rstd, ln_w, (const __nv_bfloat16 *)branch, branch_bias,
             ls_gamma, rowscale, rows_per_sample, M, g_x, (__nv_bfloat16 *)g_branch, part, counter, nst);
     });
-    if (cudaGetLastError() != cudaSuccess) return XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("residual_ln_bwd_kernel");
     reduce_parts_kernel<<<(D + 31) / 32, 256, 0, st>>>(part, grid, D, ls_gamma, branch_bias, g_ln_w, g_ln_b,
                                                         branch ? g_ls_gamma : nullptr, branch ? g_branch_bias : nullptr);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("reduce_parts_kernel");
+    return XQ_OK;
 }
 
 size_t xq_vit_pack_workspace_bytes(void) { return 256; }
@@ -713,20 +678,21 @@ int xq_vit_pack_qkv(const void *dq, const void *dk, const void *dv, void *dqkv, 
     if (3 * (C / 8) > PACK_NCH * 32) return XQ_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     const int C8 = C / 8;
-    int *counter = (int *)workspace;     // dynamic tile counter, reset on the stream before each launch
-    if (cudaMemsetAsync(counter, 0, sizeof(int), st) != cudaSuccess) return XQ_ERR_CUDA;
-    if (g_bias && cudaMemsetAsync(g_bias, 0, sizeof(float) * 3 * (size_t)C, st) != cudaSuccess) return XQ_ERR_CUDA;
     const int ntiles = (int)((M + PACK_TR - 1) / PACK_TR);
-    int grid = bwd_grid();
+    int grid = 0;
+    if (int rc = xq::sm_count(&grid)) return rc;
     if (grid > ntiles) grid = ntiles;
     size_t smem = (size_t)PACK_NST * 3 * PACK_TR * C8 * 16;
     const size_t red = sizeof(float) * (size_t)PACK_TR * 3 * C8 * 8;
     if (smem < red) smem = red;
-    if (cudaFuncSetAttribute(pack_qkv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return XQ_ERR_CUDA;
+    if (int rc = xq::smem_optin(pack_qkv_kernel, smem)) return rc;
+    int *counter = (int *)workspace;     // dynamic tile counter, reset on the stream before each launch
+    XQ_CUDA_TRY(cudaMemsetAsync(counter, 0, sizeof(int), st));
+    if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, sizeof(float) * 3 * (size_t)C, st));
     pack_qkv_kernel<<<grid, PACK_THREADS, smem, st>>>((const uint4 *)dq, (const uint4 *)dk, (const uint4 *)dv,
                                                       (uint4 *)dqkv, g_bias, counter, (int)M, C8);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("pack_qkv_kernel");
+    return XQ_OK;
 }
 
 int xq_vit_assemble_fwd(const void *src, int src_is_bf16, const float *table, int B, int Ls, int T, int D, int t0, float *out,
@@ -738,7 +704,8 @@ int xq_vit_assemble_fwd(const void *src, int src_is_bf16, const float *table, in
         assemble_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)src, table, Ls, T, D / 4, t0, out, total4);
     else
         assemble_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float *)src, table, Ls, T, D / 4, t0, out, total4);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("assemble_fwd_kernel");
+    return XQ_OK;
 }
 
 int xq_vit_assemble_bwd(const float *g, int B, int Ls, int T, int D, int t0, void *d_src, int src_is_bf16, float *d_table,
@@ -749,7 +716,8 @@ int xq_vit_assemble_bwd(const float *g, int B, int Ls, int T, int D, int t0, voi
         assemble_bwd_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(g, B, Ls, T, D / 4, t0, (__nv_bfloat16 *)d_src, d_table);
     else
         assemble_bwd_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(g, B, Ls, T, D / 4, t0, (float *)d_src, d_table);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("assemble_bwd_kernel");
+    return XQ_OK;
 }
 
 int xq_vit_patchify(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream) {
@@ -758,7 +726,8 @@ int xq_vit_patchify(const float *x, void *patches, int B, int Cin, int H, int W,
     const size_t total4 = (size_t)B * Cin * H * W / 4;
     patchify_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)patches, Cin, H, W,
                                                                                        p, total4);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("patchify_kernel");
+    return XQ_OK;
 }
 
 int xq_vit_gelu_fwd(const void *x, const float *bias, void *y, int M, int C, void *stream) {
@@ -767,7 +736,8 @@ int xq_vit_gelu_fwd(const void *x, const float *bias, void *y, int M, int C, voi
     int threads = C8 >= 384 ? 384 : (C8 >= 192 ? 192 : 128);
     int grid = (M + GELU_RU - 1) / GELU_RU;
     gelu_fwd_kernel<<<grid, threads, 0, (cudaStream_t)stream>>>((const uint4 *)x, bias, (uint4 *)y, M, C8);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("gelu_fwd_kernel");
+    return XQ_OK;
 }
 
 int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C, void *stream) {
@@ -775,11 +745,13 @@ int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, 
     cudaStream_t st = (cudaStream_t)stream;
     int C8 = C / 8;
     int threads = C8 >= 384 ? 384 : (C8 >= 192 ? 192 : 128);
-    int grid = persistent_grid(gelu_bwd_kernel, threads);
+    int grid = 0;
+    if (int rc = xq::persistent_grid(gelu_bwd_kernel, threads, &grid)) return rc;
     if ((M + GELU_BWD_RU - 1) / GELU_BWD_RU < grid) grid = (M + GELU_BWD_RU - 1) / GELU_BWD_RU;
-    if (g_bias && cudaMemsetAsync(g_bias, 0, sizeof(float) * (size_t)C, st) != cudaSuccess) return XQ_ERR_CUDA;
+    if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, sizeof(float) * (size_t)C, st));
     gelu_bwd_kernel<<<grid, threads, 0, st>>>((const uint4 *)x, bias, (const uint4 *)gy, (uint4 *)gx, g_bias, M, C8);
-    return cudaGetLastError() == cudaSuccess ? XQ_OK : XQ_ERR_CUDA;
+    XQ_LAUNCH_CHECK("gelu_bwd_kernel");
+    return XQ_OK;
 }
 
 }  // extern "C"

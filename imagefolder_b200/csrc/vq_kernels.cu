@@ -26,6 +26,40 @@ int record_cuda_error(cudaError_t e, const char *what) {
     return XQ_ERR_CUDA;
 }
 
+// ---------------------------------------------------------------------------------------
+// codebook prep: one thread per code.  EnT is k-major so that code tiles are plain 2-D copies.
+// ---------------------------------------------------------------------------------------
+__global__ void codebook_prep_kernel(const float *__restrict__ E, int V, int C, int Vpad, int normalize,
+                                     float *__restrict__ EnT, float *__restrict__ ee) {
+    int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= Vpad) return;
+    if (v >= V) {
+        for (int k = 0; k < C; ++k) EnT[(size_t)k * Vpad + v] = 0.f;
+        ee[v] = CUDART_INF_F;
+        return;
+    }
+    const float *e = E + (size_t)v * C;
+    float den = 1.f;
+    if (normalize) {
+        float ss = 0.f;
+        for (int k = 0; k < C; ++k) ss = fmaf(e[k], e[k], ss);
+        den = fmaxf(sqrtf(ss), XQ_EPS);
+    }
+    float s2 = 0.f;
+    for (int k = 0; k < C; ++k) {
+        float x = normalize ? e[k] / den : e[k];
+        EnT[(size_t)k * Vpad + v] = x;
+        s2 = fmaf(x, x, s2);
+    }
+    ee[v] = s2;
+}
+
+int launch_codebook_prep(const float *E, int V, int C, int Vpad, int normalize, float *EnT, float *ee, cudaStream_t stream) {
+    codebook_prep_kernel<<<(Vpad + 127) / 128, 128, 0, stream>>>(E, V, C, Vpad, normalize, EnT, ee);
+    XQ_LAUNCH_CHECK("codebook_prep_kernel");
+    return XQ_OK;
+}
+
 constexpr int TILE_R = 128;  // rows per CTA
 constexpr int TILE_V = 128;  // codes per smem tile
 constexpr int NTHREADS = 256;
@@ -229,6 +263,12 @@ __global__ void finalize_mse_kernel(const float *__restrict__ partial, int n, do
         loss[0] = mse;
         loss[1] = beta * mse;
     }
+}
+
+int launch_finalize_mse(const float *partial, int n, double inv_count, float beta, float *loss, cudaStream_t stream) {
+    finalize_mse_kernel<<<1, 32, 0, stream>>>(partial, n, inv_count, beta, loss);
+    XQ_LAUNCH_CHECK("finalize_mse_kernel");
+    return XQ_OK;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -547,17 +587,13 @@ int xq_vq_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     float *ee = (float *)ws;
     ws += align_up(sizeof(float) * (size_t)Vp, 256);
     float *partial = (float *)ws;
-    codebook_prep_kernel<<<(Vp + 127) / 128, 128, 0, stream>>>(E, V, C, Vp, codebook_norm, EnT, ee);
-    XQ_LAUNCH_CHECK("codebook_prep_kernel");
-    XQ_CUDA_TRY(cudaFuncSetAttribute(vq_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (int rc = launch_codebook_prep(E, V, C, Vp, codebook_norm, EnT, ee, stream)) return rc;
+    if (int rc = smem_optin(vq_search_kernel, smem)) return rc;
     int ctas = (N + TILE_R - 1) / TILE_R;
     vq_search_kernel<<<ctas, NTHREADS, smem, stream>>>(z, E, EnT, ee, N, C, HW, V, Vp, codebook_norm, ste_value, idx,
                                                        out, loss ? partial : nullptr, hist);
     XQ_LAUNCH_CHECK("vq_search_kernel");
-    if (loss) {
-        finalize_mse_kernel<<<1, 32, 0, stream>>>(partial, ctas, 1.0 / ((double)N * (double)C), beta, loss);
-        XQ_LAUNCH_CHECK("finalize_mse_kernel");
-    }
+    if (loss) return launch_finalize_mse(partial, ctas, 1.0 / ((double)N * (double)C), beta, loss, stream);
     return XQ_OK;
 }
 
@@ -605,9 +641,8 @@ int xq_perturb_forward(const float *z, const float *zq, const float *E, const fl
     float *EnT = (float *)ws;
     ws += align_up(sizeof(float) * (size_t)Vp * C, 256);
     float *ee = (float *)ws;
-    codebook_prep_kernel<<<(Vp + 127) / 128, 128, 0, stream>>>(E, V, C, Vp, codebook_norm, EnT, ee);
-    XQ_LAUNCH_CHECK("codebook_prep_kernel");
-    XQ_CUDA_TRY(cudaFuncSetAttribute(rank_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (int rc = launch_codebook_prep(E, V, C, Vp, codebook_norm, EnT, ee, stream)) return rc;
+    if (int rc = smem_optin(rank_select_kernel, smem)) return rc;
     rank_select_kernel<<<nbc * HW, NTHREADS, smem, stream>>>(z, zq, E, EnT, ee, rand_u, rand_j, nbc * HW, C, HW, V, Vp,
                                                             codebook_norm, alpha, delta, out, sel);
     XQ_LAUNCH_CHECK("rank_select_kernel");

@@ -18,15 +18,10 @@
 // Roles (416 threads): warpgroups 0-1 = MMA (rows 64 wg .. 64 wg + 63), warpgroup 2 = epilogue (thread = row),
 // warp 12 = TMA producer.  Pipelines: full/empty mbarriers per smem stage (TMA <-> MMA), s_full/s_empty for the score
 // tile (MMA <-> epilogue).
-#include <cuda.h>
-#include <mutex>
-
 #include "xq_common.cuh"
 #include "xq_tc.cuh"
 
 namespace xq {
-
-static long long *g_vq_tc_trace = nullptr;     // in-kernel clock trace buffer (development builds only)
 
 constexpr int TC_BM = 128;       // rows per CTA  (two wgmma M = 64 halves)
 constexpr int TC_BN = 128;       // codes per tile (wgmma N)
@@ -41,16 +36,11 @@ using xqtc::elect_one;
 using xqtc::fence_async_smem;
 using xqtc::mbar_arrive;
 using xqtc::mbar_expect_tx;
+using xqtc::mbar_fence_init;
 using xqtc::mbar_init;
-using xqtc::mbar_wait;
+using xqtc::mbar_wait_ptx;
 using xqtc::smem_u32;
-
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int x, int y, uint64_t *bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(x), "r"(y), "r"(smem_u32(bar))
-        : "memory");
-}
+using xqtc::tma_load_2d;
 
 // byte offset of element (row, k) inside a K-major SWIZZLE_128B operand made of 32-float (128 B) K chunks
 __device__ __forceinline__ uint32_t sw128_off(int row, int k, int rows_per_chunk) {
@@ -100,12 +90,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__restrict__ z, const float *__restrict__ E,
                     const float *__restrict__ En, const float *__restrict__ ee, int N, int C, int HW, int V, int Vpad,
                     int nstage, int ste_value, int64_t *__restrict__ idx_out, float *__restrict__ out,
-                    float *__restrict__ partial, float *__restrict__ hist, long long *__restrict__ dbg) {
+                    float *__restrict__ partial, float *__restrict__ hist) {
     extern __shared__ uint8_t smem_raw[];
-    // dbg (optional, CTA 0 only): [0] start, [1] after prologue; per tile t: [8+4t+1] MMA warp 0 waited full,
-    // [+2] its MMAs retired, [+3] epilogue warp 8 done with tile
-    const bool trace = dbg && blockIdx.x == 0;
-    if (trace && threadIdx.x == 0) dbg[0] = clock64();
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     TcSmem s;
     s.A = (float *)base;
@@ -133,7 +119,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
         for (int i = 0; i < nstage; ++i) { mbar_init(&s.full[i], 1); mbar_init(&s.empty[i], 8); }
         mbar_init(s.sfull, 256);
         mbar_init(s.sempty, 128);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     // rows: coalesced load of the raw NCHW tile into the swizzled A operand (consecutive threads = consecutive
     // rows of one channel), then one thread per row normalises in place with the canonical chain
@@ -162,13 +148,12 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
     }
     fence_async_smem();            // generic-proxy stores to A -> visible to the async proxy (wgmma)
     __syncthreads();
-    if (trace && threadIdx.x == 0) dbg[1] = clock64();
 
     if (warp == 12) {
         // ===== TMA producer (whole warp runs the loop, one elected lane issues) =====
         for (int t = 0; t < T; ++t) {
             const int st = t % nstage;
-            mbar_wait(&s.empty[st], ((t / nstage) & 1) ^ 1);
+            mbar_wait_ptx(&s.empty[st], ((t / nstage) & 1) ^ 1);
             if (elect_one()) {
                 mbar_expect_tx(&s.full[st], stage_bytes);
                 float *dst = s.B + (size_t)st * TC_BN * C;
@@ -184,8 +169,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
         const uint32_t a_addr = smem_u32(s.A) + wg * 64 * 128;
         for (int t = 0; t < T; ++t) {
             const int st = t % nstage;
-            mbar_wait(&s.full[st], (t / nstage) & 1);
-            if (trace && tid == 0 && t < 60) dbg[8 + 4 * t + 1] = clock64();
+            mbar_wait_ptx(&s.full[st], (t / nstage) & 1);
             const uint32_t b_addr = smem_u32(s.B + (size_t)st * TC_BN * C);
             float acc[64];
             xqtc::wgmma_fence();
@@ -201,8 +185,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
             xqtc::fence_regs(acc);
             __syncwarp();
             if (lane == 0) mbar_arrive(&s.empty[st]);       // smem stage free
-            if (trace && tid == 0 && t < 60) dbg[8 + 4 * t + 2] = clock64();
-            mbar_wait(s.sempty, (t & 1) ^ 1);               // the epilogue has read the previous tile's scores
+            mbar_wait_ptx(s.sempty, (t & 1) ^ 1);               // the epilogue has read the previous tile's scores
             float *r0 = s.S + (size_t)rq * TC_SLD, *r1 = r0 + 8 * TC_SLD;
 #pragma unroll
             for (int j = 0; j < TC_BN / 8; ++j) {
@@ -223,7 +206,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
         float *cs2 = s.cand_s2 + row * TC_CAP;
         int *cv = s.cand_v + row * TC_CAP;
         for (int t = 0; t < T; ++t) {
-            mbar_wait(s.sfull, t & 1);
+            mbar_wait_ptx(s.sfull, t & 1);
             const int vt = t * TC_BN;
             const float *srow = s.S + (size_t)row * TC_SLD;
 #pragma unroll
@@ -271,10 +254,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
                     }
                 }
             }
-
-            if (trace && warp == 8 && lane == 0 && t < 60) dbg[8 + 4 * t + 3] = clock64();
         }
-        if (trace && warp == 8 && lane == 0) dbg[2] = clock64();
         // exact canonical rescoring, warp-cooperative: for every (row, candidate group) of this warp, lane j
         // scores code j of the group against the row (row values broadcast from smem, the 32 code rows are one
         // contiguous 32*C*4-byte block of En), then a (d, code) lexicographic warp-argmin picks the winner.
@@ -333,7 +313,6 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
             if (lane == r) { best_d = rb_d; best_v = rb_v; }
         }
         s.idx[row] = best_v;
-        if (trace && warp == 8 && lane == 0) dbg[4] = clock64();
     }
     __syncthreads();
     // ---- common epilogue: z_q = normalised code (xqgan_model.py:769-771).  En[v] (prep kernel) holds exactly
@@ -359,7 +338,6 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
     }
     sq = block_sum(sq, s.red);
     if (tid == 0 && partial) partial[blockIdx.x] = sq;
-    if (trace && tid == 0) dbg[3] = clock64();
 }
 
 // row-major normalised codebook En[Vpad][C] (+ ee[Vpad]); padded rows are zero
@@ -385,18 +363,6 @@ __global__ void codebook_prep_rowmajor_kernel(const float *__restrict__ E, int V
     ee[v] = s2;
 }
 
-__global__ void finalize_mse_tc_kernel(const float *__restrict__ partial, int n, double inv_count, float beta,
-                                       float *__restrict__ loss) {
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < n; i += 32) acc += (double)partial[i];
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (threadIdx.x == 0) {
-        float mse = (float)(acc * inv_count);
-        loss[0] = mse;
-        loss[1] = beta * mse;
-    }
-}
-
 size_t vq_tc_workspace_bytes(int B, int C, int HW, int V) {
     size_t Vp = ((size_t)V + TC_BN - 1) / TC_BN * TC_BN;
     size_t ctas = ((size_t)B * HW + TC_BM - 1) / TC_BM;
@@ -413,8 +379,6 @@ int vq_tc_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     if (!vq_tc_supported(C, V, 1)) return XQ_ERR_UNSUPPORTED;
     if (workspace_bytes < vq_tc_workspace_bytes(B, C, HW, V)) return XQ_ERR_WORKSPACE;
     if (((uintptr_t)workspace & 127) != 0) return XQ_ERR_UNSUPPORTED;   // TMA global address alignment
-    xqtc::PFN_encodeTiled enc = xqtc::get_encode_fn();
-    if (!enc) return XQ_ERR_UNSUPPORTED;
     const int Vp = (V + TC_BN - 1) / TC_BN * TC_BN;
     const int N = B * HW;
     char *ws = (char *)workspace;
@@ -427,50 +391,23 @@ int vq_tc_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     const size_t smem = tc_smem_bytes(C, nstage);
     if (smem > 227 * 1024) return XQ_ERR_UNSUPPORTED;
 
-    // the tensor map depends only on (workspace pointer, Vp, C): encode it once per distinct triple
-    struct MapEntry { const void *ptr; int Vp, C; CUtensorMap tm; };
-    static std::mutex map_mu;
-    static MapEntry map_cache[8];
-    static int map_n = 0, map_next = 0;
+    // code tiles of En [Vp][C]: 32 floats (128 bytes) x TC_BN codes per box
+    const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)Vp}, strides[1] = {(cuuint64_t)C * sizeof(float)};
+    const cuuint32_t box[2] = {32u, (cuuint32_t)TC_BN};
     CUtensorMap tm;
-    {
-        std::lock_guard<std::mutex> g(map_mu);
-        bool hit = false;
-        for (int i = 0; i < map_n && !hit; ++i)
-            if (map_cache[i].ptr == (const void *)En && map_cache[i].Vp == Vp && map_cache[i].C == C) { tm = map_cache[i].tm; hit = true; }
-        if (!hit) {
-            cuuint64_t gdim[2] = {(cuuint64_t)C, (cuuint64_t)Vp};
-            cuuint64_t gstr[1] = {(cuuint64_t)C * sizeof(float)};
-            cuuint32_t box[2] = {32u, (cuuint32_t)TC_BN};
-            cuuint32_t estr[2] = {1u, 1u};
-            CUresult r = enc(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)En, gdim, gstr, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) return XQ_ERR_UNSUPPORTED;
-            map_cache[map_next] = MapEntry{(const void *)En, Vp, C, tm};
-            map_next = (map_next + 1) % 8;
-            if (map_n < 8) ++map_n;
-        }
-    }
+    if (!xqtc::tensor_map(&tm, En, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+        return XQ_ERR_UNSUPPORTED;
 
     codebook_prep_rowmajor_kernel<<<(Vp + 127) / 128, 128, 0, stream>>>(E, V, C, Vp, En, ee);
     XQ_LAUNCH_CHECK("codebook_prep_rowmajor_kernel");
     const int ctas = (N + TC_BM - 1) / TC_BM;
-    long long *dbg = g_vq_tc_trace;          // nullptr unless a development build set it (xq_dev_set_vq_trace, -DXQ_VQ_TC_TRACE)
     auto kern = C == 32 ? vq_search_tc_kernel<1> : vq_search_tc_kernel<2>;
-    XQ_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (int rc = smem_optin(kern, smem)) return rc;
     kern<<<ctas, TC_THREADS, smem, stream>>>(tm, z, E, En, ee, N, C, HW, V, Vp, nstage, ste_value, idx, out,
-                                             loss ? partial : nullptr, hist, dbg);
+                                             loss ? partial : nullptr, hist);
     XQ_LAUNCH_CHECK("vq_search_tc_kernel");
-    if (loss) {
-        finalize_mse_tc_kernel<<<1, 32, 0, stream>>>(partial, ctas, 1.0 / ((double)N * (double)C), beta, loss);
-        XQ_LAUNCH_CHECK("finalize_mse_tc_kernel");
-    }
+    if (loss) return launch_finalize_mse(partial, ctas, 1.0 / ((double)N * (double)C), beta, loss, stream);
     return XQ_OK;
 }
-
-#ifdef XQ_VQ_TC_TRACE
-extern "C" int xq_dev_set_vq_trace(void *dev_ptr) { xq::g_vq_tc_trace = (long long *)dev_ptr; return 0; }   // tools/vq_tc_trace.py
-#endif
 
 }  // namespace xq

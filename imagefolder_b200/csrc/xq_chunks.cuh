@@ -48,15 +48,4 @@ static inline int64_t chunk_prefix(const int64_t *numel, int n, int64_t *chunk_e
     return chunks;
 }
 
-// largest persistent grid of `kernel` at THREADS threads on the current device
-template <typename K>
-static inline int persistent_grid(K kernel, int64_t *max_grid) {
-    int dev = 0, sms = 0, per_sm = 0;
-    XQ_CUDA_TRY(cudaGetDevice(&dev));
-    XQ_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    XQ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, THREADS, 0));
-    *max_grid = (int64_t)sms * (per_sm > 0 ? per_sm : 1);
-    return XQ_OK;
-}
-
 }  // namespace xqc

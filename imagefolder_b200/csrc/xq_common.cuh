@@ -1,4 +1,4 @@
-// xq_common.cuh -- shared device helpers for libxqb200 (sm_90a).
+// xq_common.cuh -- shared device helpers and per-device launch state for libxqb200 (sm_90a).
 //
 // CANONICAL ARITHMETIC (DESIGN.md): every value that feeds an index decision is IEEE fp32,
 // round-to-nearest, fixed operation order, fused multiply-add only where written as fmaf().
@@ -9,6 +9,10 @@
 #include <cstdio>
 #include <math_constants.h>
 #include <stdint.h>
+
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "../../include/xqb200.h"
 
@@ -91,33 +95,58 @@ __device__ __forceinline__ float block_sum(float v, float *red) {
     return r;
 }
 
-// ---------------------------------------------------------------------------------------
-// codebook prep: one thread per code.  EnT is k-major so that code tiles are plain 2-D copies.
-// ---------------------------------------------------------------------------------------
-static __global__ void codebook_prep_kernel(const float *__restrict__ E, int V, int C, int Vpad, int normalize,
-                                     float *__restrict__ EnT, float *__restrict__ ee) {
-    int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= Vpad) return;
-    if (v >= V) {
-        for (int k = 0; k < C; ++k) EnT[(size_t)k * Vpad + v] = 0.f;
-        ee[v] = CUDART_INF_F;
-        return;
+// ---- kernels of vq_kernels.cu launched from other files (a kernel cannot be launched across files without -rdc) ----
+// EnT[C][Vpad] (k-major, normalised when `normalize`) and ee[Vpad] from the codebook E[V][C]; padded codes are zero, ee = inf
+int launch_codebook_prep(const float *E, int V, int C, int Vpad, int normalize, float *EnT, float *ee, cudaStream_t stream);
+// loss = {mse, beta * mse} from the n per-CTA squared-error partials, summed in a fixed order
+int launch_finalize_mse(const float *partial, int n, double inv_count, float beta, float *loss, cudaStream_t stream);
+
+// ---- per-device launch state ----------------------------------------------------------------------------------------
+// `inline`, not `static`: each cache below is one object for the whole library, whichever file calls it.
+
+// SM count of the current device, queried once per device
+inline int sm_count(int *n) {
+    static std::mutex mu;
+    static std::map<int, int> counts;
+    int dev = 0;
+    XQ_CUDA_TRY(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> g(mu);
+    int &c = counts[dev];
+    if (c == 0) {
+        int q = 0;
+        XQ_CUDA_TRY(cudaDeviceGetAttribute(&q, cudaDevAttrMultiProcessorCount, dev));
+        c = q;
     }
-    const float *e = E + (size_t)v * C;
-    float den = 1.f;
-    if (normalize) {
-        float ss = 0.f;
-        for (int k = 0; k < C; ++k) ss = fmaf(e[k], e[k], ss);
-        den = fmaxf(sqrtf(ss), XQ_EPS);
-    }
-    float s2 = 0.f;
-    for (int k = 0; k < C; ++k) {
-        float x = normalize ? e[k] / den : e[k];
-        EnT[(size_t)k * Vpad + v] = x;
-        s2 = fmaf(x, x, s2);
-    }
-    ee[v] = s2;
+    *n = c;
+    return XQ_OK;
 }
 
+// opts `kernel` into `bytes` of dynamic shared memory on the current device; cudaFuncSetAttribute runs only when `bytes`
+// exceeds what was last set for that kernel there
+inline int smem_optin(const void *kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void *>, size_t> set;
+    int dev = 0;
+    XQ_CUDA_TRY(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> g(mu);
+    size_t &cur = set[{dev, kernel}];
+    if (bytes > cur) {
+        XQ_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        cur = bytes;
+    }
+    return XQ_OK;
+}
+template <typename K>
+inline int smem_optin(K *kernel, size_t bytes) { return smem_optin((const void *)kernel, bytes); }
+
+// largest grid of `kernel` (`threads` per CTA, no dynamic shared memory) whose CTAs are all co-resident on the current device
+template <typename K>
+inline int persistent_grid(K kernel, int threads, int *grid) {
+    int sms = 0, per_sm = 0;
+    if (int rc = sm_count(&sms)) return rc;
+    XQ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0));
+    *grid = sms * (per_sm > 0 ? per_sm : 1);
+    return XQ_OK;
+}
 
 }  // namespace xq

@@ -1,4 +1,5 @@
-// xq_tc.cuh -- PTX wrappers for the bf16 / tf32 wgmma + TMA + mbarrier kernels of libxqb200 (sm_90a).
+// xq_tc.cuh -- PTX wrappers for the bf16 / tf32 wgmma + TMA + mbarrier kernels of libxqb200 (sm_90a), and the library's one
+// tensor-map cache.
 //
 // Shared-memory operand layouts used by the attention and GEMM kernels (all SWIZZLE_128B, 1024-byte aligned tiles):
 //   "row tile"  [R rows][64 bf16]  = what one TMA box {64, R, 1} of a [.., rows, 64*k] tensor lands as:
@@ -16,6 +17,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstring>
+#include <mutex>
+
 namespace xqtc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -31,17 +35,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ bool mbar_try(uint64_t *bar, uint32_t parity) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return done != 0;
-}
 // non-blocking poll (try_wait may put the thread to sleep for an implementation-defined time before answering "not yet";
 // an event loop that polls several barriers must not pay that for every barrier that is not ready)
 __device__ __forceinline__ bool mbar_test(uint64_t *bar, uint32_t parity) {
@@ -55,13 +48,47 @@ __device__ __forceinline__ bool mbar_test(uint64_t *bar, uint32_t parity) {
         : "memory");
     return done != 0;
 }
+// Two forms of the same wait; each kernel uses the one it runs fastest with on an H100 (80GB HBM3, 700 W).
+//   mbar_wait, a C++ loop around try_wait: the attention and GEMM kernels (attn_fwd_kernel is 1.4 % slower with the
+//     PTX loop);
+//   mbar_wait_ptx, the retry loop written in PTX: the TMA-bulk staged ViT kernels and the VQ search
+//     (residual_ln_bwd_kernel at D = 1024 and vq_search_tc_kernel<1> are 6 % and 1.4 % slower with the C++ loop).
+__device__ __forceinline__ bool mbar_try(uint64_t *bar, uint32_t parity) {
+    uint32_t done;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.b32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return done != 0;
+}
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     while (!mbar_try(bar, parity)) {}
+}
+__device__ __forceinline__ void mbar_wait_ptx(uint64_t *bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tXQ_MBAR_WAIT:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra XQ_MBAR_DONE;\n\tbra XQ_MBAR_WAIT;\n\tXQ_MBAR_DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
 // ---- TMA (tensor maps are __grid_constant__ kernel parameters) ------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
+// 1-D bulk copy global -> shared (no tensor map): `bytes` a multiple of 16, both addresses 16-byte aligned
+__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
+                 : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+        : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, int c0, int c1, int c2, uint64_t *bar) {
     asm volatile(
@@ -202,35 +229,59 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                    const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// ---- tensor maps (host) ---------------------------------------------------------------------------------------
+// Every tensor map of the library comes from tensor_map(): encoded on first use and kept in one cache of TMAP_CACHE maps
+// with round-robin eviction, under one mutex.  The key is every argument of cuTensorMapEncodeTiled that a caller chooses
+// (base, dtype, rank, dims, strides, box, swizzle), so a hit is correct whoever asks.  Element strides are 1, L2 promotion
+// 256 B, and out-of-bounds elements read as zero.  `dims` and `box` hold `rank` entries, `strides` (bytes) rank - 1.
+// `inline`, not `static`: the cache is one object for the whole library, whichever file calls it.
+// Returns false when the driver cannot encode the map.
+constexpr int TMAP_CACHE = 128;
 
-static inline PFN_encodeTiled get_encode_fn() {
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
+inline bool tensor_map(CUtensorMap *out, const void *base, CUtensorMapDataType dtype, int rank, const cuuint64_t *dims,
+                       const cuuint64_t *strides, const cuuint32_t *box, CUtensorMapSwizzle swizzle) {
+    typedef CUresult (*Encode)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                               const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    struct Entry { uint64_t key[12]; CUtensorMap map; };
+    static std::mutex mu;
+    static Entry cache[TMAP_CACHE];
+    static int n_cached = 0, next = 0;
+    static Encode encode = nullptr;
+    if (rank < 1 || rank > 3) return false;
+    uint64_t key[12] = {(uint64_t)(uintptr_t)base, (uint64_t)dtype, (uint64_t)rank, (uint64_t)swizzle};
+    for (int i = 0; i < rank; ++i) { key[4 + i] = dims[i]; key[7 + i] = box[i]; }
+    for (int i = 0; i + 1 < rank; ++i) key[10 + i] = strides[i];
+    std::lock_guard<std::mutex> g(mu);
+    for (int i = 0; i < n_cached; ++i)
+        if (memcmp(cache[i].key, key, sizeof(key)) == 0) { *out = cache[i].map; return true; }
+    if (!encode) {
         void *p = nullptr;
         cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = (PFN_encodeTiled)p;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            return false;
+        encode = (Encode)p;
     }
-    return fn;
+    const cuuint32_t estr[3] = {1u, 1u, 1u};
+    CUtensorMap m;
+    if (encode(&m, dtype, (cuuint32_t)rank, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        return false;
+    memcpy(cache[next].key, key, sizeof(key));
+    cache[next].map = m;
+    next = (next + 1) % TMAP_CACHE;
+    if (n_cached < TMAP_CACHE) ++n_cached;
+    *out = m;
+    return true;
 }
 
-// 3-D tensor map {inner, rows, batch} with box {box_inner, box_rows, 1}, SWIZZLE_128B (box_inner * elem = 128 bytes)
-static inline bool make_map_3d(CUtensorMap *tm, CUtensorMapDataType dt, size_t elem, void *base, uint64_t inner, uint64_t rows,
-                               uint64_t batch, uint64_t row_stride_bytes, uint64_t batch_stride_bytes, uint32_t box_inner,
-                               uint32_t box_rows) {
-    PFN_encodeTiled enc = get_encode_fn();
-    if (!enc) return false;
-    cuuint64_t gdim[3] = {inner, rows, batch};
-    cuuint64_t gstr[2] = {row_stride_bytes, batch_stride_bytes};
-    cuuint32_t box[3] = {box_inner, box_rows, 1u};
-    cuuint32_t estr[3] = {1u, 1u, 1u};
-    (void)elem;
-    return enc(tm, dt, 3, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+// bf16 3-D tensor map {inner, rows, batch} with box {64, box_rows, 1}, SWIZZLE_128B (64 bf16 = 128 bytes)
+inline bool tensor_map_bf16_3d(CUtensorMap *out, const void *base, uint64_t inner, uint64_t rows, uint64_t batch,
+                               uint64_t row_stride_bytes, uint64_t batch_stride_bytes, uint32_t box_rows) {
+    const cuuint64_t dims[3] = {inner, rows, batch}, strides[2] = {row_stride_bytes, batch_stride_bytes};
+    const cuuint32_t box[3] = {64u, box_rows, 1u};
+    return tensor_map(out, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 }  // namespace xqtc

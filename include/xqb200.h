@@ -206,6 +206,8 @@ int xq_usage_ema_dev(float *ema, const float *hit, int rows, int V, int64_t *rec
 int xq_vit_residual_ln_fwd(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
                            const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
                            int M, int D, float *x_out, void *y, float *mean, float *rstd, void *stream);
+/* workspace of xq_vit_residual_ln_bwd on the current device; 0 when the device cannot be queried (the cause is in
+ * xq_last_cuda_error()), and xq_vit_residual_ln_bwd refuses a workspace that small */
 size_t xq_vit_ln_bwd_workspace_bytes(int D);
 /*   G = g_xout + LayerNorm^T(g_y)  -> g_x [M,D] fp32 ; g_branch = G * rowscale * ls_gamma (bf16)
  *   g_ln_w, g_ln_b, g_ls_gamma, g_branch_bias [D] overwritten (any may be NULL) */

@@ -249,19 +249,43 @@ def test_more_column_blocks_than_sms_is_refused_without_writing():
     assert bool(d_bias.isnan().all()), "a refused call zeroed d_bias"
 
 
+def _attn_check(qkv, g):
+    """xq_vit_attn_fwd / _bwd on qkv [1, N, 192] (one head) against fp32 autograd, at tests/test_gpu_attn.py's tolerances"""
+    from imagefolder_b200 import vit_ops
+    q32 = qkv.float().requires_grad_(True)
+    q, k, v = q32.view(1, -1, 3, 64).unbind(2)
+    s = (q @ k.transpose(-1, -2)) * 0.125
+    o_ref = torch.softmax(s, -1) @ v
+    (o_ref * g.float()).sum().backward()
+    out, lse2 = vit_ops.attn_tc_forward(qkv, 1)
+    dqkv = vit_ops.attn_tc_backward(qkv, out, lse2, g, 1)
+    assert (out.float() - o_ref).abs().max().item() <= 8e-3 * max(1.0, o_ref.abs().max().item())
+    gr, d = q32.grad.view(-1, 3, 64), dqkv.float().view(-1, 3, 64)
+    for i in range(3):
+        assert (d[:, i] - gr[:, i]).abs().max().item() <= 1e-2 * max(1e-3, gr[:, i].abs().max().item())
+
+
 def test_tensor_map_cache_eviction_and_reuse():
-    """gm_get_maps keeps 32 (A, B, M, N, K) -> tensor-map entries, replaced round-robin.  36 calls with distinct (pointer, M)
-    (72 entries, forward and backward) wrap it twice; then the first combination again, and the same buffers with a smaller
-    M.  A map reused for the wrong M would read the nonzero rows after M, which changes the bias gradient."""
+    """One cache of 128 tensor maps (xqtc::tensor_map, round-robin) serves the GEMMs, the attention kernels and the VQ
+    search.  Each of 64 distinct (pointer, M) GEMM combinations adds two maps (the A operands of the forward and the
+    backward call), and an attention forward + backward on a fresh slice of a qkv buffer, interleaved after it, adds three
+    more: 320 new maps wrap the cache twice, and the GEMMs' B maps and the attention maps evict one another.  Then the first
+    combination again, and the same buffers with a smaller M.  A map reused for the wrong M would read the nonzero rows
+    after M, which changes the bias gradient; a stale attention map would read another slice."""
     N, K = 256, 128
     gen = torch.Generator(device="cuda").manual_seed(4)
-    combos = [(8 * i, 37 + 11 * i) for i in range(36)]          # (row offset, M)
+    combos = [(8 * i, 37 + 11 * i) for i in range(64)]          # (row offset, M)
     rows = max(o + m for o, m in combos) + GUARD
     x, d_out = _grid(rows, K, 2 ** -3, gen), _grid(rows, K, 2 ** -3, gen)
     w1, w2t = _grid(N, K, 2 ** -2, gen), _grid(N, K, 2 ** -2, gen)
     b1 = _bias(N, gen)
-    for off, M in combos + [combos[0], (combos[0][0], combos[0][1] - 30), (combos[-1][0], 5)]:
+    S = 128                                                      # attention sequence length
+    qkv = torch.randn(8 * len(combos) + S, 3 * 64, device="cuda", generator=gen).to(torch.bfloat16)
+    g = torch.randn(8 * len(combos) + S, 64, device="cuda", generator=gen).to(torch.bfloat16)
+    for i, (off, M) in enumerate(combos + [combos[0], (combos[0][0], combos[0][1] - 30), (combos[-1][0], 5)]):
         _check(x[off:], w1, b1, d_out[off:], w2t, M, N, K)
+        j = 8 * (i % len(combos))
+        _attn_check(qkv[j:j + S].unsqueeze(0), g[j:j + S].unsqueeze(0))
 
 
 def _mlp(C, H, O, seed):
