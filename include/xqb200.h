@@ -362,6 +362,25 @@ int xq_adamw_step(float *const *param, const float *const *grad, float *const *e
                   const int64_t *numel, const double *step_size, const double *bc2_sqrt, int n, double wd_factor,
                   double one_minus_beta1, double beta2, double one_minus_beta2, double eps, void *stream);
 
+/* ---- reconstruction metrics: PSNR and SSIM per image (csrc/metric_kernels.cu) ---------------------------------------------
+ * Replaces the scikit-image calls of the reference's reconstruction evaluation (tokenizer/vqgan/reconstruction_vqgan_ddp.py:
+ * 155-169), per image b of rec [B,C,H,W] (the clamped reconstruction, fp32, or bf16 when rec_is_bf16) and x [B,C,H,W] fp32 (the
+ * model input in [-1, 1]):
+ *   g = (x + 1) / 2 ;  r = uint8(clamp(127.5 * rec + 128, 0, 255)) / 255                   (fp32)
+ *   psnr[b] = peak_signal_noise_ratio(r, g)                     10 log10(1 / mse), mse in fp64; +inf when mse == 0
+ *   ssim[b] = structural_similarity(r, g, data_range=2.0, channel_axis=-1)
+ *             7x7 uniform window, sample covariance, K1 = 0.01, K2 = 0.03; per channel the fp64 mean of S over the windows
+ *             inside the image, then the mean over channels
+ * psnr, ssim: fp64 device arrays [B].  Deterministic (fixed-order fp64 reductions, no atomics).  C >= 1, H, W >= 7; the
+ * workspace (16-byte aligned) holds two fp64 partials per (image, channel, strip of XQ_METRIC_STRIP_ROWS rows, column tile).
+ * XQ_ERR_ARG (a bad size or flag, a NULL or misaligned pointer) and XQ_ERR_WORKSPACE are returned before anything is written.
+ * ------------------------------------------------------------------------------------------------------------------------------ */
+#define XQ_METRIC_STRIP_ROWS 32
+/* 0 when an argument is out of range */
+size_t xq_recon_psnr_ssim_workspace_bytes(int B, int C, int H, int W);
+int xq_recon_psnr_ssim(const void *rec, int rec_is_bf16, const float *x, int B, int C, int H, int W, double *psnr, double *ssim,
+                       void *ws, size_t ws_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
