@@ -1,4 +1,5 @@
-// gemm_kernel.cu -- hand-written wgmma GEMM (sm_90a) with the ViT MLP's element-wise work fused into its epilogue.
+// gemm_kernel.cu -- hand-written wgmma GEMM (sm_90a) with the ViT MLP's element-wise work fused in, run by an epilogue
+// warpgroup beside the tensor cores.
 //
 // Path: timm `Mlp.forward` inside `Block.forward`, tokenizer/tokenizer_image/dino_enc/vision_transformer.py:336-339
 //   h = GELU(fc1(y)) ; branch = fc2(h)        and its backward.
@@ -8,10 +9,20 @@
 // (the other four GEMMs of the block -- fc2 forward, the two weight gradients, the fc1 input gradient -- stay plain cuBLAS calls).
 //
 // C[M,N] = A[M,K] . B[N,K]^T, A and B K-major (row-major as PyTorch stores activations and Linear weights), bf16 in, fp32
-// accumulation in registers.  A CTA owns a 128 x 128 tile: two consumer warpgroups, each `wgmma.m64n128k16` over its 64 rows,
-// K = 64 per stage, GM_NST-stage TMA ring of 32 KB; one producer warp issues the TMA loads.  Persistent: CTA p keeps column
-// block p % (N/128) for the whole kernel (bias slice in shared memory, bias-gradient sums in registers, the weight tile hot in
-// L2) and walks the 128-row blocks.
+// accumulation in registers.  A CTA owns a 128 x 128 tile and is persistent: CTA p keeps column block p % (N/128) for the whole
+// kernel (bias slice and bias-gradient sums in registers, the weight tile hot in L2) and walks the 128-row blocks.  Roles
+// (416 threads):
+//   warps 0-7    two MMA warpgroups, `wgmma.m64n128k16` over 64 rows each, K = 64 per stage of a GM_NST-stage TMA ring of
+//                32 KB.  After a tile's K loop they round the accumulators to bf16, write them with `stmatrix` into the staging
+//                tile in shared memory and start the next tile's K loop: they touch no global memory.
+//   warps 8-11   the epilogue warpgroup: works on the staged tile with 16-byte shared-memory accesses while the MMA groups
+//                run the next tile, and moves every output with TMA stores (rows >= M are clipped by the tensor map).
+//   warp 12      TMA producer: the A / B ring and, in the backward, the stored `pre` tile of each output tile.
+// Shared memory: ring 4 x 32 KB, one staging tile, two auxiliary tiles (32 KB each: two [128][64] SWIZZLE_128B row tiles, the
+// layout of a TMA box), 224 KB in all.
+// One H100 80GB HBM3 at a 700 W power limit, 1980 MHz max SM clock, M = 65 664, N = 3072, K = 768 (tools/mlp_gemm_bench.py):
+// forward 0.700 ms (443 TFLOP/s), backward 0.750 ms (413 TFLOP/s); library GEMM + stand-alone kernel 0.723 / 0.919 ms.  The MMA
+// warps spend 96 % / 94 % of a tile's clocks in the K loop (tools/mlp_gemm_clocks.py).
 #include "xq_common.cuh"
 #include "xq_tc.cuh"
 #include "xq_gelu.cuh"
@@ -23,45 +34,95 @@ using xqv::dgelu_f;
 using xqv::gelu_f;
 
 constexpr int GM_BM = 128, GM_BN = 128, GM_BK = 64;
-constexpr int GM_THREADS = 9 * 32;                             // 2 consumer warpgroups + 1 producer warp
-constexpr int GM_NST = 5;
+constexpr int GM_THREADS = 13 * 32;                            // 2 MMA warpgroups + 1 epilogue warpgroup + 1 producer warp
+constexpr int GM_NST = 4;
 constexpr int GM_A_BYTES = GM_BM * GM_BK * 2;                  // 16 KB
 constexpr int GM_ST_BYTES = GM_A_BYTES + GM_BN * GM_BK * 2;    // A 128 x 64 + B 128 x 64
-constexpr int GM_BAR_OFF = GM_NST * GM_ST_BYTES;
-constexpr int GM_BIAS_OFF = GM_BAR_OFF + 256;
-constexpr int GM_SMEM = GM_BIAS_OFF + GM_BN * 4 + 1024;
+constexpr int GM_HALF_BYTES = GM_BM * 64 * 2;                  // one [128][64] row tile: 64 columns of an output tile
+constexpr int GM_TILE_BYTES = 2 * GM_HALF_BYTES;
+constexpr int GM_STG_OFF = GM_NST * GM_ST_BYTES;
+constexpr int GM_AUX_OFF = GM_STG_OFF + GM_TILE_BYTES;
+constexpr int GM_BAR_OFF = GM_AUX_OFF + 2 * GM_TILE_BYTES;
+constexpr int GM_SMEM = GM_BAR_OFF + 256 + 1024;
 
-// EPI 1: forward  -- C = pre-activation (bf16), C2 = GELU(pre + bias) (bf16).
-// EPI 2: backward -- the accumulator is d_act; C = d_act * GELU'(X + bias) with X (= C2 argument) the stored pre-activation;
-//                    column sums of the ROUNDED result -> dbias (fp32 atomics, one per column per CTA at the end).
-// Both epilogues apply the element-wise function to the ROUNDED bf16 value of the GEMM result, i.e. exactly what the stand-alone
+__device__ __forceinline__ void stmatrix_x4(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+                 : "memory");
+}
+__device__ __forceinline__ uint4 lds128(uint32_t saddr) {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
+    return v;
+}
+
+// Per-role clock counters, compiled in with -DXQ_GM_CLOCKS only (tools/mlp_gemm_clocks.py); otherwise every call is empty.
+// Thread 0 (first MMA warp) and the first epilogue thread of every CTA each add their laps to gm_clocks[EPI - 1][slot].
+enum { GM_CLK_KLOOP, GM_CLK_MMA_WAIT, GM_CLK_HANDOFF, GM_CLK_EPI_WAIT, GM_CLK_EPI_WORK, GM_CLK_TILES, GM_CLK_SLOTS };
+#ifdef XQ_GM_CLOCKS
+__device__ unsigned long long gm_clocks[2][GM_CLK_SLOTS];
+struct GmClock {
+    long long t, acc[GM_CLK_SLOTS] = {};
+    __device__ void start() { t = clock64(); }
+    __device__ void lap(int slot) { const long long n = clock64(); acc[slot] += n - t; t = n; }
+    __device__ void count(int slot) { ++acc[slot]; }
+    __device__ void flush(int epi) {
+        for (int i = 0; i < GM_CLK_SLOTS; ++i)
+            if (acc[i]) atomicAdd(&gm_clocks[epi - 1][i], (unsigned long long)acc[i]);
+    }
+};
+#else
+struct GmClock {
+    __device__ void start() {}
+    __device__ void lap(int) {}
+    __device__ void count(int) {}
+    __device__ void flush(int) {}
+};
+#endif
+
+// EPI 1: forward  -- the staged tile is the pre-activation: TMA-stored as it stands (tmP); GELU(pre + bias) -> tmO.
+// EPI 2: backward -- the staged tile is d_act; the producer loads the stored pre-activation tile (tmP);
+//                    d_act * GELU'(pre + bias) -> tmO; column sums of the ROUNDED result -> dbias (fp32 atomics at the end).
+// Both apply the element-wise function to the ROUNDED bf16 value of the GEMM result, i.e. exactly what the stand-alone
 // kernels compute from the tensor a library GEMM would have written.
+//
+// Barriers: full / empty per ring stage; stg_full (the 8 MMA warps have written the staging tile) / stg_empty (the epilogue
+// is done with it); aux_full / aux_empty per auxiliary tile (backward: the `pre` tile has landed / its store has been read).
 template <int EPI>
 __global__ void __launch_bounds__(GM_THREADS, 1)
-mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, __nv_bfloat16 *__restrict__ C,
-                __nv_bfloat16 *__restrict__ C2, const float *__restrict__ bias, float *__restrict__ dbias, int M, int N, int K) {
+mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmO, const float *__restrict__ bias,
+                float *__restrict__ dbias, int M, int N, int K) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t *stg = base + GM_STG_OFF;
     uint64_t *bars = (uint64_t *)(base + GM_BAR_OFF);
-    uint64_t *full = bars, *empty = bars + GM_NST;
-    float *sbias = (float *)(base + GM_BIAS_OFF);
+    uint64_t *full = bars, *empty = bars + GM_NST, *stg_full = bars + 2 * GM_NST, *stg_empty = stg_full + 1;
+    uint64_t *aux_full = stg_full + 2, *aux_empty = stg_full + 4;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (tid == 0) {
-        // empty: one arrival per consumer warp
+        // empty, stg_full: one arrival per MMA warp; stg_empty, aux_empty: the first epilogue thread
         for (int i = 0; i < GM_NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
+        mbar_init(stg_full, 8);
+        mbar_init(stg_empty, 1);
+        for (int i = 0; i < 2; ++i) { mbar_init(&aux_full[i], 1); mbar_init(&aux_empty[i], 1); }
         mbar_fence_init();
     }
-    // schedule: CTA p keeps column block nb, walks 128-row blocks mb0, mb0 + mstep, ...
+    // schedule: CTA p keeps column block nb, walks 128-row blocks mb0, mb0 + mstep, ...; t counts its tiles
     const int nN = N / GM_BN, nM = (M + GM_BM - 1) / GM_BM, nk = K / GM_BK;
     const int nb = blockIdx.x % nN, mstep = gridDim.x / nN, mb0 = blockIdx.x / nN;
-    for (int i = tid; i < GM_BN; i += GM_THREADS) sbias[i] = bias[nb * GM_BN + i];
     __syncthreads();
-    if (warp == 8) {
+    GmClock clk;
+    if (warp == 12) {
         // ===== TMA producer (whole warp runs the loop, one elected lane issues) =====
-        if (elect_one()) { tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); }
+        if (elect_one()) {
+            tma_prefetch_desc(&tmA);
+            tma_prefetch_desc(&tmB);
+            if (EPI == 2) tma_prefetch_desc(&tmP);
+        }
         __syncwarp();
-        int it = 0;
-        for (int mb = mb0; mb < nM; mb += mstep) {
+        int it = 0, t = 0;
+        for (int mb = mb0; mb < nM; mb += mstep, ++t) {
+            bool pre_sent = false;
             for (int kb = 0; kb < nk; ++kb, ++it) {
                 const int st = it % GM_NST;
                 mbar_wait(&empty[st], ((it / GM_NST) & 1) ^ 1);
@@ -71,18 +132,141 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     tma_load_3d(base + st * GM_ST_BYTES + GM_A_BYTES, &tmB, kb * GM_BK, nb * GM_BN, 0, &full[st]);
                 }
                 __syncwarp();
+                // backward: the stored pre-activation tile goes to the auxiliary tile as soon as the epilogue has released it
+                // (polled once per K step, so that the ring is not held up), at the latest with the tile's last K step;
+                // rows >= M are zero-filled
+                if (EPI == 2 && !pre_sent) {
+                    uint64_t *e = &aux_empty[t & 1];
+                    const uint32_t par = ((t >> 1) & 1) ^ 1;
+                    if (kb == nk - 1) mbar_wait(e, par);
+                    else if (!__any_sync(0xffffffffu, mbar_test(e, par))) continue;
+                    uint8_t *aux = base + GM_AUX_OFF + (t & 1) * GM_TILE_BYTES;
+                    if (elect_one()) {
+                        mbar_expect_tx(&aux_full[t & 1], GM_TILE_BYTES);
+                        tma_load_3d(aux, &tmP, nb * GM_BN, mb * GM_BM, 0, &aux_full[t & 1]);
+                        tma_load_3d(aux + GM_HALF_BYTES, &tmP, nb * GM_BN + 64, mb * GM_BM, 0, &aux_full[t & 1]);
+                    }
+                    __syncwarp();
+                    pre_sent = true;
+                }
             }
         }
         return;
     }
-    // ===== consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of each tile =====
-    const int wg = warp >> 2, wq = warp & 3;
-    const int rq = wq * 16 + (lane >> 2), cq = 2 * (lane & 3);   // fragment row (and row + 8), first column of each 8-column group
-    float bsum[GM_BN / 8][2];
+    if (warp >= 8) {
+        // ===== epilogue warpgroup: thread te owns the 8 columns of 16-byte unit uc in rows rg, rg + 8, ..., rg + 120 =====
+        const int te = tid - 8 * 32, uc = te & 15, rg = te >> 4;
+        const uint32_t ubase = (uint32_t)((uc >> 3) * GM_HALF_BYTES);
+        float b[8], bsum[8];
 #pragma unroll
-    for (int j = 0; j < GM_BN / 8; ++j) bsum[j][0] = bsum[j][1] = 0.f;
-    int it = 0;
-    for (int mb = mb0; mb < nM; mb += mstep) {
+        for (int e = 0; e < 8; ++e) { b[e] = bias[nb * GM_BN + 8 * uc + e]; bsum[e] = 0.f; }
+        clk.start();
+        int t = 0;
+        for (int mb = mb0; mb < nM; mb += mstep, ++t) {
+            uint8_t *aux = base + GM_AUX_OFF + (t & 1) * GM_TILE_BYTES;
+            mbar_wait(stg_full, t & 1);
+            if (EPI == 1) {
+                if (te == 0) {
+                    tma_store_3d(&tmP, stg, nb * GM_BN, mb * GM_BM, 0);
+                    tma_store_3d(&tmP, stg + GM_HALF_BYTES, nb * GM_BN + 64, mb * GM_BM, 0);
+                    bulk_commit();
+                }
+            } else {
+                mbar_wait(&aux_full[t & 1], (t >> 1) & 1);
+            }
+            clk.lap(GM_CLK_EPI_WAIT);
+            // bias-gradient sums of the tile's 16 rows as a binary tree (lvl[l]: a finished subtree of 2^l rows), so a term passes
+            // through 4 adds here and one per tile below, whatever M is
+            float lvl[4][8];
+            // UB 16-byte units at a time: their loads, then 8 UB independent elements of arithmetic for the warp's one scheduler
+            // slot to interleave, then their stores (the backward holds twice the operands and the sum tree: half the batch)
+            constexpr int UB = EPI == 1 ? 4 : 2;
+#pragma unroll
+            for (int ib = 0; ib < 16 / UB; ++ib) {
+                uint32_t off[UB];
+                uint4 gq[UB], xq4[UB];
+#pragma unroll
+                for (int u = 0; u < UB; ++u) {
+                    off[u] = ubase + rowtile_unit(rg + 8 * (UB * ib + u), uc & 7);
+                    gq[u] = lds128(smem_u32(stg) + off[u]);
+                    if (EPI == 2) xq4[u] = lds128(smem_u32(aux) + off[u]);
+                }
+                // a quarter of a tile after the previous tile's store was issued: it has read its auxiliary tile, which the
+                // producer may now fill with the next tile's pre-activations
+                if (EPI == 2 && ib == 4 / UB && te == 0 && t > 0) { bulk_wait_read<0>(); mbar_arrive(&aux_empty[(t - 1) & 1]); }
+#pragma unroll
+                for (int u = 0; u < UB; ++u) {
+                    const int i = UB * ib + u;
+                    const uint32_t g[4] = {gq[u].x, gq[u].y, gq[u].z, gq[u].w};
+                    uint32_t o[4];
+                    if (EPI == 1) {
+#pragma unroll
+                        for (int w = 0; w < 4; ++w) {
+                            const float g0 = __uint_as_float(g[w] << 16), g1 = __uint_as_float(g[w] & 0xffff0000u);
+                            o[w] = pack_bf16(gelu_f(g0 + b[2 * w]), gelu_f(g1 + b[2 * w + 1]));
+                        }
+                    } else {
+                        // d_act rounded to bf16 first: the stand-alone kernel reads the bf16 tensor a library GEMM wrote.
+                        // Rows >= M: the zero-filled A rows give d_act = 0, so they add nothing to the bias gradient.
+                        const uint32_t x[4] = {xq4[u].x, xq4[u].y, xq4[u].z, xq4[u].w};
+                        float v[8];
+#pragma unroll
+                        for (int w = 0; w < 4; ++w) {
+                            const float g0 = __uint_as_float(g[w] << 16), g1 = __uint_as_float(g[w] & 0xffff0000u);
+                            const float d0 = dgelu_f(__uint_as_float(x[w] << 16) + b[2 * w]);
+                            const float d1 = dgelu_f(__uint_as_float(x[w] & 0xffff0000u) + b[2 * w + 1]);
+                            o[w] = pack_bf16(g0 * d0, g1 * d1);
+                            v[2 * w] = __uint_as_float(o[w] << 16);
+                            v[2 * w + 1] = __uint_as_float(o[w] & 0xffff0000u);
+                        }
+#pragma unroll
+                        for (int l = 0; l <= 4; ++l) {
+                            if (l == 4) {
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) bsum[e] += v[e];
+                            } else if ((i >> l) & 1) {
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) v[e] = lvl[l][e] + v[e];
+                            } else {
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) lvl[l][e] = v[e];
+                                break;
+                            }
+                        }
+                    }
+                    gq[u] = make_uint4(o[0], o[1], o[2], o[3]);
+                }
+#pragma unroll
+                for (int u = 0; u < UB; ++u) sts128(smem_u32(aux) + off[u], gq[u]);
+            }
+            fence_async_smem();
+            asm volatile("bar.sync 1, 128;" ::: "memory");       // the output tile is complete, the staging tile read
+            if (te == 0) {
+                tma_store_3d(&tmO, aux, nb * GM_BN, mb * GM_BM, 0);
+                tma_store_3d(&tmO, aux + GM_HALF_BYTES, nb * GM_BN + 64, mb * GM_BM, 0);
+                bulk_commit();
+                // forward: every store but the one just issued has read its tile -- this tile's `pre` (the staging tile) and
+                // the previous tile's `act` (the auxiliary tile the next tile writes)
+                if (EPI == 1) bulk_wait_read<1>();
+                mbar_arrive(stg_empty);
+            }
+            clk.lap(GM_CLK_EPI_WORK);
+        }
+        if (te == 0) { bulk_wait<0>(); clk.flush(EPI); }
+        if (EPI == 2) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) atomicAdd(dbias + nb * GM_BN + 8 * uc + e, bsum[e]);
+        }
+        return;
+    }
+    // ===== MMA warpgroup wg: rows 64 wg .. 64 wg + 63 of each tile =====
+    const int wg = warp >> 2, wq = warp & 3;
+    // stmatrix.x4 writes four 8 x 8 matrices whose row addresses come from lanes 8 i .. 8 i + 7: rows 0-7 and 8-15 of the
+    // warp's 16 for column group 2 jj (i = 0, 1) and for column group 2 jj + 1 (i = 2, 3) -- accumulators 8 jj .. 8 jj + 7
+    const int srow = wg * 64 + wq * 16 + (lane & 15);
+    clk.start();
+    int it = 0, t = 0;
+    for (int mb = mb0; mb < nM; mb += mstep, ++t) {
         float acc[64];
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -104,52 +288,22 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         wgmma_wait<0>();
         fence_regs(acc);
         if (lane == 0) mbar_arrive(&empty[prev]);
-        const int r0 = mb * GM_BM + wg * 64 + rq;
-        const bool ok0 = r0 < M, ok1 = r0 + 8 < M;
-        __nv_bfloat16 *c0 = C + (size_t)r0 * N + nb * GM_BN, *c1 = c0 + (size_t)8 * N;
-        __nv_bfloat16 *x0 = C2 + (size_t)r0 * N + nb * GM_BN, *x1 = x0 + (size_t)8 * N;
+        if (tid == 0) clk.lap(GM_CLK_KLOOP);
+        mbar_wait(stg_empty, (t & 1) ^ 1);                       // the epilogue is done with the previous tile
+        if (tid == 0) clk.lap(GM_CLK_MMA_WAIT);
 #pragma unroll
-        for (int j = 0; j < GM_BN / 8; ++j) {
-            const int col = 8 * j + cq;
-            const float b0 = sbias[col], b1 = sbias[col + 1];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {                        // h = 0: row r0, h = 1: row r0 + 8
-                const bool ok = h ? ok1 : ok0;
-                const uint32_t g = pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-                const float g0 = __uint_as_float(g << 16), g1 = __uint_as_float(g & 0xffff0000u);
-                if (EPI == 1) {
-                    const uint32_t a = pack_bf16(gelu_f(g0 + b0), gelu_f(g1 + b1));
-                    if (ok) {
-                        *reinterpret_cast<uint32_t *>((h ? c1 : c0) + col) = g;
-                        *reinterpret_cast<uint32_t *>((h ? x1 : x0) + col) = a;
-                    }
-                } else {
-                    // d_act rounded to bf16 first: the stand-alone kernel reads the bf16 tensor a library GEMM wrote.
-                    // Rows >= M: the zero-filled A rows give d_act = 0, so they add nothing to the bias gradient.
-                    const uint32_t xs = ok ? *reinterpret_cast<const uint32_t *>((h ? x1 : x0) + col) : 0u;
-                    const float d0 = dgelu_f(__uint_as_float(xs << 16) + b0), d1 = dgelu_f(__uint_as_float(xs & 0xffff0000u) + b1);
-                    const uint32_t o = pack_bf16(g0 * d0, g1 * d1);
-                    if (ok) *reinterpret_cast<uint32_t *>((h ? c1 : c0) + col) = o;
-                    bsum[j][0] += __uint_as_float(o << 16);
-                    bsum[j][1] += __uint_as_float(o & 0xffff0000u);
-                }
-            }
+        for (int jj = 0; jj < GM_BN / 16; ++jj) {
+            const int cg = 2 * jj + (lane >> 4);                 // 8-column group: unit cg % 8 of row tile cg / 8
+            stmatrix_x4(smem_u32(stg) + (cg >> 3) * GM_HALF_BYTES + rowtile_unit(srow, cg & 7),
+                        pack_bf16(acc[8 * jj], acc[8 * jj + 1]), pack_bf16(acc[8 * jj + 2], acc[8 * jj + 3]),
+                        pack_bf16(acc[8 * jj + 4], acc[8 * jj + 5]), pack_bf16(acc[8 * jj + 6], acc[8 * jj + 7]));
         }
+        fence_async_smem();                                      // forward: a TMA store reads the staging tile
+        __syncwarp();
+        if (lane == 0) mbar_arrive(stg_full);
+        if (tid == 0) { clk.lap(GM_CLK_HANDOFF); clk.count(GM_CLK_TILES); }
     }
-    if (EPI == 2) {
-        // column sums over the warp's 16 rows: lanes with equal lane % 4 hold the same columns
-#pragma unroll
-        for (int j = 0; j < GM_BN / 8; ++j) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                float v = bsum[j][e];
-                v += __shfl_xor_sync(0xffffffffu, v, 4);
-                v += __shfl_xor_sync(0xffffffffu, v, 8);
-                v += __shfl_xor_sync(0xffffffffu, v, 16);
-                if (lane < 4) atomicAdd(dbias + nb * GM_BN + 8 * j + cq + e, v);
-            }
-        }
-    }
+    if (tid == 0) clk.flush(EPI);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------
@@ -160,16 +314,19 @@ static int gm_check(const void *a, const void *b, const void *c, const void *c2,
     return XQ_OK;
 }
 
+// `pre` is the pre-activation tensor (written by the forward, read by the backward), `out` the epilogue's result (act / d_pre)
 template <int EPI>
-static int gm_launch(const void *a, const void *b, void *c, void *c2, const float *bias, float *dbias, int M, int N, int K,
+static int gm_launch(const void *a, const void *b, const void *pre, void *out, const float *bias, float *dbias, int M, int N, int K,
                      cudaStream_t st) {
     int sms = 0;
     if (int rc = sm_count(&sms)) return rc;
     const int nN = N / GM_BN;
     if (nN > sms) return XQ_ERR_UNSUPPORTED;
-    CUtensorMap tmA, tmB;
+    CUtensorMap tmA, tmB, tmP, tmO;
     if (!tensor_map_bf16_3d(&tmA, a, K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BM) ||
-        !tensor_map_bf16_3d(&tmB, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BN))
+        !tensor_map_bf16_3d(&tmB, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BN) ||
+        !tensor_map_bf16_3d(&tmP, pre, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM) ||
+        !tensor_map_bf16_3d(&tmO, out, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM))
         return XQ_ERR_UNSUPPORTED;
     if (int rc = smem_optin(mlp_gemm_kernel<EPI>, GM_SMEM)) return rc;
     const int nM = (M + GM_BM - 1) / GM_BM;
@@ -177,7 +334,7 @@ static int gm_launch(const void *a, const void *b, void *c, void *c2, const floa
     if (per_col > nM) per_col = nM;
     // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
     if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st));
-    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, (__nv_bfloat16 *)c, (__nv_bfloat16 *)c2, bias, dbias, M, N, K);
+    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, bias, dbias, M, N, K);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
     return XQ_OK;
 }
@@ -195,7 +352,17 @@ int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, co
                          int N, int K, void *stream) {
     if (int rc = xq::gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
     if (!d_bias) return XQ_ERR_ARG;
-    return xq::gm_launch<2>(d_out, w2t, d_pre, const_cast<void *>(pre), bias, d_bias, M, N, K, (cudaStream_t)stream);
+    return xq::gm_launch<2>(d_out, w2t, pre, d_pre, bias, d_bias, M, N, K, (cudaStream_t)stream);
 }
+
+#ifdef XQ_GM_CLOCKS
+// copies the counters ([forward, backward][GM_CLK_SLOTS]) to `out` and clears them
+int xq_gm_clocks_read(unsigned long long *out) {
+    XQ_CUDA_TRY(cudaMemcpyFromSymbol(out, xq::gm_clocks, sizeof(xq::gm_clocks)));
+    unsigned long long zero[2][xq::GM_CLK_SLOTS] = {};
+    XQ_CUDA_TRY(cudaMemcpyToSymbol(xq::gm_clocks, zero, sizeof(zero)));
+    return XQ_OK;
+}
+#endif
 
 }  // extern "C"

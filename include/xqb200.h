@@ -291,6 +291,9 @@ int xq_diffaug_backward(const float *g, const float *rand01, int B, int C, int H
  * All matrices row-major bf16; bias / d_bias fp32.  N % 128 == 0, N / 128 <= SM count, K % 64 == 0 (else XQ_ERR_UNSUPPORTED),
  * any M.  pre / act / d_pre apply the same device functions to the same rounded bf16 GEMM results as that two-call sequence
  * (equal up to the GEMM's fp32 accumulation order); d_bias is summed with fp32 atomics, in no fixed order.
+ * One kernel, three roles per CTA: MMA warpgroups that hand each 128 x 128 tile, rounded to bf16, to an epilogue warpgroup
+ * through shared memory and go on to the next tile; the epilogue warpgroup; a TMA producer warp.  pre / act / d_pre are
+ * written by TMA stores (and pre read by TMA loads in the backward), so they must be 16-byte aligned like the operands.
  *   x [M,K], w [N,K] (fc1.weight as bf16)  ->  pre [M,N] = x w^T ,  act [M,N] = GELU(pre + bias)                               */
 int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream);
 /*  d_out [M,K] (gradient of the fc2 output), w2t [N,K] (fc2.weight TRANSPOSED, bf16), pre [M,N] (saved by the forward)
