@@ -100,10 +100,6 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_residual_ln_bwd.restype = c_int
     L.xq_vit_residual_ln_bwd.argtypes = [f32p, vp, f32p, f32p, f32p, f32p, vp, f32p, f32p, f32p, c_int, c_int, c_int,
                                          f32p, vp, f32p, f32p, f32p, f32p, vp, c_size_t, vp]
-    L.xq_vit_pack_qkv.restype = c_int
-    L.xq_vit_pack_qkv.argtypes = [vp, vp, vp, vp, vp, c_size_t, c_int, vp, c_size_t, vp]
-    L.xq_vit_pack_workspace_bytes.restype = c_size_t
-    L.xq_vit_pack_workspace_bytes.argtypes = []
     L.xq_vit_patchify.restype = c_int
     L.xq_vit_patchify.argtypes = [f32p, vp, c_int, c_int, c_int, c_int, c_int, vp]
     L.xq_vit_assemble_fwd.restype = c_int
@@ -231,7 +227,7 @@ EXPORTED_SYMBOLS = [
     "xq_vq_backward", "xq_perturb_workspace_bytes", "xq_perturb_forward", "xq_perturb_backward",
     "xq_ms_workspace_bytes", "xq_ms_saved_bytes", "xq_ms_total_tokens", "xq_ms_forward", "xq_ms_backward",
     "xq_ms_decode", "xq_ms_embed", "xq_usage_ema", "xq_usage_ema_dev", "xq_vit_residual_ln_fwd", "xq_vit_ln_bwd_workspace_bytes",
-    "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_pack_qkv", "xq_vit_pack_workspace_bytes", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd",
+    "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
     "xq_ema_update", "xq_adamw_step", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",

@@ -421,108 +421,6 @@ __global__ void gelu_bwd_kernel(const uint4 *__restrict__ x, const float *__rest
     }
 }
 
-// dq, dk, dv: each [M, C] bf16 dense (what the SDPA backward returns for q/k/v views of a packed
-// [M, 3C] projection) -> dqkv [M, 3C], and (optionally) g_bias [3C] = column sums of dqkv = the gradient of the
-// qkv projection bias, which autograd would otherwise compute with one more full pass over dqkv.
-// Same TMA-bulk staged skeleton as residual_ln_bwd_kernel: warp 0 stages PACK_TR rows of the three sources per tile,
-// consumer warp w copies row w (a lane owns 16-byte column chunks j*32 + lane of the PACKED row) and keeps the column
-// sums in registers; one atomicAdd per column per CTA at the end (g_bias zeroed by the launcher).
-constexpr int PACK_TR = 8;
-constexpr int PACK_NST = 4;
-constexpr int PACK_NCH = 12;                 // 16-byte chunks per lane: 3*C/8 <= 384  (C <= 1024)
-constexpr int PACK_THREADS = (PACK_TR + 1) * 32;
-__global__ void __launch_bounds__(PACK_THREADS, 1)
-pack_qkv_kernel(const uint4 *__restrict__ dq, const uint4 *__restrict__ dk, const uint4 *__restrict__ dv,
-                uint4 *__restrict__ out, float *__restrict__ g_bias, int *__restrict__ counter, int M, int C8) {
-    constexpr int TR = PACK_TR, NST = PACK_NST;
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t full[NST], empty[NST];
-    __shared__ int tile_of[NST];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int ntiles = (M + TR - 1) / TR, per_row = 3 * C8;
-    const uint32_t src_row = (uint32_t)C8 * 16;                    // bytes of one source row
-    const size_t stage_bytes = (size_t)3 * TR * src_row;           // [3][TR][C8] uint4
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TR); }
-        mbar_fence_init();
-    }
-    __syncthreads();
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int it = 0;; ++it) {
-                const int st = it % NST;
-                mbar_wait_ptx(&empty[st], ((it / NST) & 1) ^ 1);
-                const int tile = it == 0 ? (int)blockIdx.x : (int)gridDim.x + atomicAdd(counter, 1);
-                tile_of[st] = tile;
-                if (tile >= ntiles) { mbar_arrive(&full[st]); break; }
-                const int r0 = tile * TR, nr = min(TR, M - r0);
-                unsigned char *dst = smem + st * stage_bytes;
-                mbar_expect_tx(&full[st], 3u * nr * src_row);
-                bulk_g2s(dst, dq + (size_t)r0 * C8, nr * src_row, &full[st]);
-                bulk_g2s(dst + (size_t)TR * src_row, dk + (size_t)r0 * C8, nr * src_row, &full[st]);
-                bulk_g2s(dst + (size_t)2 * TR * src_row, dv + (size_t)r0 * C8, nr * src_row, &full[st]);
-            }
-        }
-    } else {
-        const int cw = warp - 1;
-        float acc[PACK_NCH][8];
-#pragma unroll
-        for (int j = 0; j < PACK_NCH; ++j)
-#pragma unroll
-            for (int k = 0; k < 8; ++k) acc[j][k] = 0.f;
-        for (int it = 0;; ++it) {
-            const int st = it % NST;
-            mbar_wait_ptx(&full[st], (it / NST) & 1);
-            const int tile = tile_of[st];
-            if (tile >= ntiles) break;
-            const int row = tile * TR + cw;
-            if (row < M) {
-                const unsigned char *base = smem + st * stage_bytes + (size_t)cw * src_row;
-#pragma unroll
-                for (int j = 0; j < PACK_NCH; ++j) {
-                    const int c = j * 32 + lane;
-                    if (c < per_row) {
-                        const int which = c / C8, cc = c - which * C8;
-                        const uint4 v = *reinterpret_cast<const uint4 *>(base + (size_t)which * TR * src_row + (size_t)cc * 16);
-                        out[(size_t)row * per_row + c] = v;
-                        if (g_bias) {
-                            const __nv_bfloat162 *p = reinterpret_cast<const __nv_bfloat162 *>(&v);
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                float2 f = __bfloat1622float2(p[k]);
-                                acc[j][2 * k] += f.x; acc[j][2 * k + 1] += f.y;
-                            }
-                        }
-                    }
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[st]);
-        }
-        if (g_bias) {
-            asm volatile("bar.sync 1, %0;" ::"n"(PACK_TR * 32) : "memory");   // every consumer is past its last tile
-            float *red = reinterpret_cast<float *>(smem) + (size_t)cw * per_row * 8;
-#pragma unroll
-            for (int j = 0; j < PACK_NCH; ++j) {
-                const int c = j * 32 + lane;
-                if (c < per_row)
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) red[c * 8 + k] = acc[j][k];
-            }
-        }
-    }
-    if (g_bias) {
-        __syncthreads();
-        const float *red = reinterpret_cast<const float *>(smem);
-        for (int e = threadIdx.x; e < per_row * 8; e += blockDim.x) {
-            float t = 0.f;
-#pragma unroll
-            for (int w = 0; w < TR; ++w) t += red[(size_t)w * per_row * 8 + e];
-            atomicAdd(g_bias + e, t);
-        }
-    }
-}
-
 // Patch embedding as a GEMM (timm PatchEmbed: Conv2d(kernel = stride = p) -> flatten -> NLC, vision_transformer.py:
 // patch_embed): non-overlapping patches make im2col a pure permutation, so the conv is
 //   tokens[B*gh*gw, D] = patches[B*gh*gw, Cin*p*p] @ W[D, Cin*p*p]^T + b .
@@ -666,32 +564,6 @@ int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_
     reduce_parts_kernel<<<(D + 31) / 32, 256, 0, st>>>(part, grid, D, ls_gamma, branch_bias, g_ln_w, g_ln_b,
                                                         branch ? g_ls_gamma : nullptr, branch ? g_branch_bias : nullptr);
     XQ_LAUNCH_CHECK("reduce_parts_kernel");
-    return XQ_OK;
-}
-
-size_t xq_vit_pack_workspace_bytes(void) { return 256; }
-
-int xq_vit_pack_qkv(const void *dq, const void *dk, const void *dv, void *dqkv, float *g_bias, size_t M, int C,
-                    void *workspace, size_t workspace_bytes, void *stream) {
-    if (!dq || !dk || !dv || !dqkv || M == 0 || M > 0x7fffffffu || C <= 0 || (C & 7) || !workspace) return XQ_ERR_ARG;
-    if (workspace_bytes < 256) return XQ_ERR_WORKSPACE;
-    if (3 * (C / 8) > PACK_NCH * 32) return XQ_ERR_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int C8 = C / 8;
-    const int ntiles = (int)((M + PACK_TR - 1) / PACK_TR);
-    int grid = 0;
-    if (int rc = xq::sm_count(&grid)) return rc;
-    if (grid > ntiles) grid = ntiles;
-    size_t smem = (size_t)PACK_NST * 3 * PACK_TR * C8 * 16;
-    const size_t red = sizeof(float) * (size_t)PACK_TR * 3 * C8 * 8;
-    if (smem < red) smem = red;
-    if (int rc = xq::smem_optin(pack_qkv_kernel, smem)) return rc;
-    int *counter = (int *)workspace;     // dynamic tile counter, reset on the stream before each launch
-    XQ_CUDA_TRY(cudaMemsetAsync(counter, 0, sizeof(int), st));
-    if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, sizeof(float) * 3 * (size_t)C, st));
-    pack_qkv_kernel<<<grid, PACK_THREADS, smem, st>>>((const uint4 *)dq, (const uint4 *)dk, (const uint4 *)dv,
-                                                      (uint4 *)dqkv, g_bias, counter, (int)M, C8);
-    XQ_LAUNCH_CHECK("pack_qkv_kernel");
     return XQ_OK;
 }
 

@@ -5,8 +5,9 @@
    [+ residual] -> LayerScale -> DropPath -> add -> LayerNorm -> cast-to-bf16
 by ONE kernel (`xq_vit_residual_ln_fwd`), GELU by one bf16 kernel and attention by the wgmma / TMA flash
 kernels of csrc/attn_kernel.cu (`xq_vit_attn_fwd/bwd`, reading the packed qkv projection in place and writing d(qkv)
-in the packed layout); the projection GEMMs stay on cuBLAS.  Attention dropout > 0 (no shipped config) and head
-dims other than 64 use the SDPA library kernel.  The residual stream is fp32 and the GEMM operands bf16,
+in the packed layout); the projection GEMMs stay on cuBLAS.  Blocks the attention kernels do not cover (head dims other
+than 64, attention dropout > 0 in training, qk_norm; no shipped config) run the module's own Attention.forward for
+their attention.  The residual stream is fp32 and the GEMM operands bf16,
 which is what bf16 autocast gives the reference, so the numerics are the reference's.
 """
 from __future__ import annotations
@@ -200,13 +201,17 @@ def mlp_forward(mlp, y):
     return F.linear(h, mlp.fc2.weight)
 
 
-ATTN_TC_ENABLED = [True]      # the wgmma attention kernels (csrc/attn_kernel.cu); tools flip it to time the library path
+# The wgmma attention kernels (csrc/attn_kernel.cu).  False runs every block's attention through the module's own
+# Attention.forward.  bench.py reads it: while it is True, the benchmarked step must show the attention kernels.
+ATTN_TC_ENABLED = [True]
 
 
-def attn_tc_ok(qkv, num_heads: int, dropout_p: float) -> bool:
-    """xq_vit_attn_fwd/bwd cover what the shipped configs run: bf16, head_dim 64, no mask, attn_drop = 0."""
-    return (ATTN_TC_ENABLED[0] and qkv.is_cuda and qkv.dtype == torch.bfloat16 and dropout_p == 0.0
-            and qkv.shape[-1] == 3 * num_heads * 64)
+def attn_tc_ok(attn, y) -> bool:
+    """xq_vit_attn_fwd/bwd cover what the shipped configs run: bf16 CUDA tokens, head_dim 64, no qk_norm, no mask and
+    an attention dropout of 0 where it applies (training)."""
+    p = attn.attn_drop.p if attn.training else 0.0
+    return (ATTN_TC_ENABLED[0] and y.is_cuda and y.dtype == torch.bfloat16 and p == 0.0 and attn.head_dim == 64
+            and isinstance(attn.q_norm, nn.Identity) and isinstance(attn.k_norm, nn.Identity))
 
 
 def attn_tc_forward(qkv, num_heads: int):
@@ -247,130 +252,44 @@ def attn_tc_backward(qkv, out, lse2, g, num_heads: int, want_bias_grad: bool = F
     return (dqkv, db) if want_bias_grad else dqkv
 
 
-def _sdpa_packed(qkv, num_heads, dropout_p):
-    """q/k/v as strided views of the packed projection (no copies); returns the leaves and the library output."""
-    B, N, C3 = qkv.shape
-    hd = C3 // 3 // num_heads
-    with torch.enable_grad():
-        src = qkv.detach().view(B, N, 3, num_heads, hd)
-        q = src[:, :, 0].transpose(1, 2).requires_grad_(True)
-        k = src[:, :, 1].transpose(1, 2).requires_grad_(True)
-        v = src[:, :, 2].transpose(1, 2).requires_grad_(True)
-        out = F.scaled_dot_product_attention(q, k, v, dropout_p=dropout_p)
-    return q, k, v, out
-
-
-def _sdpa_packed_backward(inner, dims, g, want_bias_grad: bool):
-    """d(qkv) [B,N,3C] (+ its column sums = d(bias)) from the SDPA library backward and ONE pack kernel."""
-    q, k, v, out = inner
-    B, N, C = dims
-    H, hd = q.shape[1], q.shape[3]
-    g = g.reshape(B, N, H, hd).transpose(1, 2)
-    dq, dk, dv = torch.autograd.grad(out, (q, k, v), g)
-    dqkv = torch.empty(B, N, 3 * C, dtype=dq.dtype, device=dq.device)
-    flat = [t.transpose(1, 2) for t in (dq, dk, dv)]            # [B,N,H,hd]
-    db = None
-    if all(t.is_contiguous() for t in flat) and dq.dtype == torch.bfloat16:
-        if want_bias_grad:
-            db = torch.empty(3 * C, dtype=torch.float32, device=dq.device)
-        L = _lib()
-        ws = torch.empty(int(L.xq_vit_pack_workspace_bytes()), dtype=torch.uint8, device=dq.device)
-        _call("xq_vit_pack_qkv", 1, L.xq_vit_pack_qkv, _ptr(flat[0]), _ptr(flat[1]), _ptr(flat[2]), _ptr(dqkv),
-              _ptr(db) if db is not None else None, B * N, C, _ptr(ws), ws.numel(), _stream(dq.device),
-              nbytes=B * N * C * 12)
-    else:  # layout the library did not produce in our runs; keep correctness
-        torch.stack([t.reshape(B, N, C) for t in flat], dim=2, out=dqkv.view(B, N, 3, C))
-        if want_bias_grad:
-            db = dqkv.float().sum((0, 1))
-    return dqkv, db
-
-
-class _PackedAttention(torch.autograd.Function):
-    """softmax(q k^T / sqrt(d)) v on the packed projection qkv [B,N,3*H*hd] (vision_transformer.py:175-191).
-
-    The attention itself is the SDPA library kernel; this wrapper only removes the layout glue autograd
-    adds around it: q/k/v are strided views of the packed tensor (no copies in forward; the library
-    allocates the output in [B,N,H,hd] order so the head merge is a view) and the three gradients are
-    re-packed into d(qkv) by ONE vector kernel instead of stack + permute + contiguous."""
-
-    @staticmethod
-    def forward(ctx, qkv, num_heads: int, dropout_p: float):
-        B, N, C3 = qkv.shape
-        ctx.dims = (B, N, C3 // 3)
-        ctx.tc = attn_tc_ok(qkv, num_heads, dropout_p)
-        if ctx.tc:
-            qkv = qkv.contiguous()
-            out, lse2 = attn_tc_forward(qkv, num_heads)
-            ctx.save_for_backward(qkv, out, lse2)
-            ctx.heads = num_heads
-            return out
-        ctx.inner = _sdpa_packed(qkv, num_heads, dropout_p)
-        return ctx.inner[3].detach().transpose(1, 2).reshape(B, N, C3 // 3)
-
-    @staticmethod
-    def backward(ctx, g):
-        if ctx.tc:
-            qkv, out, lse2 = ctx.saved_tensors
-            return attn_tc_backward(qkv, out, lse2, g, ctx.heads), None, None
-        inner, ctx.inner = ctx.inner, None
-        dqkv, _ = _sdpa_packed_backward(inner, ctx.dims, g, False)
-        return dqkv, None, None
-
-
-def packed_attention(qkv, num_heads, dropout_p=0.0):
-    return _PackedAttention.apply(qkv, num_heads, dropout_p)
-
-
 class _QKVAttention(torch.autograd.Function):
-    """qkv = y W^T + b ; attention(qkv)   (vision_transformer.py:175-191) as ONE autograd node, so that the bias
-    gradient is the column sum the pack kernel already has in registers (no separate sum(0) pass over d(qkv)).
-    y [B,N,C] bf16, W [3C,C] / b [3C] fp32 parameters; GEMMs are library calls in bf16 (autocast semantics)."""
+    """qkv = y W^T (+ b) ; attention(qkv)   (vision_transformer.py:175-191) as ONE autograd node on the wgmma kernels, so that
+    the bias gradient is the column sum the attention backward already has in registers (no separate sum(0) pass over
+    d(qkv)).  y [B,N,C] bf16, W [3C,C] / b [3C] (or None) fp32 parameters; GEMMs are library calls in bf16 (autocast
+    semantics)."""
 
     @staticmethod
-    def forward(ctx, y, W, b, num_heads: int, dropout_p: float):
+    def forward(ctx, y, W, b, num_heads: int):
         B, N, C = y.shape
         Wb = W.to(torch.bfloat16)
-        qkv = torch.addmm(b.to(torch.bfloat16), y.reshape(B * N, C), Wb.t()).view(B, N, 3 * C)
-        ctx.dims = (B, N, C)
-        ctx.tc = attn_tc_ok(qkv, num_heads, dropout_p)
-        if ctx.tc:
-            out, lse2 = attn_tc_forward(qkv, num_heads)
-            ctx.save_for_backward(y, Wb, qkv, out, lse2)
-            ctx.heads = num_heads
-            return out
-        ctx.inner = _sdpa_packed(qkv, num_heads, dropout_p)
-        ctx.save_for_backward(y, Wb)
-        return ctx.inner[3].detach().transpose(1, 2).reshape(B, N, C)
+        y2 = y.reshape(B * N, C)
+        qkv = (torch.addmm(b.to(torch.bfloat16), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * C)
+        out, lse2 = attn_tc_forward(qkv, num_heads)
+        ctx.save_for_backward(y, Wb, qkv, out, lse2)
+        ctx.heads = num_heads
+        return out
 
     @staticmethod
     def backward(ctx, g):
-        B, N, C = ctx.dims
-        if ctx.tc:
-            y, Wb, qkv, out, lse2 = ctx.saved_tensors
-            if ctx.needs_input_grad[2]:
-                dqkv, db = attn_tc_backward(qkv, out, lse2, g, ctx.heads, want_bias_grad=True)
-            else:
-                dqkv, db = attn_tc_backward(qkv, out, lse2, g, ctx.heads), None
+        y, Wb, qkv, out, lse2 = ctx.saved_tensors
+        B, N, C = y.shape
+        if ctx.needs_input_grad[2]:
+            dqkv, db = attn_tc_backward(qkv, out, lse2, g, ctx.heads, want_bias_grad=True)
         else:
-            inner, ctx.inner = ctx.inner, None
-            y, Wb = ctx.saved_tensors
-            dqkv, db = _sdpa_packed_backward(inner, ctx.dims, g, ctx.needs_input_grad[2])
+            dqkv, db = attn_tc_backward(qkv, out, lse2, g, ctx.heads), None
         d2 = dqkv.view(B * N, 3 * C)
         dy = (d2 @ Wb).view(B, N, C) if ctx.needs_input_grad[0] else None
         dW = (d2.t() @ y.reshape(B * N, C)).float() if ctx.needs_input_grad[1] else None
-        return dy, dW, db, None, None
+        return dy, dW, db, None
 
 
 def attention_forward(attn, y):
-    """Attention.forward (vision_transformer.py:173-197) on the fused path (no qk_norm, no mask)."""
-    if not isinstance(attn.q_norm, nn.Identity) or not isinstance(attn.k_norm, nn.Identity):
-        return attn(y)
-    p = attn.attn_drop.p if attn.training else 0.0
-    if attn.qkv.bias is not None and y.dtype == torch.bfloat16:
-        o = _QKVAttention.apply(y, attn.qkv.weight, attn.qkv.bias, attn.num_heads, p)
-    else:
-        o = packed_attention(attn.qkv(y), attn.num_heads, p)
-    return F.linear(o, attn.proj.weight)      # the proj bias is folded into the next residual_ln
+    """Attention.forward (vision_transformer.py:173-197, no mask) -> (branch, bias to fold into the next residual_ln).
+    On the wgmma kernels the proj GEMM leaves its bias to the caller; otherwise the module's own forward, bias included."""
+    if not attn_tc_ok(attn, y):
+        return attn(y), None
+    o = _QKVAttention.apply(y, attn.qkv.weight, attn.qkv.bias, attn.num_heads)
+    return F.linear(o, attn.proj.weight), attn.proj.bias
 
 
 class _PatchEmbed(torch.autograd.Function):
@@ -521,10 +440,9 @@ def run_blocks(vit, x, attn_mask=None):
     branch = bias = gamma = rs = None
     for blk in vit.blocks:
         x, y = residual_ln(x, branch, bias, gamma, rs, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
-        plain_attn = isinstance(blk.attn.q_norm, nn.Identity) and isinstance(blk.attn.k_norm, nn.Identity)
-        a = attention_forward(blk.attn, y)
+        a, a_bias = attention_forward(blk.attn, y)
         g1 = blk.ls1.gamma if hasattr(blk.ls1, "gamma") else None
-        x, y = residual_ln(x, a, blk.attn.proj.bias if plain_attn else None, g1,
+        x, y = residual_ln(x, a, a_bias, g1,
                            _droppath_scale(blk.drop_path1, Bn, dev), blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
         branch = mlp_forward(blk.mlp, y)          # fc1 bias in the GELU epilogue / kernel; fc2 bias folded into the next residual_ln
         bias = blk.mlp.fc2.bias

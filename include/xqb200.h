@@ -216,12 +216,6 @@ int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_
                            const float *ls_gamma, const float *rowscale, int rows_per_sample, int M, int D, float *g_x,
                            void *g_branch, float *g_ln_w, float *g_ln_b, float *g_ls_gamma, float *g_branch_bias,
                            void *workspace, size_t workspace_bytes, void *stream);
-/*   gradient re-packing of the fused qkv projection (vision_transformer.py:175-176): dq, dk, dv [M,C] bf16
- *   dense -> dqkv [M,3C]; replaces autograd's stack + permute + contiguous copies.  g_bias [3C] fp32 (may be NULL)
- *   receives the column sums of dqkv = the gradient of the qkv bias (nn.Linear's backward `sum(0)` pass, fused). */
-size_t xq_vit_pack_workspace_bytes(void);
-int xq_vit_pack_qkv(const void *dq, const void *dk, const void *dv, void *dqkv, float *g_bias, size_t M, int C,
-                    void *workspace, size_t workspace_bytes, void *stream);
 /*   im2col of the patch embedding (timm PatchEmbed = Conv2d(kernel = stride = p), vision_transformer.py PatchEmbed.forward):
  *   x fp32 [B,Cin,H,W] -> patches bf16 [B*(H/p)*(W/p), Cin*p*p] (K index = (c*p + ky)*p + kx = the flattened conv
  *   weight), so that tokens = patches @ weight.view(D,-1)^T + bias is a plain GEMM.  p % 4 == 0, H % p == W % p == 0. */

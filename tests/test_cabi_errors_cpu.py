@@ -5,8 +5,7 @@ or kernel that failed, not whatever an earlier call left there.
 Runs only where no GPU is usable: every call gets valid sizes and non-null dummy pointers, so it passes its argument checks
 and fails at its first CUDA call.  Before each call another entry point records an unrelated failure (xq_vq_backward's
 gradient memset), so a call that does not record its own failure leaves that message behind and fails the check.  The
-workspace-size queries xq_lpips_workspace_bytes, xq_vit_pack_workspace_bytes and xq_img_workspace_bytes make no CUDA call
-and are not listed."""
+workspace-size queries xq_lpips_workspace_bytes and xq_img_workspace_bytes make no CUDA call and are not listed."""
 import pytest
 import torch
 
@@ -23,7 +22,6 @@ CALLS = [
      "residual_ln_fwd_kernel"),
     ("xq_vit_residual_ln_bwd", (None, None, P, P, P, None, None, None, None, None, 1, 8, 768, P, None, None, None, None,
                                 None, P, BIG, None), "cudaGetDevice"),
-    ("xq_vit_pack_qkv", (P, P, P, P, None, 16, 768, P, 256, None), "cudaGetDevice"),
     ("xq_vit_assemble_fwd", (P, 1, P, 2, 4, 8, 16, 1, P, None), "assemble_fwd_kernel"),
     ("xq_vit_assemble_bwd", (P, 2, 4, 8, 16, 1, P, 0, P, None), "assemble_bwd_kernel"),
     ("xq_vit_patchify", (P, P, 2, 3, 64, 64, 16, None), "patchify_kernel"),

@@ -1,7 +1,7 @@
 """Numerics of the ViT glue kernels against a plain PyTorch fp32 / fp64 reference of the same op
 (floating-point kernels: tolerance set by the bf16 operands, written per assertion).
 
-The persistent kernels (residual_ln_bwd, pack_qkv, gelu_bwd) hand out row tiles dynamically, so they are also run at row
+The persistent kernels (residual_ln_bwd, gelu_bwd) hand out row tiles dynamically, so they are also run at row
 counts where every CTA takes several tiles (the training encoder has 128 x 513 rows), through the C ABI with every output
 buffer NaN-filled first: a tile that is never written fails, and column sums of integer-valued inputs are exact in fp32
 in any order, so they are compared by equality and a tile counted twice fails too."""
@@ -277,30 +277,99 @@ def test_fused_blocks_match_module_path():
     assert np.corrcoef(a.ravel(), b.ravel())[0, 1] > 0.9995
 
 
-def test_packed_attention_matches_explicit_softmax():
-    from imagefolder_b200.vit_ops import packed_attention
+@pytest.mark.parametrize("case,heads,qkv_bias,attn_drop", [("head_dim_32", 12, True, 0.0), ("no_qkv_bias", 6, False, 0.0),
+                                                       ("attn_drop", 6, True, 0.1)])
+def test_run_blocks_attention_inside_and_outside_the_kernels(case, heads, qkv_bias, attn_drop):
+    """run_blocks on block stacks whose attention the wgmma kernels do or do not cover, under bf16 autocast, against the
+    plain module path: head_dim 32 (the module's own attention), a qkv projection without bias at head_dim 64 (the
+    kernels), attention dropout in training (the module's own attention; its dropout draws differ from the module path's,
+    so only the kernels it called and finite gradients are checked)."""
+    from imagefolder_b200 import _capi, vit_ops
+    from imagefolder_b200.dino_enc.vision_transformer import VisionTransformer
+    torch.manual_seed(heads)
+    vit = VisionTransformer(img_size=64, patch_size=16, embed_dim=384, depth=2, num_heads=heads, qkv_bias=qkv_bias,
+                            init_values=0.5).cuda().train(attn_drop > 0)
+    for blk in vit.blocks:
+        blk.attn.attn_drop.p = attn_drop
+    x0 = torch.randn(2, 37, 384, device="cuda")
+    g = torch.randn(2, 37, 384, device="cuda")
+
+    def run():
+        x = x0.clone().requires_grad_(True)
+        with torch.autocast("cuda", dtype=torch.bfloat16):
+            y = vit_ops.run_blocks(vit, x)
+        y.float().backward(g)
+        return y.detach().float(), x.grad
+
+    _capi.TIMING = {}
+    try:
+        y_fused, gx_fused = run()
+        calls = set(_capi.TIMING)
+    finally:
+        _capi.TIMING = None
+    assert "xq_vit_residual_ln_fwd" in calls and "xq_vit_residual_ln_bwd" in calls, (case, calls)
+    attn_calls = {c for c in calls if c.startswith("xq_vit_attn_")}
+    if case == "no_qkv_bias":
+        assert {"xq_vit_attn_fwd", "xq_vit_attn_bwd"} <= attn_calls, calls
+    else:
+        assert not attn_calls, (case, calls)
+    if case == "attn_drop":
+        assert torch.isfinite(y_fused).all() and torch.isfinite(gx_fused).all()
+        assert all(torch.isfinite(p.grad).all() for p in vit.blocks.parameters() if p.grad is not None)
+        return
+    orig = vit_ops.fused_path_ok
+    vit_ops.fused_path_ok = lambda *a, **k: False
+    try:
+        y_plain, gx_plain = run()
+    finally:
+        vit_ops.fused_path_ok = orig
+    # both are bf16-GEMM pipelines; they differ only by rounding order
+    for what, u, v in (("forward", y_fused, y_plain), ("d x", gx_fused, gx_plain)):
+        a, b = u.cpu().numpy(), v.cpu().numpy()
+        assert np.abs(a - b).max() < 0.06 * np.abs(b).max(), (case, what)
+        assert np.corrcoef(a.ravel(), b.ravel())[0, 1] > 0.9995, (case, what)
+
+
+def test_qkv_attention_without_bias_matches_explicit_softmax():
+    """_QKVAttention with b = None (a qkv projection without bias) against the fp64 explicit softmax of y W^T."""
+    from imagefolder_b200.vit_ops import _QKVAttention
     torch.manual_seed(3)
     B, N, H, hd = 3, 77, 6, 64
     C = H * hd
-    qkv = torch.randn(B, N, 3 * C, device="cuda").to(torch.bfloat16).requires_grad_(True)
-    o = packed_attention(qkv, H)
+    y = torch.randn(B, N, C, device="cuda").to(torch.bfloat16).requires_grad_(True)
+    W = (torch.randn(3 * C, C, device="cuda") * C ** -0.5).to(torch.bfloat16).float()    # exact in the node's bf16 GEMMs
+    o = _QKVAttention.apply(y, W, None, H)
     assert o.shape == (B, N, C)
     g = torch.randn_like(o)
     o.backward(g)
-    q2 = qkv.detach().double().requires_grad_(True)
-    t = q2.view(B, N, 3, H, hd).permute(2, 0, 3, 1, 4)
+    y2 = y.detach().double().requires_grad_(True)
+    t = (y2 @ W.double().t()).view(B, N, 3, H, hd).permute(2, 0, 3, 1, 4)
     att = ((t[0] * hd ** -0.5) @ t[1].transpose(-2, -1)).softmax(-1)
     ref = (att @ t[2]).transpose(1, 2).reshape(B, N, C)
     ref.backward(g.double())
     np.testing.assert_allclose(o.float().detach().cpu().numpy(), ref.detach().float().cpu().numpy(), rtol=2e-2, atol=2e-2)
-    gr = q2.grad.float().cpu().numpy()
-    np.testing.assert_allclose(qkv.grad.float().cpu().numpy(), gr, rtol=3e-2, atol=3e-2 * float(np.abs(gr).max()))
+    gr = y2.grad.float().cpu().numpy()
+    np.testing.assert_allclose(y.grad.float().cpu().numpy(), gr, rtol=3e-2, atol=3e-2 * float(np.abs(gr).max()))
 
 
 def test_qkv_attention_node_matches_linear_plus_attention():
-    """_QKVAttention (projection + attention as one node; bias gradient from the pack kernel's column sums) against
-    nn.Linear + packed_attention with autograd's own sum(0) bias gradient."""
-    from imagefolder_b200.vit_ops import packed_attention, _QKVAttention
+    """_QKVAttention (projection + attention as one node; bias gradient from the attention backward's column sums) against
+    nn.Linear + the same attention kernels as a separate node, with autograd's own sum(0) bias gradient."""
+    from imagefolder_b200.vit_ops import _QKVAttention, attn_tc_backward, attn_tc_forward
+
+    class Attention(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, qkv, heads):
+            out, lse2 = attn_tc_forward(qkv, heads)
+            ctx.save_for_backward(qkv, out, lse2)
+            ctx.heads = heads
+            return out
+
+        @staticmethod
+        def backward(ctx, g):
+            qkv, out, lse2 = ctx.saved_tensors
+            return attn_tc_backward(qkv, out, lse2, g, ctx.heads), None
+
     torch.manual_seed(5)
     B, N, H, hd = 4, 131, 6, 64
     C = H * hd
@@ -308,51 +377,18 @@ def test_qkv_attention_node_matches_linear_plus_attention():
     W = (torch.randn(3 * C, C, device="cuda") * C ** -0.5).requires_grad_(True)
     b = torch.randn(3 * C, device="cuda").requires_grad_(True)
     g = torch.randn(B, N, C, device="cuda").to(torch.bfloat16)
-    o1 = _QKVAttention.apply(y, W, b, H, 0.0)
+    o1 = _QKVAttention.apply(y, W, b, H)
     gy1, gW1, gb1 = torch.autograd.grad(o1, (y, W, b), g)
     with torch.autocast("cuda", dtype=torch.bfloat16):
-        o2 = packed_attention(torch.nn.functional.linear(y, W, b), H)
+        o2 = Attention.apply(torch.nn.functional.linear(y, W, b), H)
     gy2, gW2, gb2 = torch.autograd.grad(o2, (y, W, b), g)
-    assert torch.equal(o1, o2)                                   # same GEMM + same library attention
+    assert torch.equal(o1, o2)                                   # same GEMM + same attention kernels
     assert gW1.dtype == torch.float32 and gb1.dtype == torch.float32
     np.testing.assert_allclose(gy1.float().cpu().numpy(), gy2.float().cpu().numpy(), rtol=0, atol=0)
     np.testing.assert_allclose(gW1.cpu().numpy(), gW2.cpu().numpy(), rtol=0, atol=0)
     # the fused bias gradient sums the bf16 d(qkv) in fp32 (autograd: bf16 reduce) -> equal up to bf16 rounding
     ref = gb2.cpu().numpy()
     np.testing.assert_allclose(gb1.cpu().numpy(), ref, rtol=1e-2, atol=1e-2 * float(np.abs(ref).max()))
-
-
-def test_pack_qkv_cabi_ragged_rows_and_bias():
-    from imagefolder_b200 import _capi
-    L = _capi.lib()
-    torch.manual_seed(6)
-    sms = _sms()
-    # the last two: the training encoder's rows (8,208 tiles, ~60 per CTA) and ~8 tiles per CTA at the widest C the kernel
-    # takes -- every CTA's 4-stage ring wraps and most tiles come from the atomic counter
-    for M, C in [(1, 8), (7, 64), (1031, 768), (4099, 384), (2500, 1024), (TRAIN_ROWS, 768), (8 * sms * 8 + 3, 1024)]:
-        ws = torch.empty(int(L.xq_vit_pack_workspace_bytes()), dtype=torch.uint8, device="cuda")
-
-        def pack(dq, dk, dv, gb):
-            out = _nan((M, 3 * C), torch.bfloat16)
-            _capi.check(L.xq_vit_pack_qkv(_capi.ptr(dq), _capi.ptr(dk), _capi.ptr(dv), _capi.ptr(out), _capi.ptr(gb), M, C,
-                                          _capi.ptr(ws), ws.numel(), _capi.stream_ptr(out.device)), "xq_vit_pack_qkv")
-            return out
-
-        # integer-valued gradients: the fp32 column sums are exact in any order, so the bias gradient must equal the int64
-        # sums -- a row counted twice or not at all fails at any M
-        dq, dk, dv = (torch.randint(-4, 5, (M, C), device="cuda").to(torch.bfloat16) for _ in range(3))
-        gb = torch.full((3 * C,), 7.0, device="cuda")                   # the launcher zeroes it
-        ref = torch.cat([dq, dk, dv], dim=1)
-        assert torch.equal(pack(dq, dk, dv, gb), ref)
-        assert torch.equal(gb, ref.to(torch.int64).sum(0).to(torch.float32))
-        # full-mantissa values for the copy, with and without the bias gradient
-        dq, dk, dv = (torch.randn(M, C, device="cuda").to(torch.bfloat16) for _ in range(3))
-        ref = torch.cat([dq, dk, dv], dim=1)
-        assert torch.equal(pack(dq, dk, dv, gb), ref)
-        # fp32 sums: a lane's tiles (<= ~60), 8 warps, one atomicAdd per CTA: ~200 additions deep, 200 x 2^-24 = 1.2e-5
-        _assert_within(gb, ref.double().sum(0), 1.2e-5 * ref.double().abs().sum(0), "g_bias")
-        assert torch.equal(pack(dq, dk, dv, None), ref)
-    assert L.xq_vit_pack_qkv(None, None, None, None, None, 4, 8, None, 0, None) != 0
 
 
 def test_patch_embed_gemm_matches_conv():

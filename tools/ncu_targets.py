@@ -23,8 +23,8 @@ del h, yy
 yq = torch.randn(B, S, D, device=dev).to(torch.bfloat16).requires_grad_(True)
 Wq = (torch.randn(3 * D, D, device=dev) * D ** -0.5).requires_grad_(True)
 bq = torch.randn(3 * D, device=dev, requires_grad=True)
-o = vit_ops._QKVAttention.apply(yq, Wq, bq, H, 0.0)
-torch.autograd.grad(o, (yq, Wq, bq), torch.randn_like(o))                        # pack_qkv_kernel (+ library attention)
+o = vit_ops._QKVAttention.apply(yq, Wq, bq, H)                                  # attn_fwd_kernel
+torch.autograd.grad(o, (yq, Wq, bq), torch.randn_like(o))                        # attention backward kernels
 pe = PatchEmbed(img_size=256, patch_size=16, in_chans=3, embed_dim=D).cuda()
 img = torch.rand(B, 3, 256, 256, device=dev)
 with torch.autocast("cuda", dtype=torch.bfloat16):

@@ -25,7 +25,7 @@ for (B, S, D, H) in [(2, 37, 768, 12), (3, 9, 384, 6), (1, 21, 1024, 16)]:
     yq = torch.randn(B, S, D, device=dev).to(torch.bfloat16).requires_grad_(True)
     Wq = (torch.randn(3 * D, D, device=dev) * D ** -0.5).requires_grad_(True)
     bq = torch.randn(3 * D, device=dev, requires_grad=True)
-    o = vit_ops._QKVAttention.apply(yq, Wq, bq, H, 0.0)
+    o = vit_ops._QKVAttention.apply(yq, Wq, bq, H)
     torch.autograd.grad(o, (yq, Wq, bq), torch.randn_like(o))
 pe = PatchEmbed(img_size=64, patch_size=16, in_chans=3, embed_dim=96).cuda()
 with torch.autocast("cuda", dtype=torch.bfloat16):
