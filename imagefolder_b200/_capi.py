@@ -18,7 +18,7 @@ XQ_EMA_MAX_TENSORS = 1020      # entries of one xq_ema_update launch (include/xq
 XQ_ADAMW_MAX_TENSORS = 584     # entries of one xq_adamw_step launch (include/xqb200.h)
 XQ_METRIC_STRIP_ROWS = 32      # image rows per CTA of xq_recon_psnr_ssim (include/xqb200.h)
 
-XQ_MS_VQ_ZNORM, XQ_MS_VQ_L2, XQ_MS_BSQ = 0, 1, 2
+XQ_MS_VQ_ZNORM, XQ_MS_VQ_L2, XQ_MS_BSQ, XQ_MS_BSQ_HARD = 0, 1, 2, 3
 
 
 class XqMsDesc(ctypes.Structure):

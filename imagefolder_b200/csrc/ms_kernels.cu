@@ -12,6 +12,7 @@
 //
 // Kernels: ms_forward_kernel, ms_backward_kernel, ms_decode_kernel, ms_finalize_kernel,
 //          bsq_entropy_fwd_kernel, bsq_entropy_bwd_kernel, reduce_batch_kernel, channel_norm_kernel
+#include <algorithm>
 #include <cstdlib>
 
 #include "xq_common.cuh"
@@ -22,6 +23,9 @@ constexpr int MS_THREADS = 384;       // forward / decode: 12 warps; the search 
 constexpr int MS_BWD_THREADS = 512;   // backward: no search, only latency-bound conv / pooling work -> more warps
 constexpr int MS_TILE_V = 128;
 constexpr int MS_MAX_WARPS = 16;
+
+// both LFQ modes quantize with sign bits; they differ only in the entropy term
+__host__ __device__ inline bool ms_is_bsq(int mode) { return mode == XQ_MS_BSQ || mode == XQ_MS_BSQ_HARD; }
 
 struct MsArgs {
     xq_ms_desc d;
@@ -40,7 +44,8 @@ struct MsArgs {
     float *hist;
     float *partial;       // [B] per-image loss partial
     float *F_last;        // [B,CHW] saved masked f_hat
-    float *Fprev01;       // [SN,2,CHW] (BSQ) f_hat before scale si for images 0,1
+    float *Fprev;         // [SN,fprev_imgs,CHW] (BSQ) f_hat before scale si for images b < fprev_imgs
+    int fprev_imgs;       // 2 (soft entropy: rows 0 and 1 only) or B (full-softmax entropy)
 };
 
 // ---- shared-memory carve-up ------------------------------------------------------------
@@ -476,7 +481,7 @@ ms_forward_kernel(const MsArgs a) {
     extern __shared__ __align__(16) float smem[];
     const xq_ms_desc &d = a.d;
     const int C = d.C, H = d.H, W = d.W, HW = H * W, CHW = C * HW, RP = ms_rp(H, W);
-    const bool bsq = d.mode == XQ_MS_BSQ;
+    const bool bsq = ms_is_bsq(d.mode);
     MsSmem s = ms_carve(smem, C, H, W, !bsq);
     const int b = blockIdx.x, tid = threadIdx.x;
     const float *fb = a.fn + (size_t)b * CHW;
@@ -519,8 +524,8 @@ ms_forward_kernel(const MsArgs a) {
         __syncthreads();
         ms_bicubic_up(s, C, H, W, P, RP);
         __syncthreads();
-        if (bsq && a.Fprev01 && b < 2) {
-            float *dst = a.Fprev01 + ((size_t)si * 2 + b) * CHW;
+        if (bsq && a.Fprev && b < a.fprev_imgs) {
+            float *dst = a.Fprev + ((size_t)si * a.fprev_imgs + b) * CHW;
             for (int i = tid; i < CHW; i += blockDim.x) dst[i] = s.fhat[i];
         }
         const int kphi = d.K > 0 ? d.phi_map[si] : -1;
@@ -681,6 +686,317 @@ bsq_entropy_bwd_kernel(const xq_ms_desc d, const float *__restrict__ fn, const f
     }
 }
 
+// ---- full-softmax entropy term, LFQ(soft_entropy=False) (lookup_free_quantize.py:41-79, 220-229) ---------------
+// softmax_j(2 x.code_j / 0.01) over the 2^C codes code_j = +-s factorises over the bits: P(bit k = 1 | row) = q_k =
+// sigmoid(400 s x_k).  The sample entropy is a sum of per-bit binary entropies; the codebook distribution
+// a_j = mean_r prod_k q_rk(bit k of j) does not factorise and is contracted as a = A^T Bm (A over the low lo = C/2 bits,
+// Bm over the high ones), with the A / Bm rows built in shared memory and never written to HBM.  fp32 FFMA, per-thread
+// accumulation in row order, per-CTA partials reduced in a fixed order: bitwise repeatable.
+constexpr int HB_THREADS = 256;
+constexpr int HB_RC = 32;        // rows staged per step (forward and backward)
+constexpr int HB_TILE = 64;      // edge of the a-tile one forward CTA owns
+constexpr int HB_MAX_C = 16;
+constexpr int HB_SPLIT_ROWS = 1024;   // rows per forward CTA (before the cap on the number of splits)
+constexpr int HB_MAX_SPLITS = 16;
+
+// q = sigmoid(z), qm = sigmoid(-z), each evaluated directly (1 - q would cancel to 0 long before qm underflows)
+__device__ __forceinline__ void hb_sig(float z, float &qp, float &qm) {
+    qp = 1.f / (1.f + expf(-z));
+    qm = 1.f / (1.f + expf(z));
+}
+// binary entropy of sigmoid(z), natural log: softplus(-|z|) + |z| sigmoid(-|z|)
+__device__ __forceinline__ float hb_entropy(float z) {
+    const float az = fabsf(z), e = expf(-az);
+    return log1pf(e) + az * (e / (1.f + e));
+}
+
+// rows per split and number of splits of the B*HW rows (shared by the workspace layout and the launch)
+static void hb_splits(const xq_ms_desc *d, int *splits, int *rows_per_split) {
+    const int N = d->B * d->H * d->W;
+    int ks = (N + HB_SPLIT_ROWS - 1) / HB_SPLIT_ROWS;
+    if (ks > HB_MAX_SPLITS) ks = HB_MAX_SPLITS;
+    int rps = (N + ks - 1) / ks;
+    rps = (rps + HB_RC - 1) / HB_RC * HB_RC;
+    *rows_per_split = rps;
+    *splits = (N + rps - 1) / rps;
+}
+
+// row r = b*HW + p of scale si: x_k = fn[b,k,p] - F_{si-1}[b,k,p] (Fprev[si] holds the masked f_hat before scale si)
+__device__ __forceinline__ float hb_x(const xq_ms_desc &d, const float *__restrict__ fn, const float *__restrict__ Fprev,
+                                      int si, int b, int k, int p) {
+    const int HW = d.H * d.W, CHW = d.C * HW;
+    const size_t e = (size_t)b * CHW + (size_t)k * HW + p;
+    return fn[e] - Fprev[(size_t)si * d.B * CHW + e];
+}
+
+// grid (a-tiles, splits, SN).  part[si][split][j] = sum over the split's masked rows of prod_k q_k(bit k of j) for the
+// CTA's tile of j; spart[si][split] = sum of the binary entropies (written by the tile-0 CTAs).
+__global__ void __launch_bounds__(HB_THREADS)
+bsq_hard_fwd_kernel(const xq_ms_desc d, const float *__restrict__ fn, const float *__restrict__ Fprev,
+                    const float *__restrict__ nq, int rows_per_split, float *__restrict__ part, float *__restrict__ spart) {
+    __shared__ float qp[HB_RC][HB_MAX_C + 1], qm[HB_RC][HB_MAX_C + 1];
+    __shared__ __align__(16) float As[HB_RC][HB_TILE], Bs[HB_RC][HB_TILE];
+    __shared__ float red[32];
+    const int C = d.C, lo = C / 2, hi = C - lo, Lo = 1 << lo, Hi = 1 << hi;
+    const int TL = Lo < HB_TILE ? Lo : HB_TILE, TH = Hi < HB_TILE ? Hi : HB_TILE;
+    const int ntl = Lo / TL;
+    const int tile = blockIdx.x, split = blockIdx.y, si = blockIdx.z, nsplit = gridDim.y;
+    const int jl0 = (tile % ntl) * TL, jh0 = (tile / ntl) * TH;
+    const int HW = d.H * d.W, N = d.B * HW;
+    const float zs = 400.f * d.scaler[si];
+    const int r_begin = split * rows_per_split;
+    const int r_end = min(N, r_begin + rows_per_split);
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const bool entropy_cta = tile == 0;
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    float hsum = 0.f;
+    for (int r0 = r_begin; r0 < r_end; r0 += HB_RC) {
+        for (int i = tid; i < HB_RC * C; i += blockDim.x) {
+            const int rr = i / C, k = i - rr * C, r = r0 + rr;
+            float vp = 0.f, vm = 0.f;          // rows outside the mask: A = Bm = 0 (hi >= 1 factor is 0)
+            if (r < r_end) {
+                const int b = r / HW, p = r - b * HW;
+                if (!nq || (float)si < nq[b]) {
+                    const float z = zs * hb_x(d, fn, Fprev, si, b, k, p);
+                    hb_sig(z, vp, vm);
+                    if (entropy_cta) hsum += hb_entropy(z);
+                }
+            }
+            qp[rr][k] = vp;
+            qm[rr][k] = vm;
+        }
+        __syncthreads();
+        for (int i = tid; i < HB_RC * TL; i += blockDim.x) {
+            const int rr = i / TL, j = i - rr * TL, jl = jl0 + j;
+            float v = 1.f;
+            for (int k = 0; k < lo; ++k) v = v * (((jl >> k) & 1) ? qp[rr][k] : qm[rr][k]);
+            As[rr][j] = v;
+        }
+        for (int i = tid; i < HB_RC * TH; i += blockDim.x) {
+            const int rr = i / TH, j = i - rr * TH, jh = jh0 + j;
+            float v = 1.f;
+            for (int k = 0; k < hi; ++k) v = v * (((jh >> k) & 1) ? qp[rr][lo + k] : qm[rr][lo + k]);
+            Bs[rr][j] = v;
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int rr = 0; rr < HB_RC; ++rr) {
+            float av[4], bv[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) av[i] = As[rr][(ty + 16 * i) & (TL - 1)];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) bv[j] = Bs[rr][(tx + 16 * j) & (TH - 1)];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+    float *dst = part + ((size_t)si * nsplit + split) * ((size_t)1 << C);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int jl = ty + 16 * i, jh = tx + 16 * j;
+            if (jl < TL && jh < TH) dst[(jl0 + jl) | ((jh0 + jh) << lo)] = acc[i][j];
+        }
+    if (entropy_cta) {
+        const float t = block_sum(hsum, red);
+        if (tid == 0) spart[(size_t)si * nsplit + split] = t;
+    }
+}
+
+// one CTA per scale: a = sum_split part / (n1 HW) (saved for the backward), Hc, S, the scale's weighted entropy term
+__global__ void __launch_bounds__(HB_THREADS)
+bsq_hard_fwd_reduce_kernel(const xq_ms_desc d, const float *__restrict__ nq, int nsplit, const float *__restrict__ part,
+                           const float *__restrict__ spart, float *__restrict__ abar, float *__restrict__ ent_scales) {
+    __shared__ float red[32];
+    const int si = blockIdx.x, V = 1 << d.C;
+    float n1 = 0.f;
+    for (int b = 0; b < d.B; ++b) n1 += (!nq || (float)si < nq[b]) ? 1.f : 0.f;
+    const float inv = 1.f / (n1 * (float)(d.H * d.W));
+    float hc = 0.f;
+    for (int j = threadIdx.x; j < V; j += blockDim.x) {
+        float acc = 0.f;
+        for (int ks = 0; ks < nsplit; ++ks) acc += part[((size_t)si * nsplit + ks) * V + j];
+        const float a = acc * inv;
+        abar[(size_t)si * V + j] = a;
+        hc += -a * logf(a + 1e-5f);
+    }
+    hc = block_sum(hc, red);
+    if (threadIdx.x == 0) {
+        float S = 0.f;
+        for (int ks = 0; ks < nsplit; ++ks) S += spart[(size_t)si * nsplit + ks];
+        S = S * inv;
+        ent_scales[si] = (d.w_sample * S - d.w_batch * hc) * d.entropy_weight / (n1 / (float)d.B);
+    }
+}
+
+// G = dHc/da = -log(a + 1e-5) - a / (a + 1e-5), in both index orders: G[si][jh][jl] and GT[si][jl][jh]
+__global__ void bsq_hard_grad_table_kernel(int SN, int C, const float *__restrict__ abar, float *__restrict__ G,
+                                           float *__restrict__ GT) {
+    const int lo = C / 2, hi = C - lo, V = 1 << C;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)SN * V) return;
+    const int si = (int)(i / V), j = (int)(i - (size_t)si * V);
+    const float a = abar[i];
+    const float g = -logf(a + 1e-5f) - a / (a + 1e-5f);
+    G[i] = g;
+    GT[(size_t)si * V + (size_t)(j & ((1 << lo) - 1)) * (1 << hi) + (j >> lo)] = g;
+}
+
+__host__ __device__ inline size_t hb_bwd_smem_floats(int C) {
+    const int lo = C / 2, hi = C - lo;
+    return (size_t)2 * HB_RC * ((1 << lo) + (1 << hi)) + (size_t)4 * HB_RC * (HB_MAX_C + 1) + 4 * XQ_MAX_SCALES;
+}
+
+// sum_j g[j] * d/dq_k prod_k' f_k'(bit k' of j) over n bits, f(1) = qp, f(0) = qm: pairs j, j | 1<<k share the product of
+// the other factors, so this is sum_{j: bit k = 0} (g[j | 1<<k] - g[j]) prod_{k' != k} f_k'(j).  No division by q.
+__device__ __forceinline__ float hb_loo(const float *g, const float *qp, const float *qm, int n, int k) {
+    float acc = 0.f;
+    const int half = 1 << (n - 1);
+    for (int t = 0; t < half; ++t) {
+        const int j = ((t >> k) << (k + 1)) | (t & ((1 << k) - 1));     // insert a 0 at bit k
+        float prod = g[j | (1 << k)] - g[j];
+        for (int kk = 0; kk < n; ++kk)
+            if (kk != k) prod = prod * (((j >> kk) & 1) ? qp[kk] : qm[kk]);
+        acc += prod;
+    }
+    return acc;
+}
+
+// grid = ceil(B*HW / HB_RC): each CTA owns HB_RC rows, walks every scale and writes d entropy / d fn for its rows once
+// (gent [B][C*HW], every element written: no memset, no atomics).
+__global__ void __launch_bounds__(HB_THREADS)
+bsq_hard_bwd_kernel(const xq_ms_desc d, const float *__restrict__ fn, const float *__restrict__ Fprev,
+                    const float *__restrict__ nq, const float *__restrict__ G, const float *__restrict__ GT,
+                    const float *__restrict__ g_ent, float *__restrict__ gent) {
+    extern __shared__ __align__(16) float smem[];
+    const int C = d.C, lo = C / 2, hi = C - lo, Lo = 1 << lo, Hi = 1 << hi, V = 1 << C;
+    const int HW = d.H * d.W, N = d.B * HW, SN = d.SN;
+    const int tid = threadIdx.x, r0 = blockIdx.x * HB_RC;
+    constexpr int QP = HB_MAX_C + 1;
+    float *AT = smem;                                  // [Lo][HB_RC]
+    float *BT = AT + (size_t)Lo * HB_RC;               // [Hi][HB_RC]
+    float *gA = BT + (size_t)Hi * HB_RC;               // [HB_RC][Lo]
+    float *gB = gA + (size_t)HB_RC * Lo;               // [HB_RC][Hi]
+    float *qp = gB + (size_t)HB_RC * Hi;               // [HB_RC][QP]
+    float *qm = qp + HB_RC * QP;
+    float *zz = qm + HB_RC * QP;
+    float *gacc = zz + HB_RC * QP;
+    float *s_inv = gacc + HB_RC * QP;                  // [SN] 1 / (n1 HW)
+    float *s_coef = s_inv + XQ_MAX_SCALES;             // [SN] g_ent * entropy_weight / ratio / SN
+    const float ge = g_ent ? *g_ent : 0.f;
+    for (int si = tid; si < SN; si += blockDim.x) {
+        float n1 = 0.f;
+        for (int b = 0; b < d.B; ++b) n1 += (!nq || (float)si < nq[b]) ? 1.f : 0.f;
+        s_inv[si] = 1.f / (n1 * (float)HW);
+        s_coef[si] = ge * d.entropy_weight / (n1 / (float)d.B) / (float)SN;
+    }
+    for (int i = tid; i < HB_RC * QP; i += blockDim.x) gacc[i] = 0.f;
+    __syncthreads();
+    for (int si = 0; si < SN; ++si) {
+        const float zs = 400.f * d.scaler[si];
+        int any = 0;
+        for (int i = tid; i < HB_RC * C; i += blockDim.x) {
+            const int rr = i / C, k = i - rr * C, r = r0 + rr;
+            float vp = 0.f, vm = 0.f, z = 0.f;
+            if (r < N) {
+                const int b = r / HW, p = r - b * HW;
+                if (!nq || (float)si < nq[b]) {
+                    z = zs * hb_x(d, fn, Fprev, si, b, k, p);
+                    hb_sig(z, vp, vm);
+                    any = 1;
+                }
+            }
+            qp[rr * QP + k] = vp;
+            qm[rr * QP + k] = vm;
+            zz[rr * QP + k] = z;
+        }
+        if (!__syncthreads_or(any)) continue;     // no masked row in this CTA at this scale
+        for (int i = tid; i < Lo * HB_RC; i += blockDim.x) {
+            const int jl = i / HB_RC, rr = i - jl * HB_RC;
+            float v = 1.f;
+            for (int k = 0; k < lo; ++k) v = v * (((jl >> k) & 1) ? qp[rr * QP + k] : qm[rr * QP + k]);
+            AT[i] = v;
+        }
+        for (int i = tid; i < Hi * HB_RC; i += blockDim.x) {
+            const int jh = i / HB_RC, rr = i - jh * HB_RC;
+            float v = 1.f;
+            for (int k = 0; k < hi; ++k) v = v * (((jh >> k) & 1) ? qp[rr * QP + lo + k] : qm[rr * QP + lo + k]);
+            BT[i] = v;
+        }
+        __syncthreads();
+        // gA[r][jl] = sum_jh G[jl,jh] Bm[r][jh] ; gB[r][jh] = sum_jl G[jl,jh] A[r][jl]   (16 rows per thread item)
+        const float *Gs = G + (size_t)si * V, *GTs = GT + (size_t)si * V;
+        for (int item = tid; item < Lo * (HB_RC / 16); item += blockDim.x) {
+            const int jl = item % Lo, rg = item / Lo;
+            float acc[16];
+#pragma unroll
+            for (int q = 0; q < 16; ++q) acc[q] = 0.f;
+            for (int jh = 0; jh < Hi; ++jh) {
+                const float g = __ldg(Gs + (size_t)jh * Lo + jl);
+                const float4 *bp = reinterpret_cast<const float4 *>(BT + (size_t)jh * HB_RC + rg * 16);
+#pragma unroll
+                for (int q4 = 0; q4 < 4; ++q4) {
+                    const float4 bv = bp[q4];
+                    acc[4 * q4 + 0] = fmaf(g, bv.x, acc[4 * q4 + 0]);
+                    acc[4 * q4 + 1] = fmaf(g, bv.y, acc[4 * q4 + 1]);
+                    acc[4 * q4 + 2] = fmaf(g, bv.z, acc[4 * q4 + 2]);
+                    acc[4 * q4 + 3] = fmaf(g, bv.w, acc[4 * q4 + 3]);
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < 16; ++q) gA[(size_t)(rg * 16 + q) * Lo + jl] = acc[q];
+        }
+        for (int item = tid; item < Hi * (HB_RC / 16); item += blockDim.x) {
+            const int jh = item % Hi, rg = item / Hi;
+            float acc[16];
+#pragma unroll
+            for (int q = 0; q < 16; ++q) acc[q] = 0.f;
+            for (int jl = 0; jl < Lo; ++jl) {
+                const float g = __ldg(GTs + (size_t)jl * Hi + jh);
+                const float4 *ap = reinterpret_cast<const float4 *>(AT + (size_t)jl * HB_RC + rg * 16);
+#pragma unroll
+                for (int q4 = 0; q4 < 4; ++q4) {
+                    const float4 av = ap[q4];
+                    acc[4 * q4 + 0] = fmaf(g, av.x, acc[4 * q4 + 0]);
+                    acc[4 * q4 + 1] = fmaf(g, av.y, acc[4 * q4 + 1]);
+                    acc[4 * q4 + 2] = fmaf(g, av.z, acc[4 * q4 + 2]);
+                    acc[4 * q4 + 3] = fmaf(g, av.w, acc[4 * q4 + 3]);
+                }
+            }
+#pragma unroll
+            for (int q = 0; q < 16; ++q) gB[(size_t)(rg * 16 + q) * Hi + jh] = acc[q];
+        }
+        __syncthreads();
+        // carry to z: dloss/dz_k = inv (w_sample dH_b/dz - w_batch dHc/dq_k q(1-q)),  dH_b/dz = -z q (1-q);  dz/dx = 400 s
+        const float inv = s_inv[si], coef = s_coef[si];
+        for (int i = tid; i < HB_RC * C; i += blockDim.x) {
+            const int rr = i / C, k = i - rr * C;
+            const float *qpr = qp + rr * QP, *qmr = qm + rr * QP;
+            const float pq = qpr[k] * qmr[k];
+            if (qpr[k] == 0.f && qmr[k] == 0.f) continue;   // row outside the mask at this scale
+            const float dq = k < lo ? hb_loo(gA + (size_t)rr * Lo, qpr, qmr, lo, k)
+                                    : hb_loo(gB + (size_t)rr * Hi, qpr + lo, qmr + lo, hi, k - lo);
+            const float dz = inv * (d.w_sample * (-zz[rr * QP + k] * pq) - d.w_batch * (dq * pq));
+            gacc[rr * QP + k] += coef * (dz * zs);
+        }
+        __syncthreads();
+    }
+    for (int i = tid; i < HB_RC * C; i += blockDim.x) {
+        const int rr = i / C, k = i - rr * C, r = r0 + rr;
+        if (r >= N) continue;
+        const int b = r / HW, p = r - b * HW;
+        gent[(size_t)b * C * HW + (size_t)k * HW + p] = gacc[rr * QP + k];
+    }
+}
+
 // =========================================================================================
 // backward: one CTA per image.  Walks the scales in reverse, recomputing u_k / h_k from the
 // saved indices (same device code as the forward -> bit-identical), Appendix A.2.
@@ -691,7 +1007,8 @@ struct MsBwdArgs {
     const int64_t *idx_all;
     const float *F_last;
     const float *g_out, *g_vq, *g_commit;
-    const float *gent;    // [2][CHW] entropy gradient wrt fn (BSQ) or null
+    const float *gent;    // [gent_imgs][CHW] entropy gradient wrt fn (BSQ) or null
+    int gent_imgs;        // 2 (soft entropy) or B (full-softmax entropy)
     float *gf;            // [B,CHW] gradient wrt f
     float *gE;            // [V,C] (atomics)
     float *dWpart;        // [B][K][C*C*9]
@@ -742,7 +1059,7 @@ ms_backward_kernel(const MsBwdArgs a) {
     extern __shared__ __align__(16) float smem[];
     const xq_ms_desc &d = a.d;
     const int C = d.C, H = d.H, W = d.W, HW = H * W, CHW = C * HW, RP = ms_rp(H, W), SN = d.SN;
-    const bool bsq = d.mode == XQ_MS_BSQ;
+    const bool bsq = ms_is_bsq(d.mode);
     MsBwdSmem s = ms_bwd_carve(smem, C, H, W);
     // adapter so the forward primitives can be reused
     MsSmem fs;
@@ -767,7 +1084,7 @@ ms_backward_kernel(const MsBwdArgs a) {
     float *gfb = a.gf + (size_t)b * CHW;
     for (int i = tid; i < CHW; i += blockDim.x) {
         float g = a.g_out ? a.g_out[(size_t)b * CHW + i] : 0.f;
-        if (a.gent && b < 2) g += a.gent[(size_t)b * CHW + i];
+        if (a.gent && b < a.gent_imgs) g += a.gent[(size_t)b * CHW + i];
         gfb[i] = g;
     }
     const float nq_b = a.nq ? a.nq[b] : 3.0e38f;
@@ -963,7 +1280,7 @@ ms_decode_kernel(const MsDecArgs a) {
     extern __shared__ __align__(16) float smem[];
     const xq_ms_desc &d = a.d;
     const int C = d.C, H = d.H, W = d.W, HW = H * W, CHW = C * HW, RP = ms_rp(H, W);
-    const bool bsq = d.mode == XQ_MS_BSQ;
+    const bool bsq = ms_is_bsq(d.mode);
     MsSmem s = ms_carve(smem, C, H, W, false);
     const int b = blockIdx.x, tid = threadIdx.x;
     for (int i = tid; i < CHW; i += blockDim.x) s.fhat[i] = a.fhat_in ? a.fhat_in[(size_t)b * CHW + i] : 0.f;
@@ -1037,9 +1354,10 @@ static int ms_vpad(int V) { return (V + MS_TILE_V - 1) / MS_TILE_V * MS_TILE_V; 
 static int ms_check(const xq_ms_desc *d) {
     if (!d) return XQ_ERR_ARG;
     if (d->B <= 0 || d->C <= 0 || d->H <= 0 || d->W <= 0 || d->SN <= 0 || d->SN > XQ_MAX_SCALES) return XQ_ERR_ARG;
-    if (d->mode < 0 || d->mode > 2) return XQ_ERR_ARG;
-    if (d->mode == XQ_MS_BSQ) { if (d->C > 30 || d->V != (1 << d->C)) return XQ_ERR_ARG; }
+    if (d->mode < 0 || d->mode > XQ_MS_BSQ_HARD) return XQ_ERR_ARG;
+    if (ms_is_bsq(d->mode)) { if (d->C > 30 || d->V != (1 << d->C)) return XQ_ERR_ARG; }
     else if (d->V <= 0) return XQ_ERR_ARG;
+    if (d->mode == XQ_MS_BSQ_HARD && d->C > HB_MAX_C) return XQ_ERR_UNSUPPORTED;
     for (int si = 0; si < d->SN; ++si) {
         int P = d->patch_nums[si];
         if (P <= 0 || P > d->H || P > d->W) return XQ_ERR_ARG;
@@ -1053,13 +1371,17 @@ static int ms_check(const xq_ms_desc *d) {
 
 struct MsWs {
     float *EnT, *ee, *fn, *partial, *ent_scales, *pbar, *gent, *dWpart, *dbpart;
+    float *hb_part, *hb_spart, *hb_G, *hb_GT;   // full-softmax entropy: per-split partials, dHc/da in both orders
     size_t total;
 };
+// images whose f_hat before every scale is saved (and whose entropy gradient the backward adds): the soft entropy term
+// only reads batch rows 0 and 1, the full-softmax one every image
+static int ms_ent_imgs(const xq_ms_desc *d) { return d->mode == XQ_MS_BSQ_HARD ? d->B : 2; }
 static MsWs ms_ws_layout(const xq_ms_desc *d, void *base) {
     MsWs w;
     char *p = (char *)base;
     size_t chw = (size_t)d->C * d->H * d->W;
-    size_t Vp = d->mode == XQ_MS_BSQ ? 0 : (size_t)ms_vpad(d->V);
+    size_t Vp = ms_is_bsq(d->mode) ? 0 : (size_t)ms_vpad(d->V);
     auto take = [&](size_t bytes) { char *q = p; p += align_up(bytes, 256); return (float *)q; };
     w.EnT = take(sizeof(float) * Vp * d->C);
     w.ee = take(sizeof(float) * Vp);
@@ -1067,9 +1389,16 @@ static MsWs ms_ws_layout(const xq_ms_desc *d, void *base) {
     w.partial = take(sizeof(float) * d->B);
     w.ent_scales = take(sizeof(float) * XQ_MAX_SCALES);
     w.pbar = take(sizeof(float) * XQ_MAX_SCALES * d->C * 2);
-    w.gent = take(sizeof(float) * 2 * chw);
+    w.gent = take(sizeof(float) * ms_ent_imgs(d) * chw);
     w.dWpart = take(sizeof(float) * (size_t)d->B * (d->K > 0 ? d->K : 0) * d->C * d->C * 9);
     w.dbpart = take(sizeof(float) * (size_t)d->B * (d->K > 0 ? d->K : 0) * d->C);
+    const bool hard = d->mode == XQ_MS_BSQ_HARD;
+    int splits = 0, rps = 0;
+    if (hard) hb_splits(d, &splits, &rps);
+    w.hb_part = take(hard ? sizeof(float) * (size_t)d->SN * splits * d->V : 0);
+    w.hb_spart = take(hard ? sizeof(float) * (size_t)d->SN * splits : 0);
+    w.hb_G = take(hard ? sizeof(float) * (size_t)d->SN * d->V : 0);
+    w.hb_GT = take(hard ? sizeof(float) * (size_t)d->SN * d->V : 0);
     w.total = (size_t)(p - (char *)base);
     return w;
 }
@@ -1089,8 +1418,9 @@ size_t xq_ms_saved_bytes(const xq_ms_desc *d) {
     if (ms_check(d) != XQ_OK) return 0;
     size_t chw = (size_t)d->C * d->H * d->W;
     size_t n = (size_t)d->B * chw;                                  // F_last
-    if (d->mode == XQ_MS_BSQ) n += (size_t)d->SN * 2 * chw;         // Fprev01
+    if (ms_is_bsq(d->mode)) n += (size_t)d->SN * ms_ent_imgs(d) * chw;   // Fprev
     if (d->mode == XQ_MS_BSQ) n += (size_t)XQ_MAX_SCALES * d->C * 2; // pbar
+    if (d->mode == XQ_MS_BSQ_HARD) n += (size_t)d->SN * d->V;        // abar
     if (d->channel_norm) n += (size_t)d->B * chw;                   // fn
     return sizeof(float) * n;
 }
@@ -1102,14 +1432,16 @@ int64_t xq_ms_total_tokens(const xq_ms_desc *d) {
     return t;
 }
 
-struct MsSaved { float *F_last, *Fprev01, *pbar, *fn; };
+struct MsSaved { float *F_last, *Fprev, *pbar, *abar, *fn; };
 static MsSaved ms_saved_layout(const xq_ms_desc *d, void *base) {
     MsSaved s;
     float *p = (float *)base;
     size_t chw = (size_t)d->C * d->H * d->W;
     s.F_last = p; p += (size_t)d->B * chw;
-    s.Fprev01 = nullptr; s.pbar = nullptr; s.fn = nullptr;
-    if (d->mode == XQ_MS_BSQ) { s.Fprev01 = p; p += (size_t)d->SN * 2 * chw; s.pbar = p; p += (size_t)XQ_MAX_SCALES * d->C * 2; }
+    s.Fprev = nullptr; s.pbar = nullptr; s.abar = nullptr; s.fn = nullptr;
+    if (ms_is_bsq(d->mode)) { s.Fprev = p; p += (size_t)d->SN * ms_ent_imgs(d) * chw; }
+    if (d->mode == XQ_MS_BSQ) { s.pbar = p; p += (size_t)XQ_MAX_SCALES * d->C * 2; }
+    if (d->mode == XQ_MS_BSQ_HARD) { s.abar = p; p += (size_t)d->SN * d->V; }
     if (d->channel_norm) { s.fn = p; p += (size_t)d->B * chw; }
     return s;
 }
@@ -1120,18 +1452,19 @@ int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const flo
     int rc = ms_check(d);
     if (rc != XQ_OK) return rc;
     if (!f || !out || !idx_all || !workspace) return XQ_ERR_ARG;
-    const bool bsq = d->mode == XQ_MS_BSQ;
+    const bool bsq = ms_is_bsq(d->mode);
     if (!bsq && !E) return XQ_ERR_ARG;
     if (d->K > 0 && (!phi_w || !phi_b)) return XQ_ERR_ARG;
     if (with_losses && (!loss || !saved)) return XQ_ERR_ARG;
-    if (bsq && with_losses && d->B < 2) return XQ_ERR_ARG;  // reference indexes batch row 1 (lookup_free_quantize.py:285)
+    // the soft entropy term indexes batch row 1 (lookup_free_quantize.py:285)
+    if (d->mode == XQ_MS_BSQ && with_losses && d->B < 2) return XQ_ERR_ARG;
     MsWs ws = ms_ws_layout(d, workspace);
     if (workspace_bytes < ws.total) return XQ_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)stream_;
     const int C = d->C, H = d->H, W = d->W, HW = H * W;
     size_t smem = sizeof(float) * ms_fwd_smem_floats(C, H, W, d->SN, !bsq);
     if (smem > 227 * 1024) return XQ_ERR_UNSUPPORTED;
-    MsSaved sv = {nullptr, nullptr, nullptr, nullptr};
+    MsSaved sv = {nullptr, nullptr, nullptr, nullptr, nullptr};
     if (saved) sv = ms_saved_layout(d, saved);
 
     MsArgs a;
@@ -1156,15 +1489,28 @@ int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const flo
     a.out = out; a.idx_all = idx_all; a.fhat_scales = fhat_scales; a.hist = hist;
     a.partial = with_losses ? ws.partial : nullptr;
     a.F_last = saved ? sv.F_last : nullptr;
-    a.Fprev01 = (bsq && with_losses) ? sv.Fprev01 : nullptr;
+    a.Fprev = (bsq && with_losses) ? sv.Fprev : nullptr;
+    a.fprev_imgs = ms_ent_imgs(d);
     if ((rc = smem_optin(ms_forward_kernel, smem)) != XQ_OK) return rc;
     ms_forward_kernel<<<d->B, MS_THREADS, smem, stream>>>(a);
     XQ_LAUNCH_CHECK("ms_forward_kernel");
     if (with_losses) {
         const float *ent = nullptr;
-        if (bsq) {
-            bsq_entropy_fwd_kernel<<<d->SN, 256, 0, stream>>>(*d, a.fn, sv.Fprev01, n_quantizers, ws.ent_scales, sv.pbar);
+        if (d->mode == XQ_MS_BSQ) {
+            bsq_entropy_fwd_kernel<<<d->SN, 256, 0, stream>>>(*d, a.fn, sv.Fprev, n_quantizers, ws.ent_scales, sv.pbar);
             XQ_LAUNCH_CHECK("bsq_entropy_fwd_kernel");
+            ent = ws.ent_scales;
+        } else if (d->mode == XQ_MS_BSQ_HARD) {
+            int splits, rps;
+            hb_splits(d, &splits, &rps);
+            const int lo = C / 2, hi = C - lo;
+            const int tiles = ((1 << lo) / std::min(1 << lo, HB_TILE)) * ((1 << hi) / std::min(1 << hi, HB_TILE));
+            bsq_hard_fwd_kernel<<<dim3(tiles, splits, d->SN), HB_THREADS, 0, stream>>>(*d, a.fn, sv.Fprev, n_quantizers, rps,
+                                                                                     ws.hb_part, ws.hb_spart);
+            XQ_LAUNCH_CHECK("bsq_hard_fwd_kernel");
+            bsq_hard_fwd_reduce_kernel<<<d->SN, HB_THREADS, 0, stream>>>(*d, n_quantizers, splits, ws.hb_part, ws.hb_spart,
+                                                                           sv.abar, ws.ent_scales);
+            XQ_LAUNCH_CHECK("bsq_hard_fwd_reduce_kernel");
             ent = ws.ent_scales;
         }
         double inv_n = 1.0 / ((double)d->B * C * HW);
@@ -1181,7 +1527,7 @@ int xq_ms_backward(const xq_ms_desc *d, const float *f, const float *E, const fl
     int rc = ms_check(d);
     if (rc != XQ_OK) return rc;
     if (!f || !idx_all || !saved || !gf || !workspace) return XQ_ERR_ARG;
-    const bool bsq = d->mode == XQ_MS_BSQ;
+    const bool bsq = ms_is_bsq(d->mode);
     if (!bsq && (!E || !gE)) return XQ_ERR_ARG;
     if (d->K > 0 && (!phi_w || !phi_b || !gphi_w || !gphi_b)) return XQ_ERR_ARG;
     MsWs ws = ms_ws_layout(d, workspace);
@@ -1201,10 +1547,22 @@ int xq_ms_backward(const xq_ms_desc *d, const float *f, const float *E, const fl
     a.F_last = sv.F_last;
     a.g_out = g_out; a.g_vq = g_vq; a.g_commit = g_commit;
     a.gent = nullptr;
-    if (bsq && g_entropy) {
+    a.gent_imgs = ms_ent_imgs(d);
+    if (d->mode == XQ_MS_BSQ && g_entropy) {
         XQ_CUDA_TRY(cudaMemsetAsync(ws.gent, 0, sizeof(float) * 2 * chw, stream));
-        bsq_entropy_bwd_kernel<<<d->SN, 256, 0, stream>>>(*d, a.fn, sv.Fprev01, n_quantizers, sv.pbar, g_entropy, ws.gent);
+        bsq_entropy_bwd_kernel<<<d->SN, 256, 0, stream>>>(*d, a.fn, sv.Fprev, n_quantizers, sv.pbar, g_entropy, ws.gent);
         XQ_LAUNCH_CHECK("bsq_entropy_bwd_kernel");
+        a.gent = ws.gent;
+    } else if (d->mode == XQ_MS_BSQ_HARD && g_entropy) {
+        const size_t nv = (size_t)d->SN * d->V;
+        bsq_hard_grad_table_kernel<<<(unsigned)((nv + 255) / 256), 256, 0, stream>>>(d->SN, C, sv.abar, ws.hb_G, ws.hb_GT);
+        XQ_LAUNCH_CHECK("bsq_hard_grad_table_kernel");
+        const size_t hsmem = sizeof(float) * hb_bwd_smem_floats(C);
+        if ((rc = smem_optin(bsq_hard_bwd_kernel, hsmem)) != XQ_OK) return rc;
+        const int rows = d->B * H * W;
+        bsq_hard_bwd_kernel<<<(rows + HB_RC - 1) / HB_RC, HB_THREADS, hsmem, stream>>>(*d, a.fn, sv.Fprev, n_quantizers, ws.hb_G,
+                                                                                      ws.hb_GT, g_entropy, ws.gent);
+        XQ_LAUNCH_CHECK("bsq_hard_bwd_kernel");
         a.gent = ws.gent;
     }
     a.gf = gf; a.gE = bsq ? nullptr : gE;
@@ -1232,7 +1590,7 @@ int xq_ms_decode(const xq_ms_desc *d, const int64_t *idx_all, const float *E, co
     int rc = ms_check(d);
     if (rc != XQ_OK) return rc;
     if (!idx_all) return XQ_ERR_ARG;
-    const bool bsq = d->mode == XQ_MS_BSQ;
+    const bool bsq = ms_is_bsq(d->mode);
     if (!bsq && !E) return XQ_ERR_ARG;
     if (d->K > 0 && (!phi_w || !phi_b)) return XQ_ERR_ARG;
     size_t smem = sizeof(float) * ms_fwd_smem_floats(d->C, d->H, d->W, d->SN, false);

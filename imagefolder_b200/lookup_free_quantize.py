@@ -3,11 +3,16 @@ tokenizer/tokenizer_image/lookup_free_quantize.py (LFQ :83).
 
 Same constructor, return 5-tuple and state_dict keys (`ema_vocab_hit_SV`, `scaler`,
 `quant_resi.qresi_ls.*`; non-persistent `mask`, `codebook`).  The arithmetic runs in
-libxqb200.so (csrc/ms_kernels.cu: ms_forward_kernel mode XQ_MS_BSQ + bsq_entropy_*_kernel).
+libxqb200.so (csrc/ms_kernels.cu: ms_forward_kernel mode XQ_MS_BSQ + bsq_entropy_*_kernel, or mode
+XQ_MS_BSQ_HARD + bsq_hard_*_kernel for soft_entropy=False).
 
 Reference behaviour that is kept on purpose:
-  * the entropy term indexes the batch with an INT mask (`z[mask]`, :285) and therefore only ever
-    looks at batch rows 0 and 1 -- reproduced exactly (and B >= 2 is required like there);
+  * soft_entropy=True: the entropy term indexes the batch with an INT mask (`z[mask]`, :285) and therefore
+    only ever looks at batch rows 0 and 1 -- reproduced exactly (and B >= 2 is required like there);
+  * soft_entropy=False: entropy_loss over the 2^C-code softmax (:41-79, :220-229), a real masked mean over
+    every image that still quantizes at the scale.  It is evaluated in closed form (per-bit sigmoids; the
+    codebook distribution as a 2^(C/2) x 2^(C - C/2) contraction), so the [B, HW, 2^C] logits are never built.
+    1 <= C <= 16; B == 1 raises like the reference (einops cannot reduce its 0-d masked mean);
   * all three losses are divided by SN (:238-240), unlike VectorQuantizer2;
   * the dead einsum + softmax over the 2^C codebook (:286-287, result overwritten) is NOT computed.
 """
@@ -92,16 +97,21 @@ class LFQ(_MultiScaleBase):
         if not self.training:
             # the reference's eval branch raises (list + int, :174)
             raise TypeError('can only concatenate list (not "int") to list')
-        if not self.soft_entropy:
-            raise NotImplementedError("soft_entropy=False (full 2^C softmax entropy, :221-229) is not built; "
-                                      "every shipped config uses soft_entropy=True")
+        if not self.soft_entropy and self.Cvae > 16:
+            raise NotImplementedError(f"soft_entropy=False is built for 1 <= Cvae <= 16 (got {self.Cvae})")
         if f_BChw.dtype != torch.float32:
             f_BChw = f_BChw.float()
         B, Cc, H, W = f_BChw.shape
         if B < 2:
-            # soft_entropy_loss gathers batch rows with the int mask (values 0/1), :285
-            raise IndexError(f"index 1 is out of bounds for dimension 0 with size {B}")
+            if self.soft_entropy:
+                # soft_entropy_loss gathers batch rows with the int mask (values 0/1), :285
+                raise IndexError(f"index 1 is out of bounds for dimension 0 with size {B}")
+            # entropy_loss: mask.squeeze() is 0-d, masked_mean returns a 0-d tensor and einops' "... D -> D" raises (:62)
+            raise RuntimeError('Error while processing mean-reduction pattern "... D -> D": expected >=1 dims, '
+                               'received a 0-dim tensor (batch size 1)')
         d, w, b, pns = self._desc(B, H, W)
+        if not self.soft_entropy:
+            d.mode = C.XQ_MS_BSQ_HARD
         nq = self._n_quantizers(B, dropout, f_BChw.device, require_dropout=True)
         f_hat, vq, commit, ent, idx_all, hist = ops.ms_forward(f_BChw, None, w, b, nq, d, want_hist=True)
         usages = self._update_usage(hist, f_BChw.numel() / f_BChw.shape[1], ret_usages)

@@ -152,7 +152,7 @@ class _MSForward(torch.autograd.Function):
         hist = torch.zeros(desc.SN, desc.V, dtype=torch.float32, device=dev) if want_hist else None
         saved = C.workspace(L.xq_ms_saved_bytes(desc), dev)
         ws = C.workspace(L.xq_ms_workspace_bytes(desc), dev)
-        nk = 2 + (1 if desc.channel_norm else 0) + (1 if E is not None else 1)
+        nk = 2 + (1 if desc.channel_norm else 0) + (1 if E is not None else 1) + (1 if desc.mode == C.XQ_MS_BSQ_HARD else 0)
         C.call("xq_ms_forward", nk, L.xq_ms_forward, desc, C.ptr(f), C.ptr(E), C.ptr(phi_w), C.ptr(phi_b), C.ptr(nq), 1,
                C.ptr(out), C.ptr(idx_all), None, C.ptr(loss), C.ptr(hist), C.ptr(saved), C.ptr(ws), ws.numel(),
                C.stream_ptr(dev))
@@ -180,6 +180,7 @@ class _MSForward(torch.autograd.Function):
         gb = torch.empty_like(phi_b) if phi_b is not None else None
         ws = C.workspace(L.xq_ms_workspace_bytes(desc), dev)
         nk = 1 + (2 if phi_w is not None else 0) + (1 if (E is None and g_ent is not None) else 0)
+        nk += 1 if (desc.mode == C.XQ_MS_BSQ_HARD and g_ent is not None) else 0
         C.call("xq_ms_backward", nk, L.xq_ms_backward, desc, C.ptr(f), C.ptr(E), C.ptr(phi_w), C.ptr(phi_b), C.ptr(nq),
                C.ptr(idx_all), C.ptr(saved), C.ptr(g_out), C.ptr(g_vq), C.ptr(g_commit), C.ptr(g_ent), C.ptr(gf),
                C.ptr(gE), C.ptr(gw), C.ptr(gb), C.ptr(ws), ws.numel(), C.stream_ptr(dev))

@@ -104,6 +104,18 @@ int xq_perturb_backward(const float *z_nchw, const float *g_nchw, int B, int C, 
 #define XQ_MS_VQ_ZNORM 0 /* VectorQuantizer2, using_znorm=True  (argmax cosine)        */
 #define XQ_MS_VQ_L2 1    /* VectorQuantizer2, using_znorm=False (argmin L2)            */
 #define XQ_MS_BSQ 2      /* LFQ: sign bits, code = +-scaler[si]                        */
+/* LFQ(soft_entropy=False): the same quantizer, with the entropy term of entropy_loss (lookup_free_quantize.py:41-79,
+ * 220-229), the softmax over all 2^C codes at temperature 0.01, evaluated in closed form instead of the soft path's
+ * per-bit approximation.  Per scale si and masked row r (every position of every image b with si < n_quantizers[b]):
+ *   q_rk = sigmoid(400 * scaler[si] * x_rk),  x = f (normalised when channel_norm) - f_hat before scale si
+ *   sample entropy  S  = mean_r sum_k H_b(q_rk)
+ *   codebook entropy Hc = -sum_j a_j log(a_j + 1e-5),  a_j = mean_r prod_k q_rk(bit k of j)  (bits little-endian),
+ *     a = A^T Bm over the low floor(C/2) / high bits, contracted in fp32 on the CUDA cores in a fixed order
+ *   entropy = mean_si (w_sample S - w_batch Hc) * entropy_weight / (n1 / B)
+ * The backward carries the gradient to every image.  Deterministic: no atomics, fixed reduction order.
+ * Refusals: C > 16 -> XQ_ERR_UNSUPPORTED (the 2^C code-probability table is kept per scale).  B == 1 is accepted here
+ * (the reference module raises for it; imagefolder_b200 mirrors that in Python). */
+#define XQ_MS_BSQ_HARD 3
 
 typedef struct {
     int B, C, H, W;       /* f is [B,C,H,W]                                             */
