@@ -120,6 +120,10 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_fc1_gelu_fwd.argtypes = [vp, vp, f32p, vp, vp, c_int, c_int, c_int, vp]
     L.xq_vit_fc2_dgelu_bwd.restype = c_int
     L.xq_vit_fc2_dgelu_bwd.argtypes = [vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, vp]
+    L.xq_vit_fc1_lora_gelu_fwd.restype = c_int
+    L.xq_vit_fc1_lora_gelu_fwd.argtypes = [vp, vp, vp, vp, f32p, vp, vp, c_int, c_int, c_int, c_int, vp]
+    L.xq_vit_fc2_lora_dgelu_bwd.restype = c_int
+    L.xq_vit_fc2_lora_dgelu_bwd.argtypes = [vp, vp, vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, c_int, vp]
     L.xq_lpips_workspace_bytes.restype = c_size_t
     L.xq_lpips_workspace_bytes.argtypes = [c_int, c_int]
     L.xq_lpips_layer_forward.restype = c_int
@@ -227,7 +231,7 @@ EXPORTED_SYMBOLS = [
     "xq_vq_backward", "xq_perturb_workspace_bytes", "xq_perturb_forward", "xq_perturb_backward",
     "xq_ms_workspace_bytes", "xq_ms_saved_bytes", "xq_ms_total_tokens", "xq_ms_forward", "xq_ms_backward",
     "xq_ms_decode", "xq_ms_embed", "xq_usage_ema", "xq_usage_ema_dev", "xq_vit_residual_ln_fwd", "xq_vit_ln_bwd_workspace_bytes",
-    "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd",
+    "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd", "xq_vit_fc2_lora_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
     "xq_ema_update", "xq_adamw_step", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",

@@ -7,6 +7,12 @@
 //   xq_vit_fc1_gelu_fwd   pre = y W1^T (bf16) ; act = GELU(pre + b1)                       [epilogue writes both]
 //   xq_vit_fc2_dgelu_bwd  d_pre = (d_branch W2) * GELU'(pre + b1) ; d_b1 = colsum(d_pre)    [epilogue reads pre]
 // (the other four GEMMs of the block -- fc2 forward, the two weight gradients, the fc1 input gradient -- stay plain cuBLAS calls).
+// Their LoRA forms (fc1 / fc2 wrapped by dino_enc/lora.py, u = s y A1^T and v = s d_branch B2 rank-R activations, R <= 64):
+//   xq_vit_fc1_lora_gelu_fwd   pre = y W1^T + u B1^T                 ; act = GELU(pre + b1)
+//   xq_vit_fc2_lora_dgelu_bwd  d_pre = (d_branch W2 + v A2) * GELU'(pre + b1) ; d_b1 = colsum(d_pre)
+// are the same kernel with one more K stage: the producer loads the [128][64] tiles of u / v and of the K-major adapter
+// (B1 [N,R], A2^T [N,R]) after the main K loop, TMA zero-filling the columns >= R, and the MMA warps accumulate it into the
+// same fp32 accumulators before the single rounding to bf16.
 //
 // C[M,N] = A[M,K] . B[N,K]^T, A and B K-major (row-major as PyTorch stores activations and Linear weights), bf16 in, fp32
 // accumulation in registers.  A CTA owns a 128 x 128 tile and is persistent: CTA p keeps column block p % (N/128) for the whole
@@ -85,13 +91,15 @@ struct GmClock {
 // Both apply the element-wise function to the ROUNDED bf16 value of the GEMM result, i.e. exactly what the stand-alone
 // kernels compute from the tensor a library GEMM would have written.
 //
+// R > 0: the rank-R tail stage (tmU: [M,R] activation, tmL: [N,R] adapter) follows the nk stages of the main K loop.
 // Barriers: full / empty per ring stage; stg_full (the 8 MMA warps have written the staging tile) / stg_empty (the epilogue
 // is done with it); aux_full / aux_empty per auxiliary tile (backward: the `pre` tile has landed / its store has been read).
 template <int EPI>
 __global__ void __launch_bounds__(GM_THREADS, 1)
 mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmO, const float *__restrict__ bias,
-                float *__restrict__ dbias, int M, int N, int K) {
+                const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmO,
+                const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmL, const float *__restrict__ bias,
+                float *__restrict__ dbias, int M, int N, int K, int R) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t *stg = base + GM_STG_OFF;
@@ -108,7 +116,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         mbar_fence_init();
     }
     // schedule: CTA p keeps column block nb, walks 128-row blocks mb0, mb0 + mstep, ...; t counts its tiles
-    const int nN = N / GM_BN, nM = (M + GM_BM - 1) / GM_BM, nk = K / GM_BK;
+    const int nN = N / GM_BN, nM = (M + GM_BM - 1) / GM_BM, nk = K / GM_BK, nks = nk + (R > 0);
     const int nb = blockIdx.x % nN, mstep = gridDim.x / nN, mb0 = blockIdx.x / nN;
     __syncthreads();
     GmClock clk;
@@ -118,18 +126,23 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             tma_prefetch_desc(&tmA);
             tma_prefetch_desc(&tmB);
             if (EPI == 2) tma_prefetch_desc(&tmP);
+            if (R > 0) { tma_prefetch_desc(&tmU); tma_prefetch_desc(&tmL); }
         }
         __syncwarp();
         int it = 0, t = 0;
         for (int mb = mb0; mb < nM; mb += mstep, ++t) {
             bool pre_sent = false;
-            for (int kb = 0; kb < nk; ++kb, ++it) {
+            for (int kb = 0; kb < nks; ++kb, ++it) {
                 const int st = it % GM_NST;
                 mbar_wait(&empty[st], ((it / GM_NST) & 1) ^ 1);
                 if (elect_one()) {
+                    // the rank-R stage: columns >= R of both boxes are zero-filled and count towards the transaction bytes
+                    const bool tail = kb == nk;
                     mbar_expect_tx(&full[st], GM_ST_BYTES);
-                    tma_load_3d(base + st * GM_ST_BYTES, &tmA, kb * GM_BK, mb * GM_BM, 0, &full[st]);      // rows >= M: zero-filled
-                    tma_load_3d(base + st * GM_ST_BYTES + GM_A_BYTES, &tmB, kb * GM_BK, nb * GM_BN, 0, &full[st]);
+                    tma_load_3d(base + st * GM_ST_BYTES, tail ? &tmU : &tmA, tail ? 0 : kb * GM_BK, mb * GM_BM, 0,
+                                &full[st]);                                                        // rows >= M: zero-filled
+                    tma_load_3d(base + st * GM_ST_BYTES + GM_A_BYTES, tail ? &tmL : &tmB, tail ? 0 : kb * GM_BK, nb * GM_BN, 0,
+                                &full[st]);
                 }
                 __syncwarp();
                 // backward: the stored pre-activation tile goes to the auxiliary tile as soon as the epilogue has released it
@@ -138,7 +151,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 if (EPI == 2 && !pre_sent) {
                     uint64_t *e = &aux_empty[t & 1];
                     const uint32_t par = ((t >> 1) & 1) ^ 1;
-                    if (kb == nk - 1) mbar_wait(e, par);
+                    if (kb == nks - 1) mbar_wait(e, par);
                     else if (!__any_sync(0xffffffffu, mbar_test(e, par))) continue;
                     uint8_t *aux = base + GM_AUX_OFF + (t & 1) * GM_TILE_BYTES;
                     if (elect_one()) {
@@ -271,7 +284,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         int prev = -1;
-        for (int kb = 0; kb < nk; ++kb, ++it) {
+        for (int kb = 0; kb < nks; ++kb, ++it) {
             const int st = it % GM_NST;
             mbar_wait(&full[st], (it / GM_NST) & 1);
             const uint64_t ad = desc_k_sw128(smem_u32(base + st * GM_ST_BYTES + wg * (GM_A_BYTES / 2)));
@@ -314,10 +327,18 @@ static int gm_check(const void *a, const void *b, const void *c, const void *c2,
     return XQ_OK;
 }
 
+// the LoRA entry points' extra operands: u / v [M,R] and the K-major adapter [N,R]; R % 8 == 0 keeps their rows 16-byte aligned
+static int gm_check_lora(const void *u, const void *l, int R) {
+    if (!u || !l || R < 8 || R > GM_BK || R % 8 != 0) return XQ_ERR_ARG;
+    if ((((uintptr_t)u | (uintptr_t)l) & 15) != 0) return XQ_ERR_ARG;
+    return XQ_OK;
+}
+
 // `pre` is the pre-activation tensor (written by the forward, read by the backward), `out` the epilogue's result (act / d_pre)
 template <int EPI>
-static int gm_launch(const void *a, const void *b, const void *pre, void *out, const float *bias, float *dbias, int M, int N, int K,
-                     cudaStream_t st) {
+// R > 0 adds the rank-R stage u [M,R] . l [N,R]^T; R == 0 ignores u / l
+static int gm_launch(const void *a, const void *b, const void *u, const void *l, const void *pre, void *out, const float *bias,
+                     float *dbias, int M, int N, int K, int R, cudaStream_t st) {
     int sms = 0;
     if (int rc = sm_count(&sms)) return rc;
     const int nN = N / GM_BN;
@@ -328,13 +349,17 @@ static int gm_launch(const void *a, const void *b, const void *pre, void *out, c
         !tensor_map_bf16_3d(&tmP, pre, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM) ||
         !tensor_map_bf16_3d(&tmO, out, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM))
         return XQ_ERR_UNSUPPORTED;
+    CUtensorMap tmU = tmA, tmL = tmB;
+    if (R > 0 && (!tensor_map_bf16_3d(&tmU, u, R, M, 1, (uint64_t)R * 2, (uint64_t)M * R * 2, GM_BM) ||
+                  !tensor_map_bf16_3d(&tmL, l, R, N, 1, (uint64_t)R * 2, (uint64_t)N * R * 2, GM_BN)))
+        return XQ_ERR_UNSUPPORTED;
     if (int rc = smem_optin(mlp_gemm_kernel<EPI>, GM_SMEM)) return rc;
     const int nM = (M + GM_BM - 1) / GM_BM;
     int per_col = sms / nN;                               // CTAs per column block
     if (per_col > nM) per_col = nM;
     // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
     if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st));
-    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, bias, dbias, M, N, K);
+    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, tmU, tmL, bias, dbias, M, N, K, R);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
     return XQ_OK;
 }
@@ -345,14 +370,29 @@ extern "C" {
 
 int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream) {
     if (int rc = xq::gm_check(x, w, pre, act, bias, M, N, K)) return rc;
-    return xq::gm_launch<1>(x, w, pre, act, bias, nullptr, M, N, K, (cudaStream_t)stream);
+    return xq::gm_launch<1>(x, w, nullptr, nullptr, pre, act, bias, nullptr, M, N, K, 0, (cudaStream_t)stream);
 }
 
 int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias, int M,
                          int N, int K, void *stream) {
     if (int rc = xq::gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
     if (!d_bias) return XQ_ERR_ARG;
-    return xq::gm_launch<2>(d_out, w2t, pre, d_pre, bias, d_bias, M, N, K, (cudaStream_t)stream);
+    return xq::gm_launch<2>(d_out, w2t, nullptr, nullptr, pre, d_pre, bias, d_bias, M, N, K, 0, (cudaStream_t)stream);
+}
+
+int xq_vit_fc1_lora_gelu_fwd(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre, void *act,
+                             int M, int N, int K, int R, void *stream) {
+    if (int rc = xq::gm_check(x, w, pre, act, bias, M, N, K)) return rc;
+    if (int rc = xq::gm_check_lora(u, b_lora, R)) return rc;
+    return xq::gm_launch<1>(x, w, u, b_lora, pre, act, bias, nullptr, M, N, K, R, (cudaStream_t)stream);
+}
+
+int xq_vit_fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre, const float *bias,
+                              void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream) {
+    if (int rc = xq::gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
+    if (int rc = xq::gm_check_lora(v, a2t, R)) return rc;
+    if (!d_bias) return XQ_ERR_ARG;
+    return xq::gm_launch<2>(d_out, w2t, v, a2t, pre, d_pre, bias, d_bias, M, N, K, R, (cudaStream_t)stream);
 }
 
 #ifdef XQ_GM_CLOCKS

@@ -1,8 +1,8 @@
 """DINOv2Encoder / DINOv2Decoder -- drop-in for tokenizer/tokenizer_image/dino_enc/dinov2.py
 (:18 and :201): ViT backbone + learnable latent tokens, level embedding, mask tokens, ToPixel.
 
-Only tuning_method 'full' / 'frozen' are built (peft LoRA variants need the un-vendored peft
-package and are not selected by any shipped config, xqgan_model.py:96,114).
+tuning_method 'full', 'frozen', 'lora' and 'lora_unfreeze_patch_embed' are built, in the constructors and in `finetine`; the
+LoRA ones wrap the ViT with lora.py, a restatement of the peft 0.13.0 calls the reference makes.  'lat_lora' is not built.
 Sub-module / parameter names match the reference so released checkpoints load unchanged.
 
 Both classes split their forward into (1) the token ASSEMBLY -- everything between the batch-dependent rows (patch
@@ -19,11 +19,16 @@ import torch
 import torch.nn as nn
 
 from ..vit_ops import assemble_tokens, patch_embed, run_blocks
+from .lora import LoraConfig, get_peft_model
 from .to_pixel import ToPixel
 from .vision_transformer import Attention, create_model, trunc_normal_
 
 _NAMES = ['vit_small_patch14_dinov2.lvd142m', 'vit_base_patch14_dinov2.lvd142m', 'vit_large_patch14_dinov2.lvd142m']
-_LORA_MSG = "tuning_method={!r} needs peft (LoRA); not built"
+# modules_to_save of the reference's two LoRA methods (dinov2.py:57, 63); both adapt exactly the MLP Linears
+_LORA_SAVE = {'lora': ['norm'], 'lora_unfreeze_patch_embed': ['patch_embed.proj', 'patch_embed.norm', 'norm']}
+_LORA_TARGETS = r".*\.mlp\.fc\d"
+_LAT_LORA_MSG = ("tuning_method='lat_lora' needs models.peft_models.lora.LatentLoRALinear, which the reference imports "
+                 "(dinov2.py:69, 132) but does not contain; not built")
 
 
 def _autocast_off(x):
@@ -40,13 +45,27 @@ def _freeze(module):
         param.requires_grad = False
 
 
-def _adopt_backbone(owner, model, tuning_method):
-    """`self.model = model` for 'full', the same with frozen parameters for 'frozen' (dinov2.py:41-62 / 228-249)."""
-    if tuning_method not in ('full', 'frozen'):
-        raise NotImplementedError(_LORA_MSG.format(tuning_method))
+def _tuned(model, tuning_method, tuning_kwargs):
+    """the backbone for `tuning_method` (dinov2.py:51-80 / 114-142 / 241-253 / 291-304): `model` itself for 'full', with
+    frozen parameters for 'frozen', wrapped with rank-r adapters on every mlp.fc1 / mlp.fc2 for the LoRA methods"""
+    if tuning_method == 'full':
+        return model
     if tuning_method == 'frozen':
         _freeze(model)
-    owner.model = model
+        return model
+    if tuning_method in _LORA_SAVE:
+        peft_model = get_peft_model(model, LoraConfig(target_modules=_LORA_TARGETS, modules_to_save=_LORA_SAVE[tuning_method],
+                                                      **tuning_kwargs))
+        peft_model.print_trainable_parameters()
+        return peft_model
+    if tuning_method == 'lat_lora':
+        raise NotImplementedError(_LAT_LORA_MSG)
+    raise NotImplementedError(f"tuning_method={tuning_method!r} is not one of the reference's; not built")
+
+
+def _adopt_backbone(owner, model, tuning_method, tuning_kwargs):
+    """`self.model` = the backbone tuned by `tuning_method` (dinov2.py:51-80 / 241-253)."""
+    owner.model = _tuned(model, tuning_method, tuning_kwargs)
     owner.embed_dim = model.embed_dim
     owner.num_img_tokens = model.patch_embed.num_patches
     owner.num_prefix_tokens = model.num_prefix_tokens
@@ -74,10 +93,7 @@ def _static_sequence(vit, training):
 
 class _Tunable:
     def finetine(self, tuning_method, tuning_kwargs={'r': 8}):            # (sic) the reference's spelling
-        if tuning_method == 'frozen':
-            _freeze(self.model)
-        elif tuning_method != 'full':
-            raise NotImplementedError(_LORA_MSG.format(tuning_method))
+        self.model = _tuned(self.model, tuning_method, tuning_kwargs)
 
 
 class DINOv2Encoder(_Tunable, nn.Module):
@@ -89,7 +105,7 @@ class DINOv2Encoder(_Tunable, nn.Module):
         assert model_name in _NAMES, f"{model_name} not found"
         self.num_latent_tokens, self.use_attn_mask = num_latent_tokens, use_attn_mask
         self.product_quant, self.abs_pos_embed = product_quant, abs_pos_embed
-        _adopt_backbone(self, create_model(model_name, pretrained=pretrained, **model_kwargs), tuning_method)
+        _adopt_backbone(self, create_model(model_name, pretrained=pretrained, **model_kwargs), tuning_method, tuning_kwargs)
         if not num_latent_tokens:
             return
         D, L = self.embed_dim, num_latent_tokens
@@ -157,7 +173,12 @@ class DINOv2Decoder(_Tunable, nn.Module):
         self.use_rope, self.cond_latent = use_rope, cond_latent
         self.num_latent_tokens, self.abs_pos_embed = num_latent_tokens, abs_pos_embed
         vit_kwargs = dict(model_kwargs, num_latent_tokens=num_latent_tokens, attn_layer=Attention)
-        _adopt_backbone(self, create_model(model_name, pretrained=pretrained, **vit_kwargs), tuning_method)
+        model = create_model(model_name, pretrained=pretrained, **vit_kwargs)
+        # the decoder never embeds pixels: drop the unused projection so that it is neither trained nor checkpointed (before
+        # any LoRA wrapping, so that a saved copy of patch_embed.proj holds no parameters either)
+        del model.patch_embed.proj.bias
+        del model.patch_embed.proj.weight
+        _adopt_backbone(self, model, tuning_method, tuning_kwargs)
         D = self.embed_dim
         self.mask_token = nn.Parameter(torch.zeros(1, 1, D))
         nn.init.normal_(self.mask_token, std=1e-6)
@@ -169,9 +190,6 @@ class DINOv2Decoder(_Tunable, nn.Module):
             trunc_normal_(self.latent_pos_embed, std=.02)
         self.to_pixel = ToPixel(to_pixel=to_pixel, img_size=model_kwargs['img_size'], in_channels=in_channels, in_dim=D,
                                 patch_size=model_kwargs['patch_size'])
-        # the decoder never embeds pixels: drop the unused projection so that it is neither trained nor checkpointed
-        del self.model.patch_embed.proj.bias
-        del self.model.patch_embed.proj.weight
 
     def no_weight_decay(self):
         return ['model.pos_embed', 'model.cls_token', 'model.dist_token', 'mask_token', 'latent_pos_embed']

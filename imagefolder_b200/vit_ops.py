@@ -22,6 +22,16 @@ from ._capi import call as _call, lib as _lib, ptr as _ptr, stream_ptr as _strea
 _SUPPORTED_D = (384, 768, 1024)
 
 
+def _lora():
+    from .dino_enc import lora          # imported here: dino_enc imports this module
+    return lora
+
+
+def _live(m):
+    """the module that runs `m`'s forward: the trainable copy of a LoRA `modules_to_save` wrapper (dino_enc/lora.py), else `m`"""
+    return _lora().active_module(m)
+
+
 class _ResidualLN(torch.autograd.Function):
     """(x, branch, branch_bias, ls_gamma, rowscale, ln_w, ln_b) -> (x_out fp32, y bf16)
     x_out = x + rowscale * ls_gamma * (branch + branch_bias);  y = LayerNorm(x_out)."""
@@ -192,13 +202,119 @@ class _FusedMLP(torch.autograd.Function):
         return dy, dW1, (db1 if ctx.needs_input_grad[2] else None), dW2
 
 
+def _scaled_mm(a, b, s: float):
+    """bf16(s * (a @ b)): the scale applied to the fp32 accumulator, one rounding"""
+    return torch.addmm(a.new_zeros(()), a, b, beta=0, alpha=s)
+
+
+def _pad_rank(t, dim: int, R: int):
+    """zero rows (dim 0) / columns (dim 1) up to rank R: the kernel's rank stage needs R % 8 == 0"""
+    n = t.shape[dim]
+    if n == R:
+        return t.contiguous()
+    return F.pad(t, (0, R - n) if dim == 1 else (0, 0, 0, R - n))
+
+
+class _LoRAMLP(torch.autograd.Function):
+    """branch = fc2(GELU(fc1(y))) WITHOUT the fc2 bias, fc1 / fc2 LoRA-wrapped (dino_enc/lora.py, lora_dropout inactive):
+    fc(x) = x W^T + b + s (x A^T) B^T.  With u = bf16(s1 y A1^T) and v = bf16(s2 g B2) (rank-r library GEMMs):
+      forward   pre = y W1^T + u B1^T, act = GELU(pre + b1)      xq_vit_fc1_lora_gelu_fwd (u B1^T: one more K stage)
+                branch = act W2^T + s2 (act A2^T) B2^T           library
+      backward  d_pre = (g W2 + v A2) * GELU'(pre + b1), d_b1   xq_vit_fc2_lora_dgelu_bwd
+                dy = d_pre W1 + s1 (d_pre B1) A1, the four adapter gradients, and dW1 / dW2 / d_b1 only for parameters that
+                require grad (LoRA freezes them: their GEMMs are not run).
+    The base and rank-r products of `pre` / `d_act` share one fp32 accumulator and one rounding (DESIGN.md section 8)."""
+
+    @staticmethod
+    def forward(ctx, y, W1, b1, W2, A1, B1, A2, B2, s1: float, s2: float):
+        K, N = W1.shape[1], W1.shape[0]
+        y2 = y.reshape(-1, K)
+        if not y2.is_contiguous():
+            y2 = y2.contiguous()
+        M = y2.shape[0]
+        r = A1.shape[0]
+        R = -(-r // 8) * 8
+        bf = torch.bfloat16
+        W1b, W2b, b1f = W1.to(bf), W2.to(bf), b1.float()
+        A1b, B1b = _pad_rank(A1.to(bf), 0, R), _pad_rank(B1.to(bf), 1, R)           # [R, K], [N, R]
+        A2b, B2b = _pad_rank(A2.to(bf), 0, R), _pad_rank(B2.to(bf), 1, R)           # [R, N], [Ko, R]
+        u = _scaled_mm(y2, A1b.t(), s1)
+        pre = torch.empty(M, N, dtype=bf, device=y.device)
+        act = torch.empty(M, N, dtype=bf, device=y.device)
+        L = C.lib()
+        C.call("xq_vit_fc1_lora_gelu_fwd", 1, L.xq_vit_fc1_lora_gelu_fwd, C.ptr(y2), C.ptr(W1b), C.ptr(u), C.ptr(B1b), C.ptr(b1f),
+               C.ptr(pre), C.ptr(act), M, N, K, R, C.stream_ptr(y.device),
+               nbytes=M * (K + R) * 2 + N * (K + R) * 2 + M * N * 4, nflops=2.0 * M * N * (K + R))
+        h2 = _scaled_mm(act, A2b.t(), s2)
+        branch = torch.addmm(act @ W2b.t(), h2, B2b.t())
+        ctx.save_for_backward(y2, pre, act, u, h2, W1b, W2b, b1f, A1b, B1b, A2b, B2b)
+        ctx.cfg = (s1, s2, r)
+        ctx.out_shape = y.shape[:-1] + (W2.shape[0],)
+        ctx.in_shape = y.shape
+        return branch.view(ctx.out_shape)
+
+    @staticmethod
+    def backward(ctx, g):
+        y2, pre, act, u, h2, W1b, W2b, b1f, A1b, B1b, A2b, B2b = ctx.saved_tensors
+        s1, s2, r = ctx.cfg
+        need = ctx.needs_input_grad
+        M, N = pre.shape
+        Ko, R = W2b.shape[0], A1b.shape[0]
+        g2 = g.reshape(M, Ko)
+        if g2.dtype != torch.bfloat16:
+            g2 = g2.to(torch.bfloat16)
+        if not g2.is_contiguous():
+            g2 = g2.contiguous()
+        v = _scaled_mm(g2, B2b, s2)                     # [M, R]
+        W2t = W2b.t().contiguous()                      # [hidden, out]: the K-major B operand of d_act = g W2
+        A2t = A2b.t().contiguous()                      # [hidden, R]: the K-major adapter of the rank stage v A2
+        dpre = torch.empty_like(pre)
+        db1 = torch.empty(N, dtype=torch.float32, device=pre.device)
+        L = C.lib()
+        C.call("xq_vit_fc2_lora_dgelu_bwd", 1, L.xq_vit_fc2_lora_dgelu_bwd, C.ptr(g2), C.ptr(W2t), C.ptr(v), C.ptr(A2t), C.ptr(pre),
+               C.ptr(b1f), C.ptr(dpre), C.ptr(db1), M, N, Ko, R, C.stream_ptr(pre.device),
+               nbytes=M * (Ko + R) * 2 + N * (Ko + R) * 2 + M * N * 4, nflops=2.0 * M * N * (Ko + R))
+        t1 = _scaled_mm(dpre, B1b, s1)                  # [M, R] = s1 d_pre B1
+        dy = torch.addmm(dpre @ W1b, t1, A1b).view(ctx.in_shape) if need[0] else None
+        dW1 = (dpre.t() @ y2).float() if need[1] else None
+        dW2 = (g2.t() @ act).float() if need[3] else None
+        dA1 = (t1.t() @ y2).float()[:r] if need[4] else None
+        dB1 = (dpre.t() @ u).float()[:, :r] if need[5] else None
+        dA2 = (v.t() @ act).float()[:r] if need[6] else None
+        dB2 = (g2.t() @ h2).float()[:, :r] if need[7] else None
+        return dy, dW1, (db1 if need[2] else None), dW2, dA1, dB1, dA2, dB2, None, None
+
+
+def _lora_off(fc) -> bool:
+    """a LoRA Linear whose lora_dropout does nothing"""
+    d = fc.lora_dropout[fc.active_adapter]
+    return isinstance(d, nn.Identity) or not d.training or d.p == 0.0
+
+
+def _linear_no_bias(fc, x):
+    """fc(x) without its bias, for an nn.Linear or a LoRA Linear"""
+    out = F.linear(x, fc.weight)
+    return out + fc.lora_delta(x) if isinstance(fc, _lora().Linear) else out
+
+
 def mlp_forward(mlp, y):
     """timm Mlp (fc1 -> GELU -> fc2, drop = 0) without the fc2 bias; fused wgmma path when the shapes allow, else library GEMMs +
-    the stand-alone bias / GELU kernel."""
-    if mlp_tc_ok(y, mlp.fc1, mlp.fc2):
-        return _FusedMLP.apply(y, mlp.fc1.weight, mlp.fc1.bias, mlp.fc2.weight)
-    h = gelu_bias(F.linear(y, mlp.fc1.weight), mlp.fc1.bias)
-    return F.linear(h, mlp.fc2.weight)
+    the stand-alone bias / GELU kernel.  LoRA-wrapped fc1 and fc2 with inactive lora_dropout and r <= 64 take the LoRA form of
+    the fused path; any other LoRA Linear adds its `lora_delta` to a library GEMM."""
+    fc1, fc2 = mlp.fc1, mlp.fc2
+    lora = _lora()
+    if isinstance(fc1, lora.Linear) or isinstance(fc2, lora.Linear):
+        if (isinstance(fc1, lora.Linear) and isinstance(fc2, lora.Linear) and _lora_off(fc1) and _lora_off(fc2)
+                and fc1.r[fc1.active_adapter] <= 64 and fc2.r[fc2.active_adapter] == fc1.r[fc1.active_adapter]
+                and mlp_tc_ok(y, fc1, fc2)):
+            a1, a2 = fc1.active_adapter, fc2.active_adapter
+            return _LoRAMLP.apply(y, fc1.weight, fc1.bias, fc2.weight, fc1.lora_A[a1].weight, fc1.lora_B[a1].weight,
+                                  fc2.lora_A[a2].weight, fc2.lora_B[a2].weight, fc1.scaling[a1], fc2.scaling[a2])
+        return _linear_no_bias(fc2, gelu_bias(_linear_no_bias(fc1, y), fc1.bias))
+    if mlp_tc_ok(y, fc1, fc2):
+        return _FusedMLP.apply(y, fc1.weight, fc1.bias, fc2.weight)
+    h = gelu_bias(F.linear(y, fc1.weight), fc1.bias)
+    return F.linear(h, fc2.weight)
 
 
 # The wgmma attention kernels (csrc/attn_kernel.cu).  False runs every block's attention through the module's own
@@ -211,7 +327,7 @@ def attn_tc_ok(attn, y) -> bool:
     an attention dropout of 0 where it applies (training)."""
     p = attn.attn_drop.p if attn.training else 0.0
     return (ATTN_TC_ENABLED[0] and y.is_cuda and y.dtype == torch.bfloat16 and p == 0.0 and attn.head_dim == 64
-            and isinstance(attn.q_norm, nn.Identity) and isinstance(attn.k_norm, nn.Identity))
+            and isinstance(_live(attn.q_norm), nn.Identity) and isinstance(_live(attn.k_norm), nn.Identity))
 
 
 def attn_tc_forward(qkv, num_heads: int):
@@ -330,17 +446,19 @@ class _PatchEmbed(torch.autograd.Function):
 
 def patch_embed_ok(pe, x) -> bool:
     p = pe.patch_size[0]
+    proj = _live(pe.proj)
     return (x.is_cuda and x.dtype == torch.float32 and not x.requires_grad and torch.is_autocast_enabled()
-            and torch.get_autocast_dtype("cuda") == torch.bfloat16 and isinstance(pe.norm, nn.Identity)
+            and torch.get_autocast_dtype("cuda") == torch.bfloat16 and isinstance(_live(pe.norm), nn.Identity)
             and pe.patch_size[0] == pe.patch_size[1] and p % 4 == 0 and x.shape[2] % p == 0 and x.shape[3] % p == 0
-            and tuple(pe.proj.stride) == tuple(pe.proj.kernel_size) and tuple(pe.proj.padding) == (0, 0))
+            and tuple(proj.stride) == tuple(proj.kernel_size) and tuple(proj.padding) == (0, 0))
 
 
 def patch_embed(pe, x):
     """PatchEmbed.forward on the fused path when it applies (bf16 autocast, fp32 CUDA image that needs no gradient,
     patch % 4 == 0, no norm); otherwise the module's own conv."""
     if patch_embed_ok(pe, x):
-        return _PatchEmbed.apply(x, pe.proj.weight, pe.proj.bias)
+        proj = _live(pe.proj)
+        return _PatchEmbed.apply(x, proj.weight, proj.bias)
     return pe(x)
 
 
@@ -448,5 +566,6 @@ def run_blocks(vit, x, attn_mask=None):
         bias = blk.mlp.fc2.bias
         gamma = blk.ls2.gamma if hasattr(blk.ls2, "gamma") else None
         rs = _droppath_scale(blk.drop_path2, Bn, dev)
-    _, y = residual_ln(x, branch, bias, gamma, rs, vit.norm.weight, vit.norm.bias, vit.norm.eps)
+    norm = _live(vit.norm)
+    _, y = residual_ln(x, branch, bias, gamma, rs, norm.weight, norm.bias, norm.eps)
     return y

@@ -306,6 +306,21 @@ int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *p
  *   ->  d_pre [M,N] = (d_out w2t^T) * GELU'(pre + bias) ,  d_bias [N] = column sums of the rounded d_pre                      */
 int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
                          int M, int N, int K, void *stream);
+/* LoRA forms of the two calls above, for fc1 / fc2 wrapped with rank-R adapters (imagefolder_b200/dino_enc/lora.py, peft's
+ * `base_layer(x) + lora_B(lora_A(x)) * scaling`).  The caller forms the rank-R activation; the kernel adds its product with
+ * the adapter as one more K stage, into the same fp32 accumulators, before the single rounding of the GEMM result:
+ *   u [M,R] = s x A1^T (bf16), b_lora [N,R] = lora_B of fc1 (bf16)
+ *     ->  pre [M,N] = x w^T + u b_lora^T ,  act [M,N] = GELU(pre + bias)
+ *   v [M,R] = s d_out B2 (bf16), a2t [N,R] = lora_A of fc2 TRANSPOSED (bf16)
+ *     ->  d_pre [M,N] = (d_out w2t^T + v a2t^T) * GELU'(pre + bias) ,  d_bias [N] = column sums of the rounded d_pre
+ * Equal, bit for bit, to xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd on the operands concatenated along K and zero-padded to
+ * K + 64 ([x | u], [w | b_lora]) up to the fp32 accumulation order.  Same checks and codes as those two, plus
+ * 8 <= R <= 64 with R % 8 == 0 and u / v, b_lora / a2t non-NULL and 16-byte aligned (else XQ_ERR_ARG).  A refused call writes
+ * nothing. */
+int xq_vit_fc1_lora_gelu_fwd(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre, void *act,
+                             int M, int N, int K, int R, void *stream);
+int xq_vit_fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre, const float *bias,
+                              void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream);
 
 /* ---- input pipeline: the training / validation image transforms (SURVEY.md section 8 row f-4, csrc/img_kernels.cu) ---------
  * Replaces the per-image CPU transform of the reference's DataLoader workers:
