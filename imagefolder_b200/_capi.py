@@ -39,6 +39,12 @@ class XqError(RuntimeError):
 
 
 _lib = None
+# ViT entry points with an `_f16` twin (include/xqb200.h): same arguments, fp16 instead of bf16 data
+F16_TWINS = [
+    "xq_vit_residual_ln_fwd", "xq_vit_residual_ln_bwd", "xq_vit_patchify", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd",
+    "xq_vit_attn_fwd", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd",
+    "xq_vit_fc2_lora_dgelu_bwd",
+]
 
 
 def lib() -> ctypes.CDLL:
@@ -124,6 +130,11 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_fc1_lora_gelu_fwd.argtypes = [vp, vp, vp, vp, f32p, vp, vp, c_int, c_int, c_int, c_int, vp]
     L.xq_vit_fc2_lora_dgelu_bwd.restype = c_int
     L.xq_vit_fc2_lora_dgelu_bwd.argtypes = [vp, vp, vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, c_int, vp]
+    # fp16 twins of the 16-bit ViT entry points: the same argument lists
+    for name in F16_TWINS:
+        twin = getattr(L, name + "_f16")
+        twin.restype = c_int
+        twin.argtypes = getattr(L, name).argtypes
     L.xq_lpips_workspace_bytes.restype = c_size_t
     L.xq_lpips_workspace_bytes.argtypes = [c_int, c_int]
     L.xq_lpips_layer_forward.restype = c_int
@@ -235,4 +246,4 @@ EXPORTED_SYMBOLS = [
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
     "xq_ema_update", "xq_adamw_step", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
-]
+] + [n + "_f16" for n in F16_TWINS]

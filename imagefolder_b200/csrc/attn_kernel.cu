@@ -1,4 +1,6 @@
-// attn_kernel.cu -- wgmma / TMA flash attention for the ViT blocks (head_dim 64, bf16, no mask), sm_90a.
+// attn_kernel.cu -- wgmma / TMA flash attention for the ViT blocks (head_dim 64, bf16 or f16, no mask), sm_90a.
+// Every kernel is a template over the 16-bit element type (xq_tc.cuh: Bf16 / F16); the `_f16` entry points are the f16
+// instantiations (fp16 autocast).  P, dS and the outputs are rounded to that type; lse, delta and the dQ accumulator are fp32.
 //
 // Replaces F.scaled_dot_product_attention in Attention.forward
 //   (tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197: q,k,v = qkv.reshape(B,N,3,H,hd).permute(2,0,3,1,4);
@@ -38,8 +40,9 @@ struct AttnFwdSmem {
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
+template <typename E>
 __global__ void __launch_bounds__(AT_THREADS, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16 *__restrict__ out, float *__restrict__ lse2, int N, int H,
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, typename E::T *__restrict__ out, float *__restrict__ lse2, int N, int H,
                 int nQ /* query tiles per (b,h) */, float c /* softmax scale * log2(e) */) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -107,7 +110,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16 *__rest
         const uint64_t kd = desc_k_sw128(smem_u32(base + AttnFwdSmem::K + st * AT_TILE));
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n128k16_ss<0, 0>(s, desc_adv(qd, k * 32), desc_adv(kd, k * 32), (uint32_t)k);
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n128k16_ss<E, 0, 0>(s, desc_adv(qd, k * 32), desc_adv(kd, k * 32), (uint32_t)k);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(s);
@@ -144,13 +147,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16 *__rest
             const float p0 = ex2_approx(fmaf(s[i], c, -mc[hh])), p1 = ex2_approx(fmaf(s[i + 1], c, -mc[hh]));
             l[hh] += p0 + p1;
             // accumulator group jj = i / 4 (8 keys); k-step jj / 2; register (jj & 1) * 2 + hh
-            pa[i >> 3][((i >> 2) & 1) * 2 + hh] = pack_bf16(p0, p1);
+            pa[i >> 3][((i >> 2) & 1) * 2 + hh] = E::pack(p0, p1);
         }
         mbar_wait(&v_full[st], ph);
         const uint64_t vd = desc_mn_sw128(smem_u32(base + AttnFwdSmem::V + st * AT_TILE), AT_TILE);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < AT_BN / 16; ++k) wgmma_m64n64k16_rs<1>(o, pa[k], desc_adv(vd, k * 2048), 1u);
+        for (int k = 0; k < AT_BN / 16; ++k) wgmma_m64n64k16_rs<E, 1>(o, pa[k], desc_adv(vd, k * 2048), 1u);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(o);
@@ -169,10 +172,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16 *__rest
         if (n >= N) continue;
         const float inv = 1.0f / l[hh];
         if (cq == 0) lse2[(size_t)bh * N + n] = fmaf(m[hh], c, log2f(l[hh]));
-        __nv_bfloat16 *orow = out + ((size_t)b * N + n) * H * AT_D + h * AT_D;
+        typename E::T *orow = out + ((size_t)b * N + n) * H * AT_D + h * AT_D;
 #pragma unroll
         for (int jj = 0; jj < AT_D / 8; ++jj)
-            *reinterpret_cast<uint32_t *>(orow + 8 * jj + cq) = pack_bf16(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+            *reinterpret_cast<uint32_t *>(orow + 8 * jj + cq) = E::pack(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
     }
 }
 
@@ -181,8 +184,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, __nv_bfloat16 *__rest
 // each with its own online softmax, merged by shuffles at the end.  Same outputs as the tile kernel (out row, lse2).
 constexpr int AT_TAIL_MAX = 0;     // 0: ragged query tiles always run on the tile kernel (dead warps skip the softmax math)
 
+template <typename E>
 __global__ void __launch_bounds__(128)
-attn_fwd_tail_kernel(const __nv_bfloat16 *__restrict__ qkv, __nv_bfloat16 *__restrict__ out, float *__restrict__ lse2, int B, int N,
+attn_fwd_tail_kernel(const typename E::T *__restrict__ qkv, typename E::T *__restrict__ out, float *__restrict__ lse2, int B, int N,
                      int H, int n0 /* first tail row */, float c) {
     const int lane = threadIdx.x & 31;
     const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -193,15 +197,15 @@ attn_fwd_tail_kernel(const __nv_bfloat16 *__restrict__ qkv, __nv_bfloat16 *__res
     const int b = bh / H, h = bh - b * H;
     const int n = n0 + r;
     const size_t W = (size_t)3 * H * AT_D;
-    const __nv_bfloat16 *qp = qkv + ((size_t)b * N + n) * W + h * AT_D;
+    const typename E::T *qp = qkv + ((size_t)b * N + n) * W + h * AT_D;
     float qf[AT_D];
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
         const uint4 x = *reinterpret_cast<const uint4 *>(qp + u * 8);
-        const __nv_bfloat162 *x2 = reinterpret_cast<const __nv_bfloat162 *>(&x);
+        const typename E::T2 *x2 = reinterpret_cast<const typename E::T2 *>(&x);
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            const float2 f = __bfloat1622float2(x2[e]);
+            const float2 f = E::to2(x2[e]);
             qf[u * 8 + 2 * e] = f.x * c;             // scores directly in the log2 domain
             qf[u * 8 + 2 * e + 1] = f.y * c;
         }
@@ -210,16 +214,16 @@ attn_fwd_tail_kernel(const __nv_bfloat16 *__restrict__ qkv, __nv_bfloat16 *__res
 #pragma unroll
     for (int i = 0; i < AT_D; ++i) o[i] = 0.f;
     for (int key = lane; key < N; key += 32) {
-        const __nv_bfloat16 *kp = qkv + ((size_t)b * N + key) * W + (H + h) * AT_D;
-        const __nv_bfloat16 *vp = kp + (size_t)H * AT_D;
+        const typename E::T *kp = qkv + ((size_t)b * N + key) * W + (H + h) * AT_D;
+        const typename E::T *vp = kp + (size_t)H * AT_D;
         float s = 0.f;
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
             const uint4 x = *reinterpret_cast<const uint4 *>(kp + u * 8);
-            const __nv_bfloat162 *x2 = reinterpret_cast<const __nv_bfloat162 *>(&x);
+            const typename E::T2 *x2 = reinterpret_cast<const typename E::T2 *>(&x);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float2 f = __bfloat1622float2(x2[e]);
+                const float2 f = E::to2(x2[e]);
                 s = fmaf(qf[u * 8 + 2 * e], f.x, s);
                 s = fmaf(qf[u * 8 + 2 * e + 1], f.y, s);
             }
@@ -232,10 +236,10 @@ attn_fwd_tail_kernel(const __nv_bfloat16 *__restrict__ qkv, __nv_bfloat16 *__res
 #pragma unroll
         for (int u = 0; u < 8; ++u) {
             const uint4 x = *reinterpret_cast<const uint4 *>(vp + u * 8);
-            const __nv_bfloat162 *x2 = reinterpret_cast<const __nv_bfloat162 *>(&x);
+            const typename E::T2 *x2 = reinterpret_cast<const typename E::T2 *>(&x);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float2 f = __bfloat1622float2(x2[e]);
+                const float2 f = E::to2(x2[e]);
                 o[u * 8 + 2 * e] = fmaf(o[u * 8 + 2 * e], corr, p * f.x);
                 o[u * 8 + 2 * e + 1] = fmaf(o[u * 8 + 2 * e + 1], corr, p * f.y);
             }
@@ -258,8 +262,8 @@ attn_fwd_tail_kernel(const __nv_bfloat16 *__restrict__ qkv, __nv_bfloat16 *__res
         if (i == 2 * lane) mine0 = x;
         if (i == 2 * lane + 1) mine1 = x;
     }
-    __nv_bfloat16 *op = out + ((size_t)b * N + n) * H * AT_D + h * AT_D;
-    *reinterpret_cast<uint32_t *>(op + 2 * lane) = pack_bf16(mine0 * inv, mine1 * inv);
+    typename E::T *op = out + ((size_t)b * N + n) * H * AT_D + h * AT_D;
+    *reinterpret_cast<uint32_t *>(op + 2 * lane) = E::pack(mine0 * inv, mine1 * inv);
     if (lane == 0) lse2[(size_t)bh * N + n] = M + log2f(l);
 }
 
@@ -294,18 +298,19 @@ struct AttnBwdSmem {
 // dV / dK epilogue: the thread's accumulator fragment (rows rq, rq + 8 of the warpgroup's keys) * mul -> bf16 -> the packed
 // gradient, and the column sums of the ROUNDED values of the warp's 16 rows -> qkv-bias gradient.  Rows beyond N hold zeros
 // (masked keys) and are not stored.
-__device__ __forceinline__ void bwd_epilogue_frag(const float (&acc)[32], float mul, __nv_bfloat16 *__restrict__ row0,
+template <typename E>
+__device__ __forceinline__ void bwd_epilogue_frag(const float (&acc)[32], float mul, typename E::T *__restrict__ row0,
                                                   size_t row_stride, bool ok0, bool ok1, float *__restrict__ g_bias_cols, int lane) {
     const int cq = 2 * (lane & 3);
 #pragma unroll
     for (int jj = 0; jj < AT_D / 8; ++jj) {
-        const uint32_t w0 = pack_bf16(acc[4 * jj] * mul, acc[4 * jj + 1] * mul);
-        const uint32_t w1 = pack_bf16(acc[4 * jj + 2] * mul, acc[4 * jj + 3] * mul);
+        const uint32_t w0 = E::pack(acc[4 * jj] * mul, acc[4 * jj + 1] * mul);
+        const uint32_t w1 = E::pack(acc[4 * jj + 2] * mul, acc[4 * jj + 3] * mul);
         if (ok0) *reinterpret_cast<uint32_t *>(row0 + 8 * jj + cq) = w0;
         if (ok1) *reinterpret_cast<uint32_t *>(row0 + 8 * row_stride + 8 * jj + cq) = w1;
         if (g_bias_cols) {
-            float s0 = __uint_as_float(w0 << 16) + __uint_as_float(w1 << 16);
-            float s1 = __uint_as_float(w0 & 0xffff0000u) + __uint_as_float(w1 & 0xffff0000u);
+            float s0 = E::lo(w0) + E::lo(w1);
+            float s1 = E::hi(w0) + E::hi(w1);
 #pragma unroll
             for (int o = 4; o < 32; o <<= 1) {
                 s0 += __shfl_xor_sync(0xffffffffu, s0, o);
@@ -319,9 +324,10 @@ __device__ __forceinline__ void bwd_epilogue_frag(const float (&acc)[32], float 
     }
 }
 
+template <typename E>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO, const float *__restrict__ lseP,
-                const float *__restrict__ deltaP, float *__restrict__ dq_acc, __nv_bfloat16 *__restrict__ dqkv, float *__restrict__ g_bias,
+                const float *__restrict__ deltaP, float *__restrict__ dq_acc, typename E::T *__restrict__ dqkv, float *__restrict__ g_bias,
                 int N, int H, int Npad, float c, float scale) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -392,9 +398,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
         float s[32], dp[32];
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64k16_ss<0, 0>(s, desc_adv(kd_k, k * 32), desc_adv(desc_k_sw128(qa), k * 32), (uint32_t)k);
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64k16_ss<E, 0, 0>(s, desc_adv(kd_k, k * 32), desc_adv(desc_k_sw128(qa), k * 32), (uint32_t)k);
 #pragma unroll
-        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64k16_ss<0, 0>(dp, desc_adv(vd_k, k * 32), desc_adv(desc_k_sw128(da), k * 32), (uint32_t)k);
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n64k16_ss<E, 0, 0>(dp, desc_adv(vd_k, k * 32), desc_adv(desc_k_sw128(da), k * 32), (uint32_t)k);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(s);
@@ -410,11 +416,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
                 const bool ok = hh ? kok1 : kok0;
                 const float p0 = ok ? ex2_approx(fmaf(s[4 * jj + 2 * hh], c, -Lq.x)) : 0.f;
                 const float p1 = ok ? ex2_approx(fmaf(s[4 * jj + 2 * hh + 1], c, -Lq.y)) : 0.f;
-                const uint32_t pw = pack_bf16(p0, p1);
-                // dS from the bf16-rounded P (the values the dV MMA consumes)
-                const float d0 = __uint_as_float(pw << 16) * (dp[4 * jj + 2 * hh] - Dq.x);
-                const float d1 = __uint_as_float(pw & 0xffff0000u) * (dp[4 * jj + 2 * hh + 1] - Dq.y);
-                const uint32_t dw = pack_bf16(d0, d1);
+                const uint32_t pw = E::pack(p0, p1);
+                // dS from the rounded P (the values the dV MMA consumes)
+                const float d0 = E::lo(pw) * (dp[4 * jj + 2 * hh] - Dq.x);
+                const float d1 = E::hi(pw) * (dp[4 * jj + 2 * hh + 1] - Dq.y);
+                const uint32_t dw = E::pack(d0, d1);
                 pa[jj >> 1][(jj & 1) * 2 + hh] = pw;
                 sa[jj >> 1][(jj & 1) * 2 + hh] = dw;
                 // dS^T row (key rq + 8 hh) -> smem, queries along the row: the MN-major A operand of dQ = dS K
@@ -428,11 +434,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < AB_BQ / 16; ++k) {
-            wgmma_m64n64k16_rs<1>(dv, pa[k], desc_adv(dd_mn, k * 2048), 1u);
-            wgmma_m64n64k16_rs<1>(dk, sa[k], desc_adv(qd_mn, k * 2048), 1u);
+            wgmma_m64n64k16_rs<E, 1>(dv, pa[k], desc_adv(dd_mn, k * 2048), 1u);
+            wgmma_m64n64k16_rs<E, 1>(dk, sa[k], desc_adv(qd_mn, k * 2048), 1u);
         }
 #pragma unroll
-        for (int k = 0; k < 64 / 16; ++k) wgmma_m64n64k16_ss<1, 1>(dq, desc_adv(dsd, k * 2048), desc_adv(kd_mn, k * 2048), (uint32_t)k);
+        for (int k = 0; k < 64 / 16; ++k) wgmma_m64n64k16_ss<E, 1, 1>(dq, desc_adv(dsd, k * 2048), desc_adv(kd_mn, k * 2048), (uint32_t)k);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(dv);
@@ -454,9 +460,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
         }
     }
     const size_t W = (size_t)3 * H * AT_D;
-    __nv_bfloat16 *row = dqkv + ((size_t)b * N + key0) * W;
-    bwd_epilogue_frag(dv, 1.0f, row + colV, W, kok0, kok1, g_bias ? g_bias + colV : nullptr, lane);
-    bwd_epilogue_frag(dk, scale, row + colK, W, kok0, kok1, g_bias ? g_bias + colK : nullptr, lane);
+    typename E::T *row = dqkv + ((size_t)b * N + key0) * W;
+    bwd_epilogue_frag<E>(dv, 1.0f, row + colV, W, kok0, kok1, g_bias ? g_bias + colV : nullptr, lane);
+    bwd_epilogue_frag<E>(dk, scale, row + colK, W, kok0, kok1, g_bias ? g_bias + colK : nullptr, lane);
 }
 
 
@@ -475,17 +481,18 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
 constexpr int AB_KTAIL_MAX = 4;
 constexpr int AB_PREP_ROWS = 128;
 
+template <typename E>
 __device__ __forceinline__ void unpack8(const uint4 &w, float (&f)[8]) {
     const uint32_t x[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
-    for (int e = 0; e < 4; ++e) { f[2 * e] = __uint_as_float(x[e] << 16); f[2 * e + 1] = __uint_as_float(x[e] & 0xffff0000u); }
+    for (int e = 0; e < 4; ++e) { f[2 * e] = E::lo(x[e]); f[2 * e + 1] = E::hi(x[e]); }
 }
 
-template <int NT>
+template <typename E, int NT>
 __global__ void __launch_bounds__(256, 2)
-attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 *__restrict__ out, const __nv_bfloat16 *__restrict__ dout,
+attn_bwd_prep_kernel(const typename E::T *__restrict__ qkv, const typename E::T *__restrict__ out, const typename E::T *__restrict__ dout,
                      const float *__restrict__ lse2, float *__restrict__ lseP, float *__restrict__ deltaP, float *__restrict__ dq_acc,
-                     float *__restrict__ dsT, __nv_bfloat16 *__restrict__ dqkv, float *__restrict__ g_bias, int N, int H, int Npad,
+                     float *__restrict__ dsT, typename E::T *__restrict__ dqkv, float *__restrict__ g_bias, int N, int H, int Npad,
                      float c, float scale) {
     constexpr int NTA = NT > 0 ? NT : 1;
     __shared__ float red[NT > 0 ? 8 : 1][2][NTA][AT_D];
@@ -494,7 +501,7 @@ attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 
     const int lane = threadIdx.x & 31, sub = threadIdx.x & 7, rloc = threadIdx.x >> 3;
     const int n0 = N - NT;
     const size_t W = (size_t)3 * H * AT_D;
-    const __nv_bfloat16 *qb = qkv + (size_t)b * N * W + h * AT_D + sub * 8;
+    const typename E::T *qb = qkv + (size_t)b * N * W + h * AT_D + sub * 8;
     const size_t ob = (size_t)b * N * H * AT_D + h * AT_D + sub * 8;
     float aK[NTA][8], aV[NTA][8];
     if constexpr (NT > 0) {
@@ -502,7 +509,7 @@ attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 
         if (threadIdx.x < NT * 16) {
             const int t = threadIdx.x >> 4, isv = (threadIdx.x >> 3) & 1;
             float f[8];
-            unpack8(*reinterpret_cast<const uint4 *>(qb + (size_t)(n0 + t) * W + (size_t)(1 + isv) * H * AT_D), f);
+            unpack8<E>(*reinterpret_cast<const uint4 *>(qb + (size_t)(n0 + t) * W + (size_t)(1 + isv) * H * AT_D), f);
 #pragma unroll
             for (int e = 0; e < 8; ++e) skv[isv][t][sub * 8 + e] = f[e];
         }
@@ -559,8 +566,8 @@ attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 
                 gw[ps] = src[PASSES * 256];
                 qw[ps] = src[2 * PASSES * 256];
             }
-            unpack8(ow[ps], ov);
-            unpack8(gw[ps], gv);
+            unpack8<E>(ow[ps], ov);
+            unpack8<E>(gw[ps], gv);
             float dl = 0.f;
 #pragma unroll
             for (int e = 0; e < 8; ++e) dl = fmaf(ov[e], gv[e], dl);
@@ -579,7 +586,7 @@ attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 
             }
             if constexpr (NT > 0) {
                 float qv[8];
-                unpack8(qw[ps], qv);
+                unpack8<E>(qw[ps], qv);
 #pragma unroll
                 for (int t = 0; t < NT; ++t) {
                     float sx = 0.f, pd = 0.f;
@@ -626,9 +633,9 @@ attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 
                 float sum = 0.f;
 #pragma unroll
                 for (int w8 = 0; w8 < 8; ++w8) sum += red[w8][which][t][d];
-                const __nv_bfloat16 val = __float2bfloat16(sum * (which == 0 ? scale : 1.0f));
+                const typename E::T val = E::from(sum * (which == 0 ? scale : 1.0f));
                 dqkv[((size_t)b * N + n0 + t) * W + (size_t)(1 + which) * H * AT_D + h * AT_D + d] = val;
-                bsum += __bfloat162float(val);
+                bsum += E::to(val);
             }
             if (g_bias) atomicAdd(g_bias + (size_t)(1 + which) * H * AT_D + h * AT_D + d, bsum);
         }
@@ -640,9 +647,10 @@ attn_bwd_prep_kernel(const __nv_bfloat16 *__restrict__ qkv, const __nv_bfloat16 
 // column groups, four row passes with the loads issued up front: a block never mixes heads.
 constexpr int AB_CONV_ROWS = 128;
 
+template <typename E>
 __global__ void __launch_bounds__(256)
-attn_dq_convert_kernel(const float *__restrict__ dq_acc, const __nv_bfloat16 *__restrict__ qkv, const float *__restrict__ dsT,
-                       __nv_bfloat16 *__restrict__ dqkv, float *__restrict__ g_bias, int N, int H, int n0, int nt, float scale) {
+attn_dq_convert_kernel(const float *__restrict__ dq_acc, const typename E::T *__restrict__ qkv, const float *__restrict__ dsT,
+                       typename E::T *__restrict__ dqkv, float *__restrict__ g_bias, int N, int H, int n0, int nt, float scale) {
     __shared__ float red[8][AT_D];
     __shared__ float skt[AB_KTAIL_MAX][AT_D];
     const int part = threadIdx.x & 7, rloc = threadIdx.x >> 3;
@@ -660,7 +668,7 @@ attn_dq_convert_kernel(const float *__restrict__ dq_acc, const __nv_bfloat16 *__
     if (nt > 0) {
         for (int i = threadIdx.x; i < nt * AT_D; i += 256) {
             const int t = i / AT_D, d = i - t * AT_D;
-            skt[t][d] = __bfloat162float(qkv[(((size_t)bb * N + n0 + t) * 3 * H + H + hh) * AT_D + d]);
+            skt[t][d] = E::to(qkv[(((size_t)bb * N + n0 + t) * 3 * H + H + hh) * AT_D + d]);
         }
         __syncthreads();
     }
@@ -679,14 +687,14 @@ attn_dq_convert_kernel(const float *__restrict__ dq_acc, const __nv_bfloat16 *__
                 for (int e = 0; e < 8; ++e) x[e] = fmaf(ds, skt[t][part * 8 + e], x[e]);
             }
             uint4 o;
-            o.x = pack_bf16(x[0] * scale, x[1] * scale);
-            o.y = pack_bf16(x[2] * scale, x[3] * scale);
-            o.z = pack_bf16(x[4] * scale, x[5] * scale);
-            o.w = pack_bf16(x[6] * scale, x[7] * scale);
+            o.x = E::pack(x[0] * scale, x[1] * scale);
+            o.y = E::pack(x[2] * scale, x[3] * scale);
+            o.z = E::pack(x[4] * scale, x[5] * scale);
+            o.w = E::pack(x[6] * scale, x[7] * scale);
             *reinterpret_cast<uint4 *>(dqkv + (((size_t)bb * N + n) * 3 * H + hh) * AT_D + part * 8) = o;
             const uint32_t w[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
-            for (int e = 0; e < 4; ++e) { v[2 * e] += __uint_as_float(w[e] << 16); v[2 * e + 1] += __uint_as_float(w[e] & 0xffff0000u); }
+            for (int e = 0; e < 4; ++e) { v[2 * e] += E::lo(w[e]); v[2 * e + 1] += E::hi(w[e]); }
         }
     }
     if (!g_bias) return;
@@ -727,18 +735,10 @@ static size_t attn_bwd_ws_layout(int B, int N, int H, size_t *off_lse, size_t *o
     return acc + 2 * st + dst;
 }
 
-}  // namespace xq
-
-extern "C" {
-
-size_t xq_vit_attn_bwd_workspace_bytes(int B, int N, int H) {
-    if (B <= 0 || N <= 0 || H <= 0) return 0;
-    return xq::attn_bwd_ws_layout(B, N, H, nullptr, nullptr, nullptr);
-}
-
-int xq_vit_attn_bwd(const void *qkv, const void *out, const void *d_out, const float *lse2, void *dqkv, float *g_bias, int B, int N,
+template <typename E>
+static int attn_bwd(const void *qkv, const void *out, const void *d_out, const float *lse2, void *dqkv, float *g_bias, int B, int N,
                     int H, int head_dim, float scale, void *workspace, size_t workspace_bytes, void *stream) {
-    using namespace xq;
+    using T = typename E::T;
     if (!qkv || !out || !d_out || !lse2 || !dqkv || !workspace || B <= 0 || N <= 0 || H <= 0) return XQ_ERR_ARG;
     if (head_dim != AT_D) return XQ_ERR_UNSUPPORTED;
     if (((uintptr_t)qkv & 15) || ((uintptr_t)out & 15) || ((uintptr_t)d_out & 15) || ((uintptr_t)dqkv & 15) || ((uintptr_t)workspace & 255))
@@ -752,8 +752,8 @@ int xq_vit_attn_bwd(const void *qkv, const void *out, const void *d_out, const f
     float *dsT = (float *)((char *)workspace + off_dst);
     const uint64_t W = (uint64_t)3 * H * AT_D, Wo = (uint64_t)H * AT_D;
     CUtensorMap tmQKV, tmDO;
-    if (!tensor_map_bf16_3d(&tmQKV, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AB_BQ) ||
-        !tensor_map_bf16_3d(&tmDO, d_out, Wo, N, B, Wo * 2, (uint64_t)N * Wo * 2, AB_BQ))
+    if (!tensor_map_16_3d(&tmQKV, E::TMAP, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AB_BQ) ||
+        !tensor_map_16_3d(&tmDO, E::TMAP, d_out, Wo, N, B, Wo * 2, (uint64_t)N * Wo * 2, AB_BQ))
         return XQ_ERR_UNSUPPORTED;
     const int nt = attn_bwd_ktail(N);                                     // few trailing keys: CUDA-core kernel, not a key block
     const int nK = nt ? N / AT_BN : (N + AT_BN - 1) / AT_BN;
@@ -765,52 +765,79 @@ int xq_vit_attn_bwd(const void *qkv, const void *out, const void *d_out, const f
         dim3 grid(nt ? 1u : (unsigned)(Npad / AB_PREP_ROWS), (unsigned)(B * H));
         // the NT > 0 variants' two-stage row buffer
         const size_t ps = nt ? (size_t)2 * 3 * (AB_PREP_ROWS / 32) * 256 * 16 : 0;
-        decltype(&attn_bwd_prep_kernel<0>) const preps[] = {attn_bwd_prep_kernel<0>, attn_bwd_prep_kernel<1>, attn_bwd_prep_kernel<2>,
-                                                            attn_bwd_prep_kernel<3>, attn_bwd_prep_kernel<4>};
+        decltype(&attn_bwd_prep_kernel<E, 0>) const preps[] = {attn_bwd_prep_kernel<E, 0>, attn_bwd_prep_kernel<E, 1>,
+                                                               attn_bwd_prep_kernel<E, 2>, attn_bwd_prep_kernel<E, 3>,
+                                                               attn_bwd_prep_kernel<E, 4>};
         const auto prep = preps[nt < 4 ? nt : 4];
         if (int rc = smem_optin(prep, ps)) return rc;
-        prep<<<grid, 256, ps, st>>>((const __nv_bfloat16 *)qkv, (const __nv_bfloat16 *)out, (const __nv_bfloat16 *)d_out, lse2, lseP,
-                                    deltaP, acc, dsT, (__nv_bfloat16 *)dqkv, g_bias, N, H, Npad, c2, scale);
+        prep<<<grid, 256, ps, st>>>((const T *)qkv, (const T *)out, (const T *)d_out, lse2, lseP, deltaP, acc, dsT, (T *)dqkv, g_bias,
+                                    N, H, Npad, c2, scale);
         XQ_LAUNCH_CHECK("attn_bwd_prep_kernel");
     }
     const size_t smem = AttnBwdSmem::BYTES + 1024;
-    if (int rc = smem_optin(attn_bwd_kernel, smem)) return rc;
-    attn_bwd_kernel<<<dim3((unsigned)nK, (unsigned)(B * H)), AB_THREADS, smem, st>>>(tmQKV, tmDO, lseP, deltaP, acc,
-                                                                                     (__nv_bfloat16 *)dqkv, g_bias, N, H, Npad, c2, scale);
+    if (int rc = smem_optin(attn_bwd_kernel<E>, smem)) return rc;
+    attn_bwd_kernel<E><<<dim3((unsigned)nK, (unsigned)(B * H)), AB_THREADS, smem, st>>>(tmQKV, tmDO, lseP, deltaP, acc, (T *)dqkv,
+                                                                                        g_bias, N, H, Npad, c2, scale);
     XQ_LAUNCH_CHECK("attn_bwd_kernel");
     {
         dim3 grid((unsigned)((N + AB_CONV_ROWS - 1) / AB_CONV_ROWS), (unsigned)(B * H));
-        attn_dq_convert_kernel<<<grid, 256, 0, st>>>(acc, (const __nv_bfloat16 *)qkv, dsT, (__nv_bfloat16 *)dqkv, g_bias, N, H, N - nt, nt, scale);
+        attn_dq_convert_kernel<E><<<grid, 256, 0, st>>>(acc, (const T *)qkv, dsT, (T *)dqkv, g_bias, N, H, N - nt, nt, scale);
         XQ_LAUNCH_CHECK("attn_dq_convert_kernel");
     }
     return XQ_OK;
 }
 
-int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream) {
-    using namespace xq;
+template <typename E>
+static int attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream) {
+    using T = typename E::T;
     if (!qkv || !out || !lse2 || B <= 0 || N <= 0 || H <= 0) return XQ_ERR_ARG;
     if (head_dim != AT_D) return XQ_ERR_UNSUPPORTED;
     if (((uintptr_t)qkv & 15) || ((uintptr_t)out & 15)) return XQ_ERR_ARG;
     const uint64_t W = (uint64_t)3 * H * AT_D;
     CUtensorMap tmQKV;
-    if (!tensor_map_bf16_3d(&tmQKV, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AT_BM)) return XQ_ERR_UNSUPPORTED;
+    if (!tensor_map_16_3d(&tmQKV, E::TMAP, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AT_BM)) return XQ_ERR_UNSUPPORTED;
     // query tiles: full 128-row tiles on the tensor cores; a short remainder (<= AT_TAIL_MAX rows) on the CUDA cores
     const int n_tail = (N % AT_BM != 0 && N % AT_BM <= AT_TAIL_MAX && N > AT_BM) ? N % AT_BM : 0;
     const int nQ = n_tail ? N / AT_BM : (N + AT_BM - 1) / AT_BM;
     const size_t smem = AttnFwdSmem::BYTES + 1024;
-    if (int rc = smem_optin(attn_fwd_kernel, smem)) return rc;
+    if (int rc = smem_optin(attn_fwd_kernel<E>, smem)) return rc;
     const long long tiles = (long long)B * H * nQ;
     if (tiles > 0x7fffffffLL) return XQ_ERR_ARG;
     const float c = scale * 1.4426950408889634f;
-    attn_fwd_kernel<<<(unsigned)tiles, AT_THREADS, smem, (cudaStream_t)stream>>>(tmQKV, (__nv_bfloat16 *)out, lse2, N, H, nQ, c);
+    attn_fwd_kernel<E><<<(unsigned)tiles, AT_THREADS, smem, (cudaStream_t)stream>>>(tmQKV, (T *)out, lse2, N, H, nQ, c);
     XQ_LAUNCH_CHECK("attn_fwd_kernel");
     if (n_tail) {
         const long long warps = (long long)B * H * n_tail;
-        attn_fwd_tail_kernel<<<(unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream>>>(
-            (const __nv_bfloat16 *)qkv, (__nv_bfloat16 *)out, lse2, B, N, H, N - n_tail, c);
+        attn_fwd_tail_kernel<E><<<(unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream>>>((const T *)qkv, (T *)out, lse2, B,
+                                                                                                 N, H, N - n_tail, c);
         XQ_LAUNCH_CHECK("attn_fwd_tail_kernel");
     }
     return XQ_OK;
+}
+
+}  // namespace xq
+
+extern "C" {
+
+size_t xq_vit_attn_bwd_workspace_bytes(int B, int N, int H) {
+    if (B <= 0 || N <= 0 || H <= 0) return 0;
+    return xq::attn_bwd_ws_layout(B, N, H, nullptr, nullptr, nullptr);
+}
+
+int xq_vit_attn_bwd(const void *qkv, const void *out, const void *d_out, const float *lse2, void *dqkv, float *g_bias, int B, int N,
+                    int H, int head_dim, float scale, void *workspace, size_t workspace_bytes, void *stream) {
+    return xq::attn_bwd<xqtc::Bf16>(qkv, out, d_out, lse2, dqkv, g_bias, B, N, H, head_dim, scale, workspace, workspace_bytes, stream);
+}
+int xq_vit_attn_bwd_f16(const void *qkv, const void *out, const void *d_out, const float *lse2, void *dqkv, float *g_bias, int B,
+                        int N, int H, int head_dim, float scale, void *workspace, size_t workspace_bytes, void *stream) {
+    return xq::attn_bwd<xqtc::F16>(qkv, out, d_out, lse2, dqkv, g_bias, B, N, H, head_dim, scale, workspace, workspace_bytes, stream);
+}
+
+int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream) {
+    return xq::attn_fwd<xqtc::Bf16>(qkv, out, lse2, B, N, H, head_dim, scale, stream);
+}
+int xq_vit_attn_fwd_f16(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream) {
+    return xq::attn_fwd<xqtc::F16>(qkv, out, lse2, B, N, H, head_dim, scale, stream);
 }
 
 }  // extern "C"

@@ -4,7 +4,7 @@
 // Path: timm `Mlp.forward` inside `Block.forward`, tokenizer/tokenizer_image/dino_enc/vision_transformer.py:336-339
 //   h = GELU(fc1(y)) ; branch = fc2(h)        and its backward.
 // Two entry points replace a cuBLAS GEMM + a stand-alone bias/GELU kernel each:
-//   xq_vit_fc1_gelu_fwd   pre = y W1^T (bf16) ; act = GELU(pre + b1)                       [epilogue writes both]
+//   xq_vit_fc1_gelu_fwd   pre = y W1^T (16-bit) ; act = GELU(pre + b1)                       [epilogue writes both]
 //   xq_vit_fc2_dgelu_bwd  d_pre = (d_branch W2) * GELU'(pre + b1) ; d_b1 = colsum(d_pre)    [epilogue reads pre]
 // (the other four GEMMs of the block -- fc2 forward, the two weight gradients, the fc1 input gradient -- stay plain cuBLAS calls).
 // Their LoRA forms (fc1 / fc2 wrapped by dino_enc/lora.py, u = s y A1^T and v = s d_branch B2 rank-R activations, R <= 64):
@@ -13,8 +13,10 @@
 // are the same kernel with one more K stage: the producer loads the [128][64] tiles of u / v and of the K-major adapter
 // (B1 [N,R], A2^T [N,R]) after the main K loop, TMA zero-filling the columns >= R, and the MMA warps accumulate it into the
 // same fp32 accumulators before the single rounding to bf16.
+// Every entry point has an `_f16` twin: the same kernel instantiated for fp16 operands and outputs (fp16 autocast), wgmma
+// .f16 instead of .bf16, f16 tensor maps and conversions; shared memory, registers and schedule are the same.
 //
-// C[M,N] = A[M,K] . B[N,K]^T, A and B K-major (row-major as PyTorch stores activations and Linear weights), bf16 in, fp32
+// C[M,N] = A[M,K] . B[N,K]^T, A and B K-major (row-major as PyTorch stores activations and Linear weights), bf16 / f16 in, fp32
 // accumulation in registers.  A CTA owns a 128 x 128 tile and is persistent: CTA p keeps column block p % (N/128) for the whole
 // kernel (bias slice and bias-gradient sums in registers, the weight tile hot in L2) and walks the 128-row blocks.  Roles
 // (416 threads):
@@ -88,13 +90,13 @@ struct GmClock {
 // EPI 1: forward  -- the staged tile is the pre-activation: TMA-stored as it stands (tmP); GELU(pre + bias) -> tmO.
 // EPI 2: backward -- the staged tile is d_act; the producer loads the stored pre-activation tile (tmP);
 //                    d_act * GELU'(pre + bias) -> tmO; column sums of the ROUNDED result -> dbias (fp32 atomics at the end).
-// Both apply the element-wise function to the ROUNDED bf16 value of the GEMM result, i.e. exactly what the stand-alone
+// Both apply the element-wise function to the ROUNDED 16-bit value of the GEMM result, i.e. exactly what the stand-alone
 // kernels compute from the tensor a library GEMM would have written.
 //
 // R > 0: the rank-R tail stage (tmU: [M,R] activation, tmL: [N,R] adapter) follows the nk stages of the main K loop.
 // Barriers: full / empty per ring stage; stg_full (the 8 MMA warps have written the staging tile) / stg_empty (the epilogue
 // is done with it); aux_full / aux_empty per auxiliary tile (backward: the `pre` tile has landed / its store has been read).
-template <int EPI>
+template <typename E, int EPI>
 __global__ void __launch_bounds__(GM_THREADS, 1)
 mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmO,
@@ -215,22 +217,22 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     if (EPI == 1) {
 #pragma unroll
                         for (int w = 0; w < 4; ++w) {
-                            const float g0 = __uint_as_float(g[w] << 16), g1 = __uint_as_float(g[w] & 0xffff0000u);
-                            o[w] = pack_bf16(gelu_f(g0 + b[2 * w]), gelu_f(g1 + b[2 * w + 1]));
+                            const float g0 = E::lo(g[w]), g1 = E::hi(g[w]);
+                            o[w] = E::pack(gelu_f(g0 + b[2 * w]), gelu_f(g1 + b[2 * w + 1]));
                         }
                     } else {
-                        // d_act rounded to bf16 first: the stand-alone kernel reads the bf16 tensor a library GEMM wrote.
+                        // d_act rounded to 16 bits first: the stand-alone kernel reads the tensor a library GEMM wrote.
                         // Rows >= M: the zero-filled A rows give d_act = 0, so they add nothing to the bias gradient.
                         const uint32_t x[4] = {xq4[u].x, xq4[u].y, xq4[u].z, xq4[u].w};
                         float v[8];
 #pragma unroll
                         for (int w = 0; w < 4; ++w) {
-                            const float g0 = __uint_as_float(g[w] << 16), g1 = __uint_as_float(g[w] & 0xffff0000u);
-                            const float d0 = dgelu_f(__uint_as_float(x[w] << 16) + b[2 * w]);
-                            const float d1 = dgelu_f(__uint_as_float(x[w] & 0xffff0000u) + b[2 * w + 1]);
-                            o[w] = pack_bf16(g0 * d0, g1 * d1);
-                            v[2 * w] = __uint_as_float(o[w] << 16);
-                            v[2 * w + 1] = __uint_as_float(o[w] & 0xffff0000u);
+                            const float g0 = E::lo(g[w]), g1 = E::hi(g[w]);
+                            const float d0 = dgelu_f(E::lo(x[w]) + b[2 * w]);
+                            const float d1 = dgelu_f(E::hi(x[w]) + b[2 * w + 1]);
+                            o[w] = E::pack(g0 * d0, g1 * d1);
+                            v[2 * w] = E::lo(o[w]);
+                            v[2 * w + 1] = E::hi(o[w]);
                         }
 #pragma unroll
                         for (int l = 0; l <= 4; ++l) {
@@ -267,8 +269,17 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
         if (te == 0) { bulk_wait<0>(); clk.flush(EPI); }
         if (EPI == 2) {
+            int col = nb * GM_BN + 8 * uc;
+            if constexpr (E::IS_F16) {
+                // the column re-derived from the special registers: kept live across the tile loop, its address spills in
+                // the f16 instantiation (one more live register in the sum tree than the bf16 one)
+                uint32_t t, c;
+                asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+                asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(c));
+                col = (int)(c % (uint32_t)nN) * GM_BN + 8 * (int)(t & 15);
+            }
 #pragma unroll
-            for (int e = 0; e < 8; ++e) atomicAdd(dbias + nb * GM_BN + 8 * uc + e, bsum[e]);
+            for (int e = 0; e < 8; ++e) atomicAdd(dbias + col + e, bsum[e]);
         }
         return;
     }
@@ -291,7 +302,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const uint64_t bd = desc_k_sw128(smem_u32(base + st * GM_ST_BYTES + GM_A_BYTES));
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < GM_BK / 16; ++k) wgmma_m64n128k16_ss<0, 0>(acc, desc_adv(ad, k * 32), desc_adv(bd, k * 32), 1u);
+            for (int k = 0; k < GM_BK / 16; ++k) wgmma_m64n128k16_ss<E, 0, 0>(acc, desc_adv(ad, k * 32), desc_adv(bd, k * 32), 1u);
             wgmma_commit();
             wgmma_wait<1>();                                     // the previous stage's MMAs have retired: release it
             fence_regs(acc);
@@ -308,8 +319,8 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         for (int jj = 0; jj < GM_BN / 16; ++jj) {
             const int cg = 2 * jj + (lane >> 4);                 // 8-column group: unit cg % 8 of row tile cg / 8
             stmatrix_x4(smem_u32(stg) + (cg >> 3) * GM_HALF_BYTES + rowtile_unit(srow, cg & 7),
-                        pack_bf16(acc[8 * jj], acc[8 * jj + 1]), pack_bf16(acc[8 * jj + 2], acc[8 * jj + 3]),
-                        pack_bf16(acc[8 * jj + 4], acc[8 * jj + 5]), pack_bf16(acc[8 * jj + 6], acc[8 * jj + 7]));
+                        E::pack(acc[8 * jj], acc[8 * jj + 1]), E::pack(acc[8 * jj + 2], acc[8 * jj + 3]),
+                        E::pack(acc[8 * jj + 4], acc[8 * jj + 5]), E::pack(acc[8 * jj + 6], acc[8 * jj + 7]));
         }
         fence_async_smem();                                      // forward: a TMA store reads the staging tile
         __syncwarp();
@@ -335,7 +346,7 @@ static int gm_check_lora(const void *u, const void *l, int R) {
 }
 
 // `pre` is the pre-activation tensor (written by the forward, read by the backward), `out` the epilogue's result (act / d_pre)
-template <int EPI>
+template <typename E, int EPI>
 // R > 0 adds the rank-R stage u [M,R] . l [N,R]^T; R == 0 ignores u / l
 static int gm_launch(const void *a, const void *b, const void *u, const void *l, const void *pre, void *out, const float *bias,
                      float *dbias, int M, int N, int K, int R, cudaStream_t st) {
@@ -344,24 +355,59 @@ static int gm_launch(const void *a, const void *b, const void *u, const void *l,
     const int nN = N / GM_BN;
     if (nN > sms) return XQ_ERR_UNSUPPORTED;
     CUtensorMap tmA, tmB, tmP, tmO;
-    if (!tensor_map_bf16_3d(&tmA, a, K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BM) ||
-        !tensor_map_bf16_3d(&tmB, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BN) ||
-        !tensor_map_bf16_3d(&tmP, pre, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM) ||
-        !tensor_map_bf16_3d(&tmO, out, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM))
+    if (!tensor_map_16_3d(&tmA, E::TMAP, a, K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BM) ||
+        !tensor_map_16_3d(&tmB, E::TMAP, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BN) ||
+        !tensor_map_16_3d(&tmP, E::TMAP, pre, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM) ||
+        !tensor_map_16_3d(&tmO, E::TMAP, out, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM))
         return XQ_ERR_UNSUPPORTED;
     CUtensorMap tmU = tmA, tmL = tmB;
-    if (R > 0 && (!tensor_map_bf16_3d(&tmU, u, R, M, 1, (uint64_t)R * 2, (uint64_t)M * R * 2, GM_BM) ||
-                  !tensor_map_bf16_3d(&tmL, l, R, N, 1, (uint64_t)R * 2, (uint64_t)N * R * 2, GM_BN)))
+    if (R > 0 && (!tensor_map_16_3d(&tmU, E::TMAP, u, R, M, 1, (uint64_t)R * 2, (uint64_t)M * R * 2, GM_BM) ||
+                  !tensor_map_16_3d(&tmL, E::TMAP, l, R, N, 1, (uint64_t)R * 2, (uint64_t)N * R * 2, GM_BN)))
         return XQ_ERR_UNSUPPORTED;
-    if (int rc = smem_optin(mlp_gemm_kernel<EPI>, GM_SMEM)) return rc;
+    if (int rc = smem_optin(mlp_gemm_kernel<E, EPI>, GM_SMEM)) return rc;
     const int nM = (M + GM_BM - 1) / GM_BM;
     int per_col = sms / nN;                               // CTAs per column block
     if (per_col > nM) per_col = nM;
     // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
     if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st));
-    mlp_gemm_kernel<EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, tmU, tmL, bias, dbias, M, N, K, R);
+    mlp_gemm_kernel<E, EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, tmU, tmL, bias, dbias, M, N, K, R);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
     return XQ_OK;
+}
+
+}  // namespace xq
+
+namespace xq {
+
+template <typename E>
+static int fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream) {
+    if (int rc = gm_check(x, w, pre, act, bias, M, N, K)) return rc;
+    return gm_launch<E, 1>(x, w, nullptr, nullptr, pre, act, bias, nullptr, M, N, K, 0, (cudaStream_t)stream);
+}
+
+template <typename E>
+static int fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias, int M,
+                         int N, int K, void *stream) {
+    if (int rc = gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
+    if (!d_bias) return XQ_ERR_ARG;
+    return gm_launch<E, 2>(d_out, w2t, nullptr, nullptr, pre, d_pre, bias, d_bias, M, N, K, 0, (cudaStream_t)stream);
+}
+
+template <typename E>
+static int fc1_lora_gelu_fwd(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre, void *act,
+                             int M, int N, int K, int R, void *stream) {
+    if (int rc = gm_check(x, w, pre, act, bias, M, N, K)) return rc;
+    if (int rc = gm_check_lora(u, b_lora, R)) return rc;
+    return gm_launch<E, 1>(x, w, u, b_lora, pre, act, bias, nullptr, M, N, K, R, (cudaStream_t)stream);
+}
+
+template <typename E>
+static int fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre, const float *bias,
+                              void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream) {
+    if (int rc = gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
+    if (int rc = gm_check_lora(v, a2t, R)) return rc;
+    if (!d_bias) return XQ_ERR_ARG;
+    return gm_launch<E, 2>(d_out, w2t, v, a2t, pre, d_pre, bias, d_bias, M, N, K, R, (cudaStream_t)stream);
 }
 
 }  // namespace xq
@@ -369,30 +415,37 @@ static int gm_launch(const void *a, const void *b, const void *u, const void *l,
 extern "C" {
 
 int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream) {
-    if (int rc = xq::gm_check(x, w, pre, act, bias, M, N, K)) return rc;
-    return xq::gm_launch<1>(x, w, nullptr, nullptr, pre, act, bias, nullptr, M, N, K, 0, (cudaStream_t)stream);
+    return xq::fc1_gelu_fwd<xqtc::Bf16>(x, w, bias, pre, act, M, N, K, stream);
+}
+int xq_vit_fc1_gelu_fwd_f16(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream) {
+    return xq::fc1_gelu_fwd<xqtc::F16>(x, w, bias, pre, act, M, N, K, stream);
 }
 
 int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias, int M,
                          int N, int K, void *stream) {
-    if (int rc = xq::gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
-    if (!d_bias) return XQ_ERR_ARG;
-    return xq::gm_launch<2>(d_out, w2t, nullptr, nullptr, pre, d_pre, bias, d_bias, M, N, K, 0, (cudaStream_t)stream);
+    return xq::fc2_dgelu_bwd<xqtc::Bf16>(d_out, w2t, pre, bias, d_pre, d_bias, M, N, K, stream);
+}
+int xq_vit_fc2_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
+                             int M, int N, int K, void *stream) {
+    return xq::fc2_dgelu_bwd<xqtc::F16>(d_out, w2t, pre, bias, d_pre, d_bias, M, N, K, stream);
 }
 
 int xq_vit_fc1_lora_gelu_fwd(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre, void *act,
                              int M, int N, int K, int R, void *stream) {
-    if (int rc = xq::gm_check(x, w, pre, act, bias, M, N, K)) return rc;
-    if (int rc = xq::gm_check_lora(u, b_lora, R)) return rc;
-    return xq::gm_launch<1>(x, w, u, b_lora, pre, act, bias, nullptr, M, N, K, R, (cudaStream_t)stream);
+    return xq::fc1_lora_gelu_fwd<xqtc::Bf16>(x, w, u, b_lora, bias, pre, act, M, N, K, R, stream);
+}
+int xq_vit_fc1_lora_gelu_fwd_f16(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre,
+                                 void *act, int M, int N, int K, int R, void *stream) {
+    return xq::fc1_lora_gelu_fwd<xqtc::F16>(x, w, u, b_lora, bias, pre, act, M, N, K, R, stream);
 }
 
 int xq_vit_fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre, const float *bias,
                               void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream) {
-    if (int rc = xq::gm_check(d_out, w2t, d_pre, pre, bias, M, N, K)) return rc;
-    if (int rc = xq::gm_check_lora(v, a2t, R)) return rc;
-    if (!d_bias) return XQ_ERR_ARG;
-    return xq::gm_launch<2>(d_out, w2t, v, a2t, pre, d_pre, bias, d_bias, M, N, K, R, (cudaStream_t)stream);
+    return xq::fc2_lora_dgelu_bwd<xqtc::Bf16>(d_out, w2t, v, a2t, pre, bias, d_pre, d_bias, M, N, K, R, stream);
+}
+int xq_vit_fc2_lora_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre,
+                                  const float *bias, void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream) {
+    return xq::fc2_lora_dgelu_bwd<xqtc::F16>(d_out, w2t, v, a2t, pre, bias, d_pre, d_bias, M, N, K, R, stream);
 }
 
 #ifdef XQ_GM_CLOCKS

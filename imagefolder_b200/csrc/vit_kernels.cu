@@ -2,7 +2,7 @@
 //
 // The reference block (dino_enc/vision_transformer.py:336-339) is
 //     x = x + drop_path(ls1(attn(norm1(x))));   x = x + drop_path(ls2(mlp(norm2(x))))
-// with the residual stream in fp32 and GEMM operands in bf16 under autocast.  Eager PyTorch spends
+// with the residual stream in fp32 and GEMM operands in bf16 (or fp16) under autocast.  Eager PyTorch spends
 // one kernel per arrow (LayerNorm, cast, LayerScale mul, DropPath mul, add, GELU ...), each a full
 // HBM round trip.  Here the whole non-GEMM glue between two GEMMs is ONE pass:
 //
@@ -14,10 +14,14 @@
 //
 // Algorithmic bytes per element (row x channel): fwd 4 (x) + 2 (branch) + 4 (x_new) + 2 (y) = 12 B;
 // bwd 4 (g_xnew) + 2 (g_y) + 4 (x_new) + 2 (branch) + 4 (G) + 2 (g_branch) = 18 B.
+// Every kernel with a 16-bit operand is a template over its element type (xq_tc.cuh: Bf16 / F16); the `_f16` entry points
+// are the f16 instantiations, for fp16 autocast.
 // These TUs do not carry index decisions, so they are built with the default -fmad=true.
 #include "xq_common.cuh"
 #include "xq_gelu.cuh"
 #include "xq_tc.cuh"
+
+#include <type_traits>
 
 namespace xqv {
 
@@ -27,30 +31,34 @@ using xq::warp_sum;
 constexpr int WARPS = 8;
 constexpr int THREADS = WARPS * 32;
 
-struct bf16x4 { __nv_bfloat162 a, b; };
+// E: the 16-bit element type of the GEMM operands (xq_tc.cuh: Bf16 / F16)
+template <typename E>
+struct x4 { typename E::T2 a, b; };
 
-__device__ __forceinline__ float4 load_bf16x4(const __nv_bfloat16 *p) {
-    bf16x4 v = *reinterpret_cast<const bf16x4 *>(p);
-    float2 lo = __bfloat1622float2(v.a), hi = __bfloat1622float2(v.b);
+template <typename E>
+__device__ __forceinline__ float4 load16x4(const typename E::T *p) {
+    x4<E> v = *reinterpret_cast<const x4<E> *>(p);
+    float2 lo = E::to2(v.a), hi = E::to2(v.b);
     return make_float4(lo.x, lo.y, hi.x, hi.y);
 }
-__device__ __forceinline__ void store_bf16x4(__nv_bfloat16 *p, float4 f) {
-    bf16x4 v;
-    v.a = __floats2bfloat162_rn(f.x, f.y);
-    v.b = __floats2bfloat162_rn(f.z, f.w);
-    *reinterpret_cast<bf16x4 *>(p) = v;
+template <typename E>
+__device__ __forceinline__ void store16x4(typename E::T *p, float4 f) {
+    x4<E> v;
+    v.a = E::from2(f.x, f.y);
+    v.b = E::from2(f.z, f.w);
+    *reinterpret_cast<x4<E> *>(p) = v;
 }
 
 // One warp handles FR = 2 rows (loads of both issued before any arithmetic); NV = D / 128 float4 chunks per lane.
 //   x_new = x + rowscale * gamma_ls * (branch + branch_bias)
 constexpr int FR = 2;
-template <int NV>
+template <typename E, int NV>
 __global__ void __launch_bounds__(THREADS)
-residual_ln_fwd_kernel(const float *__restrict__ x, const __nv_bfloat16 *__restrict__ branch,
+residual_ln_fwd_kernel(const float *__restrict__ x, const typename E::T *__restrict__ branch,
                        const float *__restrict__ branch_bias, const float *__restrict__ ls_gamma,
                        const float *__restrict__ rowscale, int rows_per_sample, const float *__restrict__ ln_w,
                        const float *__restrict__ ln_b, float eps, int M, float *__restrict__ x_out,
-                       __nv_bfloat16 *__restrict__ y, float *__restrict__ mean_out, float *__restrict__ rstd_out) {
+                       typename E::T *__restrict__ y, float *__restrict__ mean_out, float *__restrict__ rstd_out) {
     constexpr int D = NV * 128;
     const int lane = threadIdx.x & 31;
     const int rbase = (blockIdx.x * WARPS + (threadIdx.x >> 5)) * FR;
@@ -65,7 +73,7 @@ residual_ln_fwd_kernel(const float *__restrict__ x, const __nv_bfloat16 *__restr
         for (int i = 0; i < NV; ++i) {
             const int col = (i * 32 + lane) * 4;
             v[u][i] = *reinterpret_cast<const float4 *>(x + base + col);
-            bv[u][i] = branch ? load_bf16x4(branch + base + col) : make_float4(0.f, 0.f, 0.f, 0.f);
+            bv[u][i] = branch ? load16x4<E>(branch + base + col) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     }
 #pragma unroll
@@ -108,7 +116,7 @@ residual_ln_fwd_kernel(const float *__restrict__ x, const __nv_bfloat16 *__restr
                 float4 o;
                 o.x = (v[u][i].x - mean) * rstd * w.x + b.x; o.y = (v[u][i].y - mean) * rstd * w.y + b.y;
                 o.z = (v[u][i].z - mean) * rstd * w.z + b.z; o.w = (v[u][i].w - mean) * rstd * w.w + b.w;
-                store_bf16x4(y + base + col, o);
+                store16x4<E>(y + base + col, o);
             }
         }
         if (lane == 0 && mean_out) { mean_out[row] = mean; rstd_out[row] = rstd; }
@@ -132,14 +140,14 @@ constexpr int LNB_THREADS = (LNB_TR + 1) * 32;
 __host__ __device__ inline size_t lnb_stage_bytes(int D) { return (size_t)LNB_TR * D * 12 + 128; }
 __host__ __device__ inline int lnb_stages(int D) { return lnb_stage_bytes(D) * 3 <= 225 * 1024 ? 3 : 2; }
 
-template <int NV>
+template <typename E, int NV>
 __global__ void __launch_bounds__(LNB_THREADS, 1)
-residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__restrict__ g_y,
+residual_ln_bwd_kernel(const float *__restrict__ g_xout, const typename E::T *__restrict__ g_y,
                        const float *__restrict__ x_out, const float *__restrict__ mean_in,
                        const float *__restrict__ rstd_in, const float *__restrict__ ln_w,
-                       const __nv_bfloat16 *__restrict__ branch, const float *__restrict__ branch_bias,
+                       const typename E::T *__restrict__ branch, const float *__restrict__ branch_bias,
                        const float *__restrict__ ls_gamma, const float *__restrict__ rowscale, int rows_per_sample,
-                       int M, float *__restrict__ g_x, __nv_bfloat16 *__restrict__ g_branch,
+                       int M, float *__restrict__ g_x, typename E::T *__restrict__ g_branch,
                        float *__restrict__ part, int *__restrict__ counter, int nst) {
     constexpr int D = NV * 128;
     constexpr int TR = LNB_TR;
@@ -151,8 +159,8 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
     const size_t stage_bytes = lnb_stage_bytes(D);
     auto st_x = [&](int st) { return reinterpret_cast<float *>(smem + st * stage_bytes); };
     auto st_r = [&](int st) { return reinterpret_cast<float *>(smem + st * stage_bytes + (size_t)TR * D * 4); };
-    auto st_gy = [&](int st) { return reinterpret_cast<__nv_bfloat16 *>(smem + st * stage_bytes + (size_t)TR * D * 8); };
-    auto st_br = [&](int st) { return reinterpret_cast<__nv_bfloat16 *>(smem + st * stage_bytes + (size_t)TR * D * 10); };
+    auto st_gy = [&](int st) { return reinterpret_cast<typename E::T *>(smem + st * stage_bytes + (size_t)TR * D * 8); };
+    auto st_br = [&](int st) { return reinterpret_cast<typename E::T *>(smem + st * stage_bytes + (size_t)TR * D * 10); };
     auto st_sc = [&](int st) { return reinterpret_cast<float *>(smem + st * stage_bytes + (size_t)TR * D * 12); };
     if (threadIdx.x == 0) {
         for (int i = 0; i < nst; ++i) { mbar_init(&full[i], 2); mbar_init(&empty[i], TR); }
@@ -213,8 +221,8 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
                 const float mean = sc[cw], rstd = sc[TR + cw], s_row = sc[2 * TR + cw];
                 const float *xs = st_x(st) + (size_t)cw * D;
                 const float *rs = st_r(st) + (size_t)cw * D;
-                const __nv_bfloat16 *gys = st_gy(st) + (size_t)cw * D;
-                const __nv_bfloat16 *brs = st_br(st) + (size_t)cw * D;
+                const typename E::T *gys = st_gy(st) + (size_t)cw * D;
+                const typename E::T *brs = st_br(st) + (size_t)cw * D;
                 // two passes over the row in SHARED memory (x-hat and g*w are recomputed in pass 2 instead of being kept
                 // in 48 more registers; shared-memory bandwidth is nowhere near binding here)
                 float c1 = 0.f, c2 = 0.f;
@@ -225,7 +233,7 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
                         const float4 xv = *reinterpret_cast<const float4 *>(xs + col);
                         const float4 xh = make_float4((xv.x - mean) * rstd, (xv.y - mean) * rstd, (xv.z - mean) * rstd,
                                                       (xv.w - mean) * rstd);
-                        const float4 g = load_bf16x4(gys + col);
+                        const float4 g = load16x4<E>(gys + col);
                         a0[i].x += g.x * xh.x; a0[i].y += g.y * xh.y; a0[i].z += g.z * xh.z; a0[i].w += g.w * xh.w;
                         a1[i].x += g.x; a1[i].y += g.y; a1[i].z += g.z; a1[i].w += g.w;
                         const float4 gw = make_float4(g.x * w4[i].x, g.y * w4[i].y, g.z * w4[i].z, g.w * w4[i].w);
@@ -244,7 +252,7 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
                         const float4 xv = *reinterpret_cast<const float4 *>(xs + col);
                         const float4 xh = make_float4((xv.x - mean) * rstd, (xv.y - mean) * rstd, (xv.z - mean) * rstd,
                                                       (xv.w - mean) * rstd);
-                        const float4 g = load_bf16x4(gys + col);
+                        const float4 g = load16x4<E>(gys + col);
                         G.x += rstd * (g.x * w4[i].x - c1 - xh.x * c2);
                         G.y += rstd * (g.y * w4[i].y - c1 - xh.y * c2);
                         G.z += rstd * (g.z * w4[i].z - c1 - xh.z * c2);
@@ -252,12 +260,12 @@ residual_ln_bwd_kernel(const float *__restrict__ g_xout, const __nv_bfloat16 *__
                     }
                     if (g_x) *reinterpret_cast<float4 *>(g_x + base + col) = G;
                     if (branch) {
-                        const float4 bv = load_bf16x4(brs + col);
+                        const float4 bv = load16x4<E>(brs + col);
                         const float4 Gs = make_float4(G.x * s_row, G.y * s_row, G.z * s_row, G.w * s_row);
                         a2[i].x += Gs.x * bv.x; a2[i].y += Gs.y * bv.y; a2[i].z += Gs.z * bv.z; a2[i].w += Gs.w * bv.w;
                         a3[i].x += Gs.x; a3[i].y += Gs.y; a3[i].z += Gs.z; a3[i].w += Gs.w;
                         if (g_branch)
-                            store_bf16x4(g_branch + base + col,
+                            store16x4<E>(g_branch + base + col,
                                          make_float4(Gs.x * gm4[i].x, Gs.y * gm4[i].y, Gs.z * gm4[i].z, Gs.w * gm4[i].w));
                     }
                 }
@@ -349,6 +357,7 @@ __device__ __forceinline__ void load_bias8(const float *bias, int c, float (&bb)
         bb[0] = b0.x; bb[1] = b0.y; bb[2] = b0.z; bb[3] = b0.w; bb[4] = b1.x; bb[5] = b1.y; bb[6] = b1.z; bb[7] = b1.w;
     }
 }
+template <typename E>
 __global__ void gelu_fwd_kernel(const uint4 *__restrict__ x, const float *__restrict__ bias, uint4 *__restrict__ y,
                                 int M, int C8) {
     // NON-persistent: one CTA per GELU_RU rows.  Fresh small CTAs avoid the lock-step load/store phases and SM imbalance of
@@ -364,11 +373,11 @@ __global__ void gelu_fwd_kernel(const uint4 *__restrict__ x, const float *__rest
 #pragma unroll
         for (int u = 0; u < GELU_RU; ++u) {
             if (row0 + u >= M) continue;
-            __nv_bfloat162 *p = reinterpret_cast<__nv_bfloat162 *>(&v[u]);
+            typename E::T2 *p = reinterpret_cast<typename E::T2 *>(&v[u]);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                float2 f = __bfloat1622float2(p[k]);
-                p[k] = __floats2bfloat162_rn(gelu_f(f.x + bb[2 * k]), gelu_f(f.y + bb[2 * k + 1]));
+                float2 f = E::to2(p[k]);
+                p[k] = E::from2(gelu_f(f.x + bb[2 * k]), gelu_f(f.y + bb[2 * k + 1]));
             }
             y[(size_t)(row0 + u) * C8 + c] = v[u];
         }
@@ -378,6 +387,7 @@ __global__ void gelu_fwd_kernel(const uint4 *__restrict__ x, const float *__rest
 // gx = gy * gelu'(x + bias); column sums of gx (= d bias) accumulate per thread, one atomicAdd per column
 // per CTA at the end (g_bias must be zeroed by the caller).
 constexpr int GELU_BWD_RU = 2;
+template <typename E>
 __global__ void gelu_bwd_kernel(const uint4 *__restrict__ x, const float *__restrict__ bias, const uint4 *__restrict__ gy,
                                 uint4 *__restrict__ gx, float *__restrict__ g_bias, int M, int C8) {
     // persistent (the column sums stay in registers, one atomicAdd per column per CTA) and SOFTWARE-PIPELINED: the loads
@@ -400,14 +410,14 @@ __global__ void gelu_bwd_kernel(const uint4 *__restrict__ x, const float *__rest
 #pragma unroll
             for (int u = 0; u < RU; ++u) {
                 if (row0 + u >= M) continue;
-                __nv_bfloat162 *p = reinterpret_cast<__nv_bfloat162 *>(&v[u]);
-                __nv_bfloat162 *q = reinterpret_cast<__nv_bfloat162 *>(&g[u]);
+                typename E::T2 *p = reinterpret_cast<typename E::T2 *>(&v[u]);
+                typename E::T2 *q = reinterpret_cast<typename E::T2 *>(&g[u]);
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
-                    float2 f = __bfloat1622float2(p[k]), h = __bfloat1622float2(q[k]);
+                    float2 f = E::to2(p[k]), h = E::to2(q[k]);
                     float r0 = h.x * dgelu_f(f.x + bb[2 * k]), r1 = h.y * dgelu_f(f.y + bb[2 * k + 1]);
                     acc[2 * k] += r0; acc[2 * k + 1] += r1;
-                    p[k] = __floats2bfloat162_rn(r0, r1);
+                    p[k] = E::from2(r0, r1);
                 }
                 gx[(size_t)(row0 + u) * C8 + c] = v[u];
             }
@@ -427,7 +437,8 @@ __global__ void gelu_bwd_kernel(const uint4 *__restrict__ x, const float *__rest
 // This kernel writes `patches` in bf16 (GEMM operand) from the fp32 NCHW image: 4 pixels (16 B in, 8 B out) per thread,
 // output-major indexing -> fully coalesced stores, 64-byte-segment loads.  (cuDNN's implicit-GEMM for Cin = 3 pads the
 // channel dimension to 8 and adds two layout conversions: 4.3 ms per step at B = 256 vs 0.1 ms here + a 0.06 ms GEMM.)
-__global__ void patchify_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ out, int Cin, int H, int W, int p,
+template <typename E>
+__global__ void patchify_kernel(const float *__restrict__ x, typename E::T *__restrict__ out, int Cin, int H, int W, int p,
                                 size_t total4) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total4) return;
@@ -440,7 +451,7 @@ __global__ void patchify_kernel(const float *__restrict__ x, __nv_bfloat16 *__re
     const int py = (int)(t % gh); t /= gh;
     const size_t b = t;
     const float4 v = *reinterpret_cast<const float4 *>(x + ((b * Cin + c) * H + (size_t)py * p + ky) * W + (size_t)px * p + kx4 * 4);
-    store_bf16x4(out + i * 4, v);
+    store16x4<E>(out + i * 4, v);
 }
 
 // Token assembly (dinov2.py:151-170 / 318-336): the encoder / decoder build their input sequence as
@@ -450,8 +461,9 @@ __global__ void patchify_kernel(const float *__restrict__ x, __nv_bfloat16 *__re
 //   out[b, t, :] = table[t, :] + (t0 <= t < t0 + Ls ? src[b, t - t0, :] : 0)
 // where `table` [T, D] is the module's own assembly evaluated once on a zero input of batch 1 (host side, autograd intact).
 // fwd: one pass (read src, write out).  bwd: ONE read of g produces d_src (cast to the source dtype) and d_table = sum_b g.
+// TS: float, or the 16-bit element trait (Bf16 / F16) of a 16-bit source
 template <typename TS>
-__global__ void assemble_fwd_kernel(const TS *__restrict__ src, const float *__restrict__ table, int Ls, int T, int D4, int t0,
+__global__ void assemble_fwd_kernel(const void *__restrict__ src, const float *__restrict__ table, int Ls, int T, int D4, int t0,
                                     float *__restrict__ out, size_t total4) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total4) return;
@@ -463,15 +475,15 @@ __global__ void assemble_fwd_kernel(const TS *__restrict__ src, const float *__r
     if (t >= t0 && t < t0 + Ls) {
         const size_t so = ((b * Ls + (t - t0)) * D4 + d4) * 4;
         float4 sv;
-        if (sizeof(TS) == 2) sv = load_bf16x4(reinterpret_cast<const __nv_bfloat16 *>(src) + so);
-        else sv = *reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(src) + so);
+        if constexpr (std::is_same<TS, float>::value) sv = *reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(src) + so);
+        else sv = load16x4<TS>(reinterpret_cast<const typename TS::T *>(src) + so);
         v.x += sv.x; v.y += sv.y; v.z += sv.z; v.w += sv.w;
     }
     *reinterpret_cast<float4 *>(out + i * 4) = v;
 }
 
 template <typename TS>
-__global__ void assemble_bwd_kernel(const float *__restrict__ g, int B, int Ls, int T, int D4, int t0, TS *__restrict__ d_src,
+__global__ void assemble_bwd_kernel(const float *__restrict__ g, int B, int Ls, int T, int D4, int t0, void *__restrict__ d_src,
                                     float *__restrict__ d_table) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;      // (t, d4)
     if (i >= T * D4) return;
@@ -490,8 +502,8 @@ __global__ void assemble_bwd_kernel(const float *__restrict__ g, int B, int Ls, 
             acc.x += v[u].x; acc.y += v[u].y; acc.z += v[u].z; acc.w += v[u].w;
             if (in_src && b0 + u < B) {
                 const size_t so = (((size_t)(b0 + u) * Ls + (t - t0)) * D4 + d4) * 4;
-                if (sizeof(TS) == 2) store_bf16x4(reinterpret_cast<__nv_bfloat16 *>(d_src) + so, v[u]);
-                else *reinterpret_cast<float4 *>(reinterpret_cast<float *>(d_src) + so) = v[u];
+                if constexpr (std::is_same<TS, float>::value) *reinterpret_cast<float4 *>(reinterpret_cast<float *>(d_src) + so) = v[u];
+                else store16x4<TS>(reinterpret_cast<typename TS::T *>(d_src) + so, v[u]);
             }
         }
     }
@@ -510,34 +522,31 @@ using namespace xqv;
         default: return XQ_ERR_UNSUPPORTED;    \
     }
 
-extern "C" {
+namespace xqv {
 
-// the TMA-staged kernels run 1 CTA / SM (their tiles fill the shared memory)
-size_t xq_vit_ln_bwd_workspace_bytes(int D) {
-    int sms = 0;
-    if (xq::sm_count(&sms) != XQ_OK) return 0;
-    return sizeof(float) * (size_t)sms * NACC * D + 256;
-}
-
-int xq_vit_residual_ln_fwd(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
+template <typename E>
+static int residual_ln_fwd(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
                            const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
                            int M, int D, float *x_out, void *y, float *mean, float *rstd, void *stream) {
+    using T = typename E::T;
     if (!x || M <= 0 || (y && (!ln_w || !ln_b)) || (!x_out && !y)) return XQ_ERR_ARG;
     if (branch && rowscale && rows_per_sample <= 0) return XQ_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     int grid = (M + WARPS * FR - 1) / (WARPS * FR);
-    XQV_DISPATCH(D, (residual_ln_fwd_kernel<NV><<<grid, THREADS, 0, st>>>(
-                        x, (const __nv_bfloat16 *)branch, branch_bias, ls_gamma, rowscale, rows_per_sample, ln_w, ln_b,
-                        eps, M, x_out, (__nv_bfloat16 *)y, mean, rstd)));
+    XQV_DISPATCH(D, (residual_ln_fwd_kernel<E, NV><<<grid, THREADS, 0, st>>>(
+                        x, (const T *)branch, branch_bias, ls_gamma, rowscale, rows_per_sample, ln_w, ln_b,
+                        eps, M, x_out, (T *)y, mean, rstd)));
     XQ_LAUNCH_CHECK("residual_ln_fwd_kernel");
     return XQ_OK;
 }
 
-int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_out, const float *mean,
+template <typename E>
+static int residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_out, const float *mean,
                            const float *rstd, const float *ln_w, const void *branch, const float *branch_bias,
                            const float *ls_gamma, const float *rowscale, int rows_per_sample, int M, int D, float *g_x,
                            void *g_branch, float *g_ln_w, float *g_ln_b, float *g_ls_gamma, float *g_branch_bias,
                            void *workspace, size_t workspace_bytes, void *stream) {
+    using T = typename E::T;
     if (!x_out || !mean || !rstd || M <= 0 || !workspace) return XQ_ERR_ARG;
     if (g_y && !ln_w) return XQ_ERR_ARG;
     if (branch && rowscale && rows_per_sample <= 0) return XQ_ERR_ARG;
@@ -555,10 +564,10 @@ int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_
     size_t smem = lnb_stage_bytes(D) * nst;
     if (smem < sizeof(float) * (size_t)LNB_TR * NACC * D) smem = sizeof(float) * (size_t)LNB_TR * NACC * D;
     XQV_DISPATCH(D, {
-        if (int rc = xq::smem_optin(residual_ln_bwd_kernel<NV>, smem)) return rc;
-        residual_ln_bwd_kernel<NV><<<grid, LNB_THREADS, smem, st>>>(
-            g_xout, (const __nv_bfloat16 *)g_y, x_out, mean, rstd, ln_w, (const __nv_bfloat16 *)branch, branch_bias,
-            ls_gamma, rowscale, rows_per_sample, M, g_x, (__nv_bfloat16 *)g_branch, part, counter, nst);
+        if (int rc = xq::smem_optin(residual_ln_bwd_kernel<E, NV>, smem)) return rc;
+        residual_ln_bwd_kernel<E, NV><<<grid, LNB_THREADS, smem, st>>>(
+            g_xout, (const T *)g_y, x_out, mean, rstd, ln_w, (const T *)branch, branch_bias,
+            ls_gamma, rowscale, rows_per_sample, M, g_x, (T *)g_branch, part, counter, nst);
     });
     XQ_LAUNCH_CHECK("residual_ln_bwd_kernel");
     reduce_parts_kernel<<<(D + 31) / 32, 256, 0, st>>>(part, grid, D, ls_gamma, branch_bias, g_ln_w, g_ln_b,
@@ -567,63 +576,135 @@ int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_
     return XQ_OK;
 }
 
-int xq_vit_assemble_fwd(const void *src, int src_is_bf16, const float *table, int B, int Ls, int T, int D, int t0, float *out,
-                        void *stream) {
-    if (!src || !table || !out || B <= 0 || Ls <= 0 || T <= 0 || D <= 0 || (D & 3) || t0 < 0 || t0 + Ls > T) return XQ_ERR_ARG;
-    const size_t total4 = (size_t)B * T * (D / 4);
-    const unsigned grid = (unsigned)((total4 + 255) / 256);
-    if (src_is_bf16)
-        assemble_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)src, table, Ls, T, D / 4, t0, out, total4);
-    else
-        assemble_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const float *)src, table, Ls, T, D / 4, t0, out, total4);
-    XQ_LAUNCH_CHECK("assemble_fwd_kernel");
-    return XQ_OK;
-}
-
-int xq_vit_assemble_bwd(const float *g, int B, int Ls, int T, int D, int t0, void *d_src, int src_is_bf16, float *d_table,
-                        void *stream) {
-    if (!g || (!d_src && !d_table) || B <= 0 || Ls <= 0 || T <= 0 || D <= 0 || (D & 3) || t0 < 0 || t0 + Ls > T) return XQ_ERR_ARG;
-    const int n = T * (D / 4);
-    if (src_is_bf16)
-        assemble_bwd_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(g, B, Ls, T, D / 4, t0, (__nv_bfloat16 *)d_src, d_table);
-    else
-        assemble_bwd_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(g, B, Ls, T, D / 4, t0, (float *)d_src, d_table);
-    XQ_LAUNCH_CHECK("assemble_bwd_kernel");
-    return XQ_OK;
-}
-
-int xq_vit_patchify(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream) {
+template <typename E>
+static int patchify(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream) {
     if (!x || !patches || B <= 0 || Cin <= 0 || H <= 0 || W <= 0 || p <= 0) return XQ_ERR_ARG;
     if ((p & 3) || H % p || W % p) return XQ_ERR_UNSUPPORTED;
     const size_t total4 = (size_t)B * Cin * H * W / 4;
-    patchify_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)patches, Cin, H, W,
-                                                                                       p, total4);
+    patchify_kernel<E><<<(unsigned)((total4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, (typename E::T *)patches, Cin, H, W,
+                                                                                          p, total4);
     XQ_LAUNCH_CHECK("patchify_kernel");
     return XQ_OK;
 }
 
-int xq_vit_gelu_fwd(const void *x, const float *bias, void *y, int M, int C, void *stream) {
+template <typename E>
+static int gelu_fwd(const void *x, const float *bias, void *y, int M, int C, void *stream) {
     if (!x || !y || M <= 0 || C <= 0 || (C & 7)) return XQ_ERR_ARG;
     int C8 = C / 8;
     int threads = C8 >= 384 ? 384 : (C8 >= 192 ? 192 : 128);
     int grid = (M + GELU_RU - 1) / GELU_RU;
-    gelu_fwd_kernel<<<grid, threads, 0, (cudaStream_t)stream>>>((const uint4 *)x, bias, (uint4 *)y, M, C8);
+    gelu_fwd_kernel<E><<<grid, threads, 0, (cudaStream_t)stream>>>((const uint4 *)x, bias, (uint4 *)y, M, C8);
     XQ_LAUNCH_CHECK("gelu_fwd_kernel");
     return XQ_OK;
 }
 
-int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C, void *stream) {
+template <typename E>
+static int gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C, void *stream) {
     if (!x || !gy || !gx || M <= 0 || C <= 0 || (C & 7)) return XQ_ERR_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     int C8 = C / 8;
     int threads = C8 >= 384 ? 384 : (C8 >= 192 ? 192 : 128);
     int grid = 0;
-    if (int rc = xq::persistent_grid(gelu_bwd_kernel, threads, &grid)) return rc;
+    if (int rc = xq::persistent_grid(gelu_bwd_kernel<E>, threads, &grid)) return rc;
     if ((M + GELU_BWD_RU - 1) / GELU_BWD_RU < grid) grid = (M + GELU_BWD_RU - 1) / GELU_BWD_RU;
     if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, sizeof(float) * (size_t)C, st));
-    gelu_bwd_kernel<<<grid, threads, 0, st>>>((const uint4 *)x, bias, (const uint4 *)gy, (uint4 *)gx, g_bias, M, C8);
+    gelu_bwd_kernel<E><<<grid, threads, 0, st>>>((const uint4 *)x, bias, (const uint4 *)gy, (uint4 *)gx, g_bias, M, C8);
     XQ_LAUNCH_CHECK("gelu_bwd_kernel");
     return XQ_OK;
+}
+
+}  // namespace xqv
+
+extern "C" {
+
+// the TMA-staged kernels run 1 CTA / SM (their tiles fill the shared memory)
+size_t xq_vit_ln_bwd_workspace_bytes(int D) {
+    int sms = 0;
+    if (xq::sm_count(&sms) != XQ_OK) return 0;
+    return sizeof(float) * (size_t)sms * NACC * D + 256;
+}
+
+int xq_vit_residual_ln_fwd(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
+                           const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
+                           int M, int D, float *x_out, void *y, float *mean, float *rstd, void *stream) {
+    return residual_ln_fwd<Bf16>(x, branch, branch_bias, ls_gamma, rowscale, rows_per_sample, ln_w, ln_b, eps, M, D, x_out, y,
+                                 mean, rstd, stream);
+}
+int xq_vit_residual_ln_fwd_f16(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
+                               const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
+                               int M, int D, float *x_out, void *y, float *mean, float *rstd, void *stream) {
+    return residual_ln_fwd<F16>(x, branch, branch_bias, ls_gamma, rowscale, rows_per_sample, ln_w, ln_b, eps, M, D, x_out, y,
+                                mean, rstd, stream);
+}
+
+int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_out, const float *mean,
+                           const float *rstd, const float *ln_w, const void *branch, const float *branch_bias,
+                           const float *ls_gamma, const float *rowscale, int rows_per_sample, int M, int D, float *g_x,
+                           void *g_branch, float *g_ln_w, float *g_ln_b, float *g_ls_gamma, float *g_branch_bias,
+                           void *workspace, size_t workspace_bytes, void *stream) {
+    return residual_ln_bwd<Bf16>(g_xout, g_y, x_out, mean, rstd, ln_w, branch, branch_bias, ls_gamma, rowscale, rows_per_sample,
+                                 M, D, g_x, g_branch, g_ln_w, g_ln_b, g_ls_gamma, g_branch_bias, workspace, workspace_bytes, stream);
+}
+int xq_vit_residual_ln_bwd_f16(const float *g_xout, const void *g_y, const float *x_out, const float *mean,
+                               const float *rstd, const float *ln_w, const void *branch, const float *branch_bias,
+                               const float *ls_gamma, const float *rowscale, int rows_per_sample, int M, int D, float *g_x,
+                               void *g_branch, float *g_ln_w, float *g_ln_b, float *g_ls_gamma, float *g_branch_bias,
+                               void *workspace, size_t workspace_bytes, void *stream) {
+    return residual_ln_bwd<F16>(g_xout, g_y, x_out, mean, rstd, ln_w, branch, branch_bias, ls_gamma, rowscale, rows_per_sample,
+                                M, D, g_x, g_branch, g_ln_w, g_ln_b, g_ls_gamma, g_branch_bias, workspace, workspace_bytes, stream);
+}
+
+// src_type: 0 fp32, 1 bf16, 2 f16 (XQ_ASSEMBLE_*)
+int xq_vit_assemble_fwd(const void *src, int src_type, const float *table, int B, int Ls, int T, int D, int t0, float *out,
+                        void *stream) {
+    if (!src || !table || !out || B <= 0 || Ls <= 0 || T <= 0 || D <= 0 || (D & 3) || t0 < 0 || t0 + Ls > T) return XQ_ERR_ARG;
+    const size_t total4 = (size_t)B * T * (D / 4);
+    const unsigned grid = (unsigned)((total4 + 255) / 256);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (src_type == XQ_ASSEMBLE_F16)
+        assemble_fwd_kernel<F16><<<grid, 256, 0, st>>>(src, table, Ls, T, D / 4, t0, out, total4);
+    else if (src_type)
+        assemble_fwd_kernel<Bf16><<<grid, 256, 0, st>>>(src, table, Ls, T, D / 4, t0, out, total4);
+    else
+        assemble_fwd_kernel<float><<<grid, 256, 0, st>>>(src, table, Ls, T, D / 4, t0, out, total4);
+    XQ_LAUNCH_CHECK("assemble_fwd_kernel");
+    return XQ_OK;
+}
+
+int xq_vit_assemble_bwd(const float *g, int B, int Ls, int T, int D, int t0, void *d_src, int src_type, float *d_table,
+                        void *stream) {
+    if (!g || (!d_src && !d_table) || B <= 0 || Ls <= 0 || T <= 0 || D <= 0 || (D & 3) || t0 < 0 || t0 + Ls > T) return XQ_ERR_ARG;
+    const int n = T * (D / 4);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (src_type == XQ_ASSEMBLE_F16)
+        assemble_bwd_kernel<F16><<<(n + 127) / 128, 128, 0, st>>>(g, B, Ls, T, D / 4, t0, d_src, d_table);
+    else if (src_type)
+        assemble_bwd_kernel<Bf16><<<(n + 127) / 128, 128, 0, st>>>(g, B, Ls, T, D / 4, t0, d_src, d_table);
+    else
+        assemble_bwd_kernel<float><<<(n + 127) / 128, 128, 0, st>>>(g, B, Ls, T, D / 4, t0, d_src, d_table);
+    XQ_LAUNCH_CHECK("assemble_bwd_kernel");
+    return XQ_OK;
+}
+
+int xq_vit_patchify(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream) {
+    return patchify<Bf16>(x, patches, B, Cin, H, W, p, stream);
+}
+int xq_vit_patchify_f16(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream) {
+    return patchify<F16>(x, patches, B, Cin, H, W, p, stream);
+}
+
+int xq_vit_gelu_fwd(const void *x, const float *bias, void *y, int M, int C, void *stream) {
+    return gelu_fwd<Bf16>(x, bias, y, M, C, stream);
+}
+int xq_vit_gelu_fwd_f16(const void *x, const float *bias, void *y, int M, int C, void *stream) {
+    return gelu_fwd<F16>(x, bias, y, M, C, stream);
+}
+
+int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C, void *stream) {
+    return gelu_bwd<Bf16>(x, bias, gy, gx, g_bias, M, C, stream);
+}
+int xq_vit_gelu_bwd_f16(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C, void *stream) {
+    return gelu_bwd<F16>(x, bias, gy, gx, g_bias, M, C, stream);
 }
 
 }  // extern "C"

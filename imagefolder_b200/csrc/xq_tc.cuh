@@ -1,8 +1,8 @@
-// xq_tc.cuh -- PTX wrappers for the bf16 / tf32 wgmma + TMA + mbarrier kernels of libxqb200 (sm_90a), and the library's one
+// xq_tc.cuh -- PTX wrappers for the bf16 / f16 / tf32 wgmma + TMA + mbarrier kernels of libxqb200 (sm_90a), and the library's one
 // tensor-map cache.
 //
 // Shared-memory operand layouts used by the attention and GEMM kernels (all SWIZZLE_128B, 1024-byte aligned tiles):
-//   "row tile"  [R rows][64 bf16]  = what one TMA box {64, R, 1} of a [.., rows, 64*k] tensor lands as:
+//   "row tile"  [R rows][64 bf16 / f16]  = what one TMA box {64, R, 1} of a [.., rows, 64*k] tensor lands as:
 //               byte(r, c) = r*128 + (((c >> 3) ^ (r & 7)) << 4) + (c & 7)*2
 //     * as a K-major operand   (MMA K runs along the 64 columns): rows are M (or N), descriptor SBO = 1024
 //     * as an MN-major operand (MMA K runs along the ROWS, M/N along the 64 columns): 8 rows = one swizzle atom,
@@ -14,6 +14,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -150,38 +151,51 @@ __device__ __forceinline__ void fence_regs(float (&d)[N]) {
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// E: the 16-bit operand type (Bf16 or F16 below); the accumulator is fp32 either way.
 // D[64 x 64] (+)= A[64 x 16] B[16 x 64], A and B from shared memory (descriptors); TA / TB: operand is MN-major
-template <int TA, int TB>
+#define XQ_WGMMA_M64N64K16_SS(TY) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB))
+template <typename E, int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+    if constexpr (E::IS_F16) XQ_WGMMA_M64N64K16_SS("f16");
+    else XQ_WGMMA_M64N64K16_SS("bf16");
 }
+#undef XQ_WGMMA_M64N64K16_SS
 
 // D[64 x 128] (+)= A[64 x 16] B[16 x 128], A and B from shared memory (descriptors); TA / TB: operand is MN-major
-template <int TA, int TB>
+#define XQ_WGMMA_M64N128K16_SS(TY) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB))
+template <typename E, int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+    if constexpr (E::IS_F16) XQ_WGMMA_M64N128K16_SS("f16");
+    else XQ_WGMMA_M64N128K16_SS("bf16");
 }
+#undef XQ_WGMMA_M64N128K16_SS
 
-// D[64 x 64] (+)= A[64 x 16] B[16 x 64], A from registers (accumulator fragment layout, bf16 pairs), B from shared memory
-template <int TB>
+// D[64 x 64] (+)= A[64 x 16] B[16 x 64], A from registers (accumulator fragment layout, 16-bit pairs), B from shared memory
+#define XQ_WGMMA_M64N64K16_RS(TY) \
+    asm volatile( \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t" \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " " \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}" \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(TB))
+template <typename E, int TB>
 __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(TB));
+    if constexpr (E::IS_F16) XQ_WGMMA_M64N64K16_RS("f16");
+    else XQ_WGMMA_M64N64K16_RS("bf16");
 }
+#undef XQ_WGMMA_M64N64K16_RS
 
 // D[64 x 128] (+)= A[64 x 8] B[8 x 128], TF32 operands (both K-major) from shared memory
 __device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
@@ -211,7 +225,7 @@ __device__ __forceinline__ bool elect_one() {
 }
 
 // ---- misc ------------------------------------------------------------------------------------------------
-// byte offset of element (row r, column c) of a [rows][64 bf16] SWIZZLE_128B row tile
+// byte offset of element (row r, column c) of a [rows][64 x 16-bit] SWIZZLE_128B row tile
 __host__ __device__ __forceinline__ uint32_t rowtile_off_bf16(int r, int c) {
     return (uint32_t)(r * 128 + ((((c >> 3) ^ (r & 7)) & 7) << 4) + (c & 7) * 2);
 }
@@ -223,6 +237,50 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));   // upper half <- first source
     return r;
 }
+__device__ __forceinline__ uint32_t pack_f16(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));    // upper half <- first source
+    return r;
+}
+
+// The two 16-bit operand types of the tensor-core kernels, as a template parameter.  Every fp32 -> 16-bit conversion
+// rounds to nearest even and gives +-inf on overflow (never .satfinite, which would clamp an f16 to +-65504 and hide the
+// overflow from a gradient scaler); lo / hi read the low / high element of a packed pair.
+struct Bf16 {
+    using T = __nv_bfloat16;
+    using T2 = __nv_bfloat162;
+    static constexpr bool IS_F16 = false;
+    static constexpr CUtensorMapDataType TMAP = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    static __device__ __forceinline__ uint32_t pack(float lo, float hi) { return pack_bf16(lo, hi); }
+    static __device__ __forceinline__ float lo(uint32_t w) { return __uint_as_float(w << 16); }
+    static __device__ __forceinline__ float hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+    static __device__ __forceinline__ T from(float x) { return __float2bfloat16(x); }
+    static __device__ __forceinline__ float to(T x) { return __bfloat162float(x); }
+    static __device__ __forceinline__ T2 from2(float a, float b) { return __floats2bfloat162_rn(a, b); }
+    static __device__ __forceinline__ float2 to2(T2 x) { return __bfloat1622float2(x); }
+};
+struct F16 {
+    using T = __half;
+    using T2 = __half2;
+    static constexpr bool IS_F16 = true;
+    static constexpr CUtensorMapDataType TMAP = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    static __device__ __forceinline__ uint32_t pack(float lo, float hi) { return pack_f16(lo, hi); }
+    static __device__ __forceinline__ float lo(uint32_t w) {
+        float f;
+        asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %1;\n\tcvt.f32.f16 %0, l;\n\t}" : "=f"(f) : "r"(w));
+        return f;
+    }
+    static __device__ __forceinline__ float hi(uint32_t w) {
+        float f;
+        asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %1;\n\tcvt.f32.f16 %0, h;\n\t}" : "=f"(f) : "r"(w));
+        return f;
+    }
+    static __device__ __forceinline__ T from(float x) { return __float2half_rn(x); }
+    static __device__ __forceinline__ float to(T x) { return __half2float(x); }
+    static __device__ __forceinline__ T2 from2(float a, float b) { return __floats2half2_rn(a, b); }
+    static __device__ __forceinline__ float2 to2(T2 x) { return __half22float2(x); }
+};
+
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -276,12 +334,13 @@ inline bool tensor_map(CUtensorMap *out, const void *base, CUtensorMapDataType d
     return true;
 }
 
-// bf16 3-D tensor map {inner, rows, batch} with box {64, box_rows, 1}, SWIZZLE_128B (64 bf16 = 128 bytes)
-inline bool tensor_map_bf16_3d(CUtensorMap *out, const void *base, uint64_t inner, uint64_t rows, uint64_t batch,
-                               uint64_t row_stride_bytes, uint64_t batch_stride_bytes, uint32_t box_rows) {
+// 16-bit 3-D tensor map {inner, rows, batch} with box {64, box_rows, 1}, SWIZZLE_128B (64 elements = 128 bytes);
+// dtype: CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 or _FLOAT16 (Bf16::TMAP / F16::TMAP)
+inline bool tensor_map_16_3d(CUtensorMap *out, CUtensorMapDataType dtype, const void *base, uint64_t inner, uint64_t rows,
+                             uint64_t batch, uint64_t row_stride_bytes, uint64_t batch_stride_bytes, uint32_t box_rows) {
     const cuuint64_t dims[3] = {inner, rows, batch}, strides[2] = {row_stride_bytes, batch_stride_bytes};
     const cuuint32_t box[3] = {64u, box_rows, 1u};
-    return tensor_map(out, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    return tensor_map(out, base, dtype, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 }  // namespace xqtc

@@ -7,8 +7,10 @@ by ONE kernel (`xq_vit_residual_ln_fwd`), GELU by one bf16 kernel and attention 
 kernels of csrc/attn_kernel.cu (`xq_vit_attn_fwd/bwd`, reading the packed qkv projection in place and writing d(qkv)
 in the packed layout); the projection GEMMs stay on cuBLAS.  Blocks the attention kernels do not cover (head dims other
 than 64, attention dropout > 0 in training, qk_norm; no shipped config) run the module's own Attention.forward for
-their attention.  The residual stream is fp32 and the GEMM operands bf16,
-which is what bf16 autocast gives the reference, so the numerics are the reference's.
+their attention.  The residual stream is fp32 and the GEMM operands are the autocast dtype, bf16 or fp16: the
+`_f16` twin of every entry point runs the same kernel instantiated for fp16.  That is what bf16 / fp16 autocast gives the
+reference, so the numerics are the reference's.  Without autocast (or under another autocast dtype) `run_blocks` takes the
+module path.
 """
 from __future__ import annotations
 
@@ -20,6 +22,27 @@ from . import _capi as C
 from ._capi import call as _call, lib as _lib, ptr as _ptr, stream_ptr as _stream
 
 _SUPPORTED_D = (384, 768, 1024)
+_HALF = (torch.bfloat16, torch.float16)       # the GEMM operand dtypes the kernels are instantiated for
+
+
+def _autocast_half():
+    """the CUDA autocast dtype when autocast is on and it is bf16 or fp16, else None"""
+    if not torch.is_autocast_enabled():
+        return None
+    dt = torch.get_autocast_dtype("cuda")
+    return dt if dt in _HALF else None
+
+
+def _op_dtype():
+    """16-bit operand dtype of a glue kernel whose inputs do not fix it: fp16 under fp16 autocast, else bf16"""
+    return torch.float16 if _autocast_half() == torch.float16 else torch.bfloat16
+
+
+def _entry(name: str, dt):
+    """(symbol name, function) of entry point `name` for 16-bit dtype `dt`: its `_f16` twin for fp16, else the bf16 one"""
+    if dt == torch.float16:
+        name += "_f16"
+    return name, getattr(C.lib(), name)
 
 
 def _lora():
@@ -33,31 +56,34 @@ def _live(m):
 
 
 class _ResidualLN(torch.autograd.Function):
-    """(x, branch, branch_bias, ls_gamma, rowscale, ln_w, ln_b) -> (x_out fp32, y bf16)
-    x_out = x + rowscale * ls_gamma * (branch + branch_bias);  y = LayerNorm(x_out)."""
+    """(x, branch, branch_bias, ls_gamma, rowscale, ln_w, ln_b) -> (x_out fp32, y 16-bit)
+    x_out = x + rowscale * ls_gamma * (branch + branch_bias);  y = LayerNorm(x_out).
+    branch / y are fp16 under fp16 autocast, else bf16 (_op_dtype)."""
 
     @staticmethod
     def forward(ctx, x, branch, branch_bias, ls_gamma, rowscale, ln_w, ln_b, eps: float):
         Bn, S, D = x.shape
         M = Bn * S
+        dt = _op_dtype()
         x = x.contiguous()
         if x.dtype != torch.float32:
             x = x.float()
         if branch is not None:
             branch = branch.contiguous()
-            if branch.dtype != torch.bfloat16:
-                branch = branch.to(torch.bfloat16)
+            if branch.dtype != dt:
+                branch = branch.to(dt)
         x_out = torch.empty_like(x)
-        y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+        y = torch.empty(x.shape, dtype=dt, device=x.device)
         mean = torch.empty(M, dtype=torch.float32, device=x.device)
         rstd = torch.empty(M, dtype=torch.float32, device=x.device)
-        L = C.lib()
-        C.call("xq_vit_residual_ln_fwd", 1, L.xq_vit_residual_ln_fwd, C.ptr(x), C.ptr(branch), C.ptr(branch_bias),
+        name, fn = _entry("xq_vit_residual_ln_fwd", dt)
+        C.call(name, 1, fn, C.ptr(x), C.ptr(branch), C.ptr(branch_bias),
                C.ptr(ls_gamma), C.ptr(rowscale), S, C.ptr(ln_w), C.ptr(ln_b), float(eps), M, D, C.ptr(x_out), C.ptr(y),
                C.ptr(mean), C.ptr(rstd), C.stream_ptr(x.device),
                nbytes=M * D * (10 + (2 if branch is not None else 0)))
         ctx.save_for_backward(x_out, mean, rstd, ln_w, branch, branch_bias, ls_gamma, rowscale)
         ctx.shape = (Bn, S, D)
+        ctx.dt = dt
         ctx.set_materialize_grads(False)
         return x_out, y
 
@@ -73,8 +99,8 @@ class _ResidualLN(torch.autograd.Function):
                 g_xout = g_xout.float()
         if g_y is not None:
             g_y = g_y.contiguous()
-            if g_y.dtype != torch.bfloat16:
-                g_y = g_y.to(torch.bfloat16)
+            if g_y.dtype != ctx.dt:
+                g_y = g_y.to(ctx.dt)
         g_x = torch.empty_like(x_out)
         g_branch = torch.empty_like(branch) if branch is not None else None
         g_w = torch.empty_like(ln_w)
@@ -83,7 +109,8 @@ class _ResidualLN(torch.autograd.Function):
         g_bb = torch.empty_like(branch_bias) if (branch is not None and branch_bias is not None) else None
         L = C.lib()
         ws = C.workspace(L.xq_vit_ln_bwd_workspace_bytes(D), dev)
-        C.call("xq_vit_residual_ln_bwd", 2, L.xq_vit_residual_ln_bwd, C.ptr(g_xout), C.ptr(g_y), C.ptr(x_out),
+        name, fn = _entry("xq_vit_residual_ln_bwd", ctx.dt)
+        C.call(name, 2, fn, C.ptr(g_xout), C.ptr(g_y), C.ptr(x_out),
                C.ptr(mean), C.ptr(rstd), C.ptr(ln_w), C.ptr(branch), C.ptr(branch_bias), C.ptr(ls_gamma),
                C.ptr(rowscale), S, M, D, C.ptr(g_x), C.ptr(g_branch), C.ptr(g_w), C.ptr(g_b), C.ptr(g_g), C.ptr(g_bb),
                C.ptr(ws), ws.numel(), C.stream_ptr(dev),
@@ -97,7 +124,7 @@ def residual_ln(x, branch, branch_bias, ls_gamma, rowscale, ln_w, ln_b, eps=1e-6
 
 
 class _GeluBias(torch.autograd.Function):
-    """y = GELU(x + bias), x bf16 [..., C] (the fc1 GEMM output WITHOUT its bias), bias fp32 [C]."""
+    """y = GELU(x + bias), x bf16 or fp16 [..., C] (the fc1 GEMM output WITHOUT its bias), bias fp32 [C]."""
 
     @staticmethod
     def forward(ctx, x, bias):
@@ -105,8 +132,8 @@ class _GeluBias(torch.autograd.Function):
         Cc = x.shape[-1]
         M = x.numel() // Cc
         y = torch.empty_like(x)
-        L = C.lib()
-        C.call("xq_vit_gelu_fwd", 1, L.xq_vit_gelu_fwd, C.ptr(x), C.ptr(bias), C.ptr(y), M, Cc, C.stream_ptr(x.device),
+        name, fn = _entry("xq_vit_gelu_fwd", x.dtype)
+        C.call(name, 1, fn, C.ptr(x), C.ptr(bias), C.ptr(y), M, Cc, C.stream_ptr(x.device),
                nbytes=M * Cc * 4)
         ctx.save_for_backward(x, bias)
         return y
@@ -115,14 +142,15 @@ class _GeluBias(torch.autograd.Function):
     def backward(ctx, gy):
         x, bias = ctx.saved_tensors
         gy = gy.contiguous()
-        if gy.dtype != torch.bfloat16:
-            gy = gy.to(torch.bfloat16)
+        dt = torch.float16 if x.dtype == torch.float16 else torch.bfloat16
+        if gy.dtype != dt:
+            gy = gy.to(dt)
         Cc = x.shape[-1]
         M = x.numel() // Cc
         gx = torch.empty_like(x)
         gb = torch.empty_like(bias) if bias is not None else None
-        L = C.lib()
-        C.call("xq_vit_gelu_bwd", 1, L.xq_vit_gelu_bwd, C.ptr(x), C.ptr(bias), C.ptr(gy), C.ptr(gx), C.ptr(gb), M, Cc,
+        name, fn = _entry("xq_vit_gelu_bwd", dt)
+        C.call(name, 1, fn, C.ptr(x), C.ptr(bias), C.ptr(gy), C.ptr(gx), C.ptr(gb), M, Cc,
                C.stream_ptr(x.device), nbytes=M * Cc * 6)
         return gx, gb
 
@@ -144,9 +172,10 @@ def _sm_count(device) -> int:
 
 
 def mlp_tc_ok(y, fc1, fc2) -> bool:
-    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd cover the shipped widths: bf16 tokens, hidden % 256 == 0, embed % 64 == 0,
+    """xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd (and their _f16 twins) cover the shipped widths: bf16 or fp16 tokens,
+    hidden % 256 == 0, embed % 64 == 0,
     out % 64 == 0 (the K of the backward GEMM), and at most one CTA column per SM (hidden / 128 <= SM count)."""
-    return (MLP_TC_ENABLED[0] and y.is_cuda and y.dtype == torch.bfloat16 and fc1.bias is not None
+    return (MLP_TC_ENABLED[0] and y.is_cuda and y.dtype in _HALF and fc1.bias is not None
             and fc1.weight.shape[0] % 256 == 0 and fc1.weight.shape[1] % 64 == 0
             and fc2.weight.shape[1] == fc1.weight.shape[0] and fc2.weight.shape[0] % 64 == 0
             and fc1.weight.shape[0] // 128 <= _sm_count(y.device))
@@ -156,7 +185,7 @@ class _FusedMLP(torch.autograd.Function):
     """branch = fc2(GELU(fc1(y)))  WITHOUT the fc2 bias (folded into the next residual_ln), timm Mlp as called from Block.forward
     (dino_enc/vision_transformer.py:336-339).  The fc1 GEMM carries bias + GELU in its epilogue, the fc2 input-gradient GEMM carries
     GELU' and the fc1-bias gradient; the other GEMMs are library calls.  Same bits as F.linear + gelu_bias (the epilogues apply
-    the same device functions to the same rounded bf16 values)."""
+    the same device functions to the same rounded 16-bit values).  Operands, weights and outputs in y's dtype, bf16 or fp16."""
 
     @staticmethod
     def forward(ctx, y, W1, b1, W2):
@@ -166,13 +195,14 @@ class _FusedMLP(torch.autograd.Function):
         if not y2.is_contiguous():
             y2 = y2.contiguous()
         M = y2.shape[0]
-        W1b = W1.to(torch.bfloat16)
-        W2b = W2.to(torch.bfloat16)
+        dt = y.dtype
+        W1b = W1.to(dt)
+        W2b = W2.to(dt)
         b1f = b1.float()
-        pre = torch.empty(M, N, dtype=torch.bfloat16, device=y.device)
-        act = torch.empty(M, N, dtype=torch.bfloat16, device=y.device)
-        L = C.lib()
-        C.call("xq_vit_fc1_gelu_fwd", 1, L.xq_vit_fc1_gelu_fwd, C.ptr(y2), C.ptr(W1b), C.ptr(b1f), C.ptr(pre), C.ptr(act), M, N, K,
+        pre = torch.empty(M, N, dtype=dt, device=y.device)
+        act = torch.empty(M, N, dtype=dt, device=y.device)
+        name, fn = _entry("xq_vit_fc1_gelu_fwd", dt)
+        C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(b1f), C.ptr(pre), C.ptr(act), M, N, K,
                C.stream_ptr(y.device), nbytes=M * K * 2 + N * K * 2 + M * N * 4, nflops=2.0 * M * N * K)
         branch = act @ W2b.t()
         ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
@@ -186,16 +216,16 @@ class _FusedMLP(torch.autograd.Function):
         M, N = pre.shape
         Ko = W2b.shape[0]
         g2 = g.reshape(M, Ko)
-        if g2.dtype != torch.bfloat16:
-            g2 = g2.to(torch.bfloat16)
+        if g2.dtype != pre.dtype:
+            g2 = g2.to(pre.dtype)
         if not g2.is_contiguous():
             g2 = g2.contiguous()
         dW2 = (g2.t() @ act).float() if ctx.needs_input_grad[3] else None
         W2t = W2b.t().contiguous()                      # [hidden, out]: the K-major B operand of d_act = g W2
         dpre = torch.empty_like(pre)
         db1 = torch.empty(N, dtype=torch.float32, device=pre.device)
-        L = C.lib()
-        C.call("xq_vit_fc2_dgelu_bwd", 1, L.xq_vit_fc2_dgelu_bwd, C.ptr(g2), C.ptr(W2t), C.ptr(pre), C.ptr(b1f), C.ptr(dpre), C.ptr(db1),
+        name, fn = _entry("xq_vit_fc2_dgelu_bwd", pre.dtype)
+        C.call(name, 1, fn, C.ptr(g2), C.ptr(W2t), C.ptr(pre), C.ptr(b1f), C.ptr(dpre), C.ptr(db1),
                M, N, Ko, C.stream_ptr(pre.device), nbytes=M * Ko * 2 + N * Ko * 2 + M * N * 4, nflops=2.0 * M * N * Ko)
         dW1 = (dpre.t() @ y2).float() if ctx.needs_input_grad[1] else None
         dy = (dpre @ W1b).view(ctx.in_shape) if ctx.needs_input_grad[0] else None
@@ -203,7 +233,7 @@ class _FusedMLP(torch.autograd.Function):
 
 
 def _scaled_mm(a, b, s: float):
-    """bf16(s * (a @ b)): the scale applied to the fp32 accumulator, one rounding"""
+    """16-bit(s * (a @ b)) in a's dtype: the scale applied to the fp32 accumulator, one rounding"""
     return torch.addmm(a.new_zeros(()), a, b, beta=0, alpha=s)
 
 
@@ -217,7 +247,8 @@ def _pad_rank(t, dim: int, R: int):
 
 class _LoRAMLP(torch.autograd.Function):
     """branch = fc2(GELU(fc1(y))) WITHOUT the fc2 bias, fc1 / fc2 LoRA-wrapped (dino_enc/lora.py, lora_dropout inactive):
-    fc(x) = x W^T + b + s (x A^T) B^T.  With u = bf16(s1 y A1^T) and v = bf16(s2 g B2) (rank-r library GEMMs):
+    fc(x) = x W^T + b + s (x A^T) B^T.  With u = 16-bit(s1 y A1^T) and v = 16-bit(s2 g B2) (rank-r library GEMMs; every
+    16-bit tensor in y's dtype, bf16 or fp16):
       forward   pre = y W1^T + u B1^T, act = GELU(pre + b1)      xq_vit_fc1_lora_gelu_fwd (u B1^T: one more K stage)
                 branch = act W2^T + s2 (act A2^T) B2^T           library
       backward  d_pre = (g W2 + v A2) * GELU'(pre + b1), d_b1   xq_vit_fc2_lora_dgelu_bwd
@@ -234,15 +265,15 @@ class _LoRAMLP(torch.autograd.Function):
         M = y2.shape[0]
         r = A1.shape[0]
         R = -(-r // 8) * 8
-        bf = torch.bfloat16
+        bf = y.dtype
         W1b, W2b, b1f = W1.to(bf), W2.to(bf), b1.float()
         A1b, B1b = _pad_rank(A1.to(bf), 0, R), _pad_rank(B1.to(bf), 1, R)           # [R, K], [N, R]
         A2b, B2b = _pad_rank(A2.to(bf), 0, R), _pad_rank(B2.to(bf), 1, R)           # [R, N], [Ko, R]
         u = _scaled_mm(y2, A1b.t(), s1)
         pre = torch.empty(M, N, dtype=bf, device=y.device)
         act = torch.empty(M, N, dtype=bf, device=y.device)
-        L = C.lib()
-        C.call("xq_vit_fc1_lora_gelu_fwd", 1, L.xq_vit_fc1_lora_gelu_fwd, C.ptr(y2), C.ptr(W1b), C.ptr(u), C.ptr(B1b), C.ptr(b1f),
+        name, fn = _entry("xq_vit_fc1_lora_gelu_fwd", bf)
+        C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(u), C.ptr(B1b), C.ptr(b1f),
                C.ptr(pre), C.ptr(act), M, N, K, R, C.stream_ptr(y.device),
                nbytes=M * (K + R) * 2 + N * (K + R) * 2 + M * N * 4, nflops=2.0 * M * N * (K + R))
         h2 = _scaled_mm(act, A2b.t(), s2)
@@ -261,8 +292,8 @@ class _LoRAMLP(torch.autograd.Function):
         M, N = pre.shape
         Ko, R = W2b.shape[0], A1b.shape[0]
         g2 = g.reshape(M, Ko)
-        if g2.dtype != torch.bfloat16:
-            g2 = g2.to(torch.bfloat16)
+        if g2.dtype != pre.dtype:
+            g2 = g2.to(pre.dtype)
         if not g2.is_contiguous():
             g2 = g2.contiguous()
         v = _scaled_mm(g2, B2b, s2)                     # [M, R]
@@ -270,8 +301,8 @@ class _LoRAMLP(torch.autograd.Function):
         A2t = A2b.t().contiguous()                      # [hidden, R]: the K-major adapter of the rank stage v A2
         dpre = torch.empty_like(pre)
         db1 = torch.empty(N, dtype=torch.float32, device=pre.device)
-        L = C.lib()
-        C.call("xq_vit_fc2_lora_dgelu_bwd", 1, L.xq_vit_fc2_lora_dgelu_bwd, C.ptr(g2), C.ptr(W2t), C.ptr(v), C.ptr(A2t), C.ptr(pre),
+        name, fn = _entry("xq_vit_fc2_lora_dgelu_bwd", pre.dtype)
+        C.call(name, 1, fn, C.ptr(g2), C.ptr(W2t), C.ptr(v), C.ptr(A2t), C.ptr(pre),
                C.ptr(b1f), C.ptr(dpre), C.ptr(db1), M, N, Ko, R, C.stream_ptr(pre.device),
                nbytes=M * (Ko + R) * 2 + N * (Ko + R) * 2 + M * N * 4, nflops=2.0 * M * N * (Ko + R))
         t1 = _scaled_mm(dpre, B1b, s1)                  # [M, R] = s1 d_pre B1
@@ -323,21 +354,21 @@ ATTN_TC_ENABLED = [True]
 
 
 def attn_tc_ok(attn, y) -> bool:
-    """xq_vit_attn_fwd/bwd cover what the shipped configs run: bf16 CUDA tokens, head_dim 64, no qk_norm, no mask and
+    """xq_vit_attn_fwd/bwd (and their _f16 twins) cover what the shipped configs run: bf16 or fp16 CUDA tokens, head_dim 64, no qk_norm, no mask and
     an attention dropout of 0 where it applies (training)."""
     p = attn.attn_drop.p if attn.training else 0.0
-    return (ATTN_TC_ENABLED[0] and y.is_cuda and y.dtype == torch.bfloat16 and p == 0.0 and attn.head_dim == 64
+    return (ATTN_TC_ENABLED[0] and y.is_cuda and y.dtype in _HALF and p == 0.0 and attn.head_dim == 64
             and isinstance(_live(attn.q_norm), nn.Identity) and isinstance(_live(attn.k_norm), nn.Identity))
 
 
 def attn_tc_forward(qkv, num_heads: int):
-    """qkv bf16 [B,N,3*H*64] (packed projection, read in place) -> (out bf16 [B,N,H*64], lse2 fp32 [B,H,N])."""
+    """qkv bf16 or fp16 [B,N,3*H*64] (packed projection, read in place) -> (out [B,N,H*64] in qkv's dtype, lse2 fp32 [B,H,N])."""
     B, N, C3 = qkv.shape
     qkv = qkv.contiguous()
-    out = torch.empty(B, N, C3 // 3, dtype=torch.bfloat16, device=qkv.device)
+    out = torch.empty(B, N, C3 // 3, dtype=qkv.dtype, device=qkv.device)
     lse2 = torch.empty(B, num_heads, N, dtype=torch.float32, device=qkv.device)
-    L = _lib()
-    _call("xq_vit_attn_fwd", 1, L.xq_vit_attn_fwd, _ptr(qkv), _ptr(out), _ptr(lse2), B, N, num_heads, 64, 0.125,
+    name, fn = _entry("xq_vit_attn_fwd", qkv.dtype)
+    _call(name, 1, fn, _ptr(qkv), _ptr(out), _ptr(lse2), B, N, num_heads, 64, 0.125,
           _stream(qkv.device), nbytes=qkv.numel() * 2 + out.numel() * 2 + lse2.numel() * 4,
           nflops=4.0 * B * num_heads * N * N * 64)
     return out, lse2
@@ -347,12 +378,12 @@ _ATTN_WS = {}
 
 
 def attn_tc_backward(qkv, out, lse2, g, num_heads: int, want_bias_grad: bool = False):
-    """d(out) bf16 [B,N,H*64] -> d(qkv) bf16 [B,N,3*H*64] written directly in the packed layout
+    """d(out) [B,N,H*64] -> d(qkv) [B,N,3*H*64] in qkv's dtype (bf16 or fp16), written directly in the packed layout
     (+ its column sums = the qkv-bias gradient, fp32 [3*H*64], when asked for)."""
     B, N, C3 = qkv.shape
     g = g.contiguous()
-    if g.dtype != torch.bfloat16:
-        g = g.to(torch.bfloat16)
+    if g.dtype != qkv.dtype:
+        g = g.to(qkv.dtype)
     dqkv = torch.empty_like(qkv)
     db = torch.empty(C3, dtype=torch.float32, device=qkv.device) if want_bias_grad else None
     L = _lib()
@@ -362,7 +393,8 @@ def attn_tc_backward(qkv, out, lse2, g, num_heads: int, want_bias_grad: bool = F
     if ws is None or ws.numel() < nbytes:
         ws = torch.empty(nbytes, dtype=torch.uint8, device=qkv.device)
         _ATTN_WS[key] = ws
-    _call("xq_vit_attn_bwd", 3, L.xq_vit_attn_bwd, _ptr(qkv), _ptr(out), _ptr(g), _ptr(lse2), _ptr(dqkv), _ptr(db), B, N, num_heads,
+    name, fn = _entry("xq_vit_attn_bwd", qkv.dtype)
+    _call(name, 3, fn, _ptr(qkv), _ptr(out), _ptr(g), _ptr(lse2), _ptr(dqkv), _ptr(db), B, N, num_heads,
           64, 0.125, _ptr(ws), ws.numel(), _stream(qkv.device), nbytes=qkv.numel() * 4 + out.numel() * 4 + lse2.numel() * 4,
           nflops=10.0 * B * num_heads * N * N * 64)
     return (dqkv, db) if want_bias_grad else dqkv
@@ -371,15 +403,15 @@ def attn_tc_backward(qkv, out, lse2, g, num_heads: int, want_bias_grad: bool = F
 class _QKVAttention(torch.autograd.Function):
     """qkv = y W^T (+ b) ; attention(qkv)   (vision_transformer.py:175-191) as ONE autograd node on the wgmma kernels, so that
     the bias gradient is the column sum the attention backward already has in registers (no separate sum(0) pass over
-    d(qkv)).  y [B,N,C] bf16, W [3C,C] / b [3C] (or None) fp32 parameters; GEMMs are library calls in bf16 (autocast
-    semantics)."""
+    d(qkv)).  y [B,N,C] bf16 or fp16, W [3C,C] / b [3C] (or None) fp32 parameters; GEMMs are library calls in y's dtype
+    (autocast semantics)."""
 
     @staticmethod
     def forward(ctx, y, W, b, num_heads: int):
         B, N, C = y.shape
-        Wb = W.to(torch.bfloat16)
+        Wb = W.to(y.dtype)
         y2 = y.reshape(B * N, C)
-        qkv = (torch.addmm(b.to(torch.bfloat16), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * C)
+        qkv = (torch.addmm(b.to(y.dtype), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * C)
         out, lse2 = attn_tc_forward(qkv, num_heads)
         ctx.save_for_backward(y, Wb, qkv, out, lse2)
         ctx.heads = num_heads
@@ -410,7 +442,8 @@ def attention_forward(attn, y):
 
 class _PatchEmbed(torch.autograd.Function):
     """timm PatchEmbed (Conv2d(kernel = stride = p) -> flatten(2).transpose(1,2)) as im2col-permutation + ONE GEMM.
-    x fp32 [B,Cin,H,W] (no gradient), W [D,Cin,p,p] / b [D] fp32 parameters -> tokens bf16 [B, gh*gw, D]."""
+    x fp32 [B,Cin,H,W] (no gradient), W [D,Cin,p,p] / b [D] fp32 parameters -> tokens [B, gh*gw, D] in the autocast dtype
+    (bf16 or fp16)."""
 
     @staticmethod
     def forward(ctx, x, W, b):
@@ -418,13 +451,14 @@ class _PatchEmbed(torch.autograd.Function):
         D, p = W.shape[0], W.shape[2]
         x = x.contiguous()
         M, K = Bn * (H // p) * (Wd // p), Cin * p * p
-        patches = torch.empty(M, K, dtype=torch.bfloat16, device=x.device)
-        L = _lib()
-        _call("xq_vit_patchify", 1, L.xq_vit_patchify, _ptr(x), _ptr(patches), Bn, Cin, H, Wd, p, _stream(x.device),
+        dt = _op_dtype()
+        patches = torch.empty(M, K, dtype=dt, device=x.device)
+        name, fn = _entry("xq_vit_patchify", dt)
+        _call(name, 1, fn, _ptr(x), _ptr(patches), Bn, Cin, H, Wd, p, _stream(x.device),
               nbytes=x.numel() * 6)
-        Wb = W.reshape(D, K).to(torch.bfloat16)
+        Wb = W.reshape(D, K).to(dt)
         if b is not None:
-            y = torch.addmm(b.to(torch.bfloat16), patches, Wb.t())
+            y = torch.addmm(b.to(dt), patches, Wb.t())
         else:
             y = patches @ Wb.t()
         ctx.save_for_backward(patches)
@@ -437,8 +471,8 @@ class _PatchEmbed(torch.autograd.Function):
         (patches,) = ctx.saved_tensors
         D = ctx.wshape[0]
         g2 = g.reshape(-1, D)
-        if g2.dtype != torch.bfloat16:
-            g2 = g2.to(torch.bfloat16)
+        if g2.dtype != patches.dtype:
+            g2 = g2.to(patches.dtype)
         dW = (g2.t() @ patches).float().view(ctx.wshape) if ctx.needs_input_grad[1] else None
         db = g2.float().sum(0) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
         return None, dW, db
@@ -447,19 +481,22 @@ class _PatchEmbed(torch.autograd.Function):
 def patch_embed_ok(pe, x) -> bool:
     p = pe.patch_size[0]
     proj = _live(pe.proj)
-    return (x.is_cuda and x.dtype == torch.float32 and not x.requires_grad and torch.is_autocast_enabled()
-            and torch.get_autocast_dtype("cuda") == torch.bfloat16 and isinstance(_live(pe.norm), nn.Identity)
+    return (x.is_cuda and x.dtype == torch.float32 and not x.requires_grad and _autocast_half() is not None
+            and isinstance(_live(pe.norm), nn.Identity)
             and pe.patch_size[0] == pe.patch_size[1] and p % 4 == 0 and x.shape[2] % p == 0 and x.shape[3] % p == 0
             and tuple(proj.stride) == tuple(proj.kernel_size) and tuple(proj.padding) == (0, 0))
 
 
 def patch_embed(pe, x):
-    """PatchEmbed.forward on the fused path when it applies (bf16 autocast, fp32 CUDA image that needs no gradient,
+    """PatchEmbed.forward on the fused path when it applies (bf16 or fp16 autocast, fp32 CUDA image that needs no gradient,
     patch % 4 == 0, no norm); otherwise the module's own conv."""
     if patch_embed_ok(pe, x):
         proj = _live(pe.proj)
         return _PatchEmbed.apply(x, proj.weight, proj.bias)
     return pe(x)
+
+
+_ASSEMBLE_TYPE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}    # src_type of xq_vit_assemble_fwd/bwd
 
 
 class _Assemble(torch.autograd.Function):
@@ -468,14 +505,14 @@ class _Assemble(torch.autograd.Function):
     @staticmethod
     def forward(ctx, src, table, t0: int):
         src = src.contiguous()
-        if src.dtype not in (torch.bfloat16, torch.float32):
+        if src.dtype not in _ASSEMBLE_TYPE:
             src = src.float()
         table = table.float().contiguous()
         B, Ls, D = src.shape
         T = table.shape[-2]
         out = torch.empty(B, T, D, dtype=torch.float32, device=src.device)
         L = _lib()
-        _call("xq_vit_assemble_fwd", 1, L.xq_vit_assemble_fwd, _ptr(src), int(src.dtype == torch.bfloat16), _ptr(table), B, Ls, T,
+        _call("xq_vit_assemble_fwd", 1, L.xq_vit_assemble_fwd, _ptr(src), _ASSEMBLE_TYPE[src.dtype], _ptr(table), B, Ls, T,
               D, int(t0), _ptr(out), _stream(src.device), nbytes=out.numel() * 4 + src.numel() * src.element_size())
         ctx.cfg = (B, Ls, T, D, int(t0), src.dtype, tuple(table.shape))
         return out
@@ -490,7 +527,7 @@ class _Assemble(torch.autograd.Function):
         d_tab = torch.empty(tshape, dtype=torch.float32, device=g.device) if ctx.needs_input_grad[1] else None
         L = _lib()
         _call("xq_vit_assemble_bwd", 1, L.xq_vit_assemble_bwd, _ptr(g), B, Ls, T, D, t0, _ptr(d_src) if d_src is not None else None,
-              int(sdt == torch.bfloat16), _ptr(d_tab) if d_tab is not None else None, _stream(g.device),
+              _ASSEMBLE_TYPE[sdt], _ptr(d_tab) if d_tab is not None else None, _stream(g.device),
               nbytes=g.numel() * 4 + (d_src.numel() * d_src.element_size() if d_src is not None else 0))
         return d_src, d_tab, None
 
@@ -507,7 +544,7 @@ def assemble_tokens(owner, path_fn, src, t0: int):
     does not hold (a configuration not anticipated here) the module path is used from then on.  Active dropout on the
     sequence makes the assembly batch-dependent: module path."""
     ok = (ASSEMBLE_ENABLED[0] and src.is_cuda and src.dim() == 3 and src.shape[-1] % 4 == 0 and torch.is_autocast_enabled()
-          and src.dtype in (torch.bfloat16, torch.float32))
+          and src.dtype in _ASSEMBLE_TYPE)
     if ok and getattr(owner, "_assemble_ok", None) is None:
         with torch.no_grad():
             probe = torch.randn(2, src.shape[1], src.shape[2], device=src.device)
@@ -536,13 +573,13 @@ def _droppath_scale(mod, batch: int, device):
 
 
 def fused_path_ok(vit, x) -> bool:
-    return (x.is_cuda and torch.is_autocast_enabled() and torch.get_autocast_dtype("cuda") == torch.bfloat16
+    return (x.is_cuda and _autocast_half() is not None
             and vit.embed_dim in _SUPPORTED_D and isinstance(vit.norm_pre, nn.Identity))
 
 
 def run_blocks(vit, x, attn_mask=None):
-    """x: [B,S,D] token stream after pos-embed (fp32).  Returns norm(blocks(x)) as bf16 on the fused
-    path, or the plain module path result otherwise (fp32 parity runs, CPU)."""
+    """x: [B,S,D] token stream after pos-embed (fp32).  Returns norm(blocks(x)) in the autocast dtype (bf16 or fp16) on the
+    fused path, or the plain module path result otherwise (fp32 parity runs, CPU)."""
     if attn_mask is not None or not fused_path_ok(vit, x):
         x = x.to(torch.matmul(x.new_ones(8, 8), x.new_ones(8, 8)).dtype)   # dinov2.py:177-179
         x = vit.norm_pre(x)

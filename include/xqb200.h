@@ -209,6 +209,11 @@ int xq_usage_ema_dev(float *ema, const float *hit, int rows, int V, int64_t *rec
  *   (LayerNorm :301,316 ; LayerScale :280-292 ; DropPath ; residual add) and Mlp's GELU.
  * Residual stream fp32 [M,D], GEMM operands bf16 (what bf16 autocast gives the reference).
  * D in {384, 768, 1024}.  `branch`, `y`, `g_y`, `g_branch` are bf16 [M,D].
+ *
+ * fp16 autocast: every ViT entry point below that takes or returns 16-bit data has an `_f16` twin with the same argument
+ * list, the same checks and return codes, in which those tensors are fp16 instead of bf16 (the same kernel instantiated for
+ * the other element type).  fp32 -> fp16 roundings are round-to-nearest-even and give +-inf on overflow (no saturation),
+ * so a gradient scaler sees an overflow as inf / NaN.
  * ------------------------------------------------------------------------------------------ */
 /*   x_out = x + rowscale[row / rows_per_sample] * ls_gamma[d] * (branch + branch_bias[d])
  *           (branch may be NULL: x_out = x; branch_bias = bias of the GEMM that produced `branch`, folded here
@@ -218,6 +223,9 @@ int xq_usage_ema_dev(float *ema, const float *hit, int rows, int V, int64_t *rec
 int xq_vit_residual_ln_fwd(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
                            const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
                            int M, int D, float *x_out, void *y, float *mean, float *rstd, void *stream);
+int xq_vit_residual_ln_fwd_f16(const float *x, const void *branch, const float *branch_bias, const float *ls_gamma,
+                               const float *rowscale, int rows_per_sample, const float *ln_w, const float *ln_b, float eps,
+                               int M, int D, float *x_out, void *y, float *mean, float *rstd, void *stream);
 /* workspace of xq_vit_residual_ln_bwd on the current device; 0 when the device cannot be queried (the cause is in
  * xq_last_cuda_error()), and xq_vit_residual_ln_bwd refuses a workspace that small */
 size_t xq_vit_ln_bwd_workspace_bytes(int D);
@@ -228,23 +236,37 @@ int xq_vit_residual_ln_bwd(const float *g_xout, const void *g_y, const float *x_
                            const float *ls_gamma, const float *rowscale, int rows_per_sample, int M, int D, float *g_x,
                            void *g_branch, float *g_ln_w, float *g_ln_b, float *g_ls_gamma, float *g_branch_bias,
                            void *workspace, size_t workspace_bytes, void *stream);
+int xq_vit_residual_ln_bwd_f16(const float *g_xout, const void *g_y, const float *x_out, const float *mean,
+                               const float *rstd, const float *ln_w, const void *branch, const float *branch_bias,
+                               const float *ls_gamma, const float *rowscale, int rows_per_sample, int M, int D, float *g_x,
+                               void *g_branch, float *g_ln_w, float *g_ln_b, float *g_ls_gamma, float *g_branch_bias,
+                               void *workspace, size_t workspace_bytes, void *stream);
 /*   im2col of the patch embedding (timm PatchEmbed = Conv2d(kernel = stride = p), vision_transformer.py PatchEmbed.forward):
  *   x fp32 [B,Cin,H,W] -> patches bf16 [B*(H/p)*(W/p), Cin*p*p] (K index = (c*p + ky)*p + kx = the flattened conv
  *   weight), so that tokens = patches @ weight.view(D,-1)^T + bias is a plain GEMM.  p % 4 == 0, H % p == W % p == 0. */
 int xq_vit_patchify(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream);
+int xq_vit_patchify_f16(const float *x, void *patches, int B, int Cin, int H, int W, int p, void *stream);
 /*   token assembly of the ViT encoder / decoder input (dino_enc/dinov2.py:151-170, 318-336):
  *     out[b,t,:] = table[t,:] + (t0 <= t < t0+Ls ? src[b,t-t0,:] : 0)   out fp32 [B,T,D], table fp32 [T,D] (the batch-
- *   independent part: cls / mask / latent tokens + positional + level embeddings), src [B,Ls,D] fp32 or bf16.
+ *   independent part: cls / mask / latent tokens + positional + level embeddings), src [B,Ls,D] fp32, bf16 or fp16.
+ *   src_type: XQ_ASSEMBLE_FP32 (0), XQ_ASSEMBLE_BF16 (1; any other value but 2 reads as bf16, as before fp16 existed) or
+ *   XQ_ASSEMBLE_F16 (2).
  *   backward: d_src = g[:, t0:t0+Ls] in the source dtype (may be NULL), d_table = sum_b g (may be NULL); one read of g. */
-int xq_vit_assemble_fwd(const void *src, int src_is_bf16, const float *table, int B, int Ls, int T, int D, int t0, float *out,
+#define XQ_ASSEMBLE_FP32 0
+#define XQ_ASSEMBLE_BF16 1
+#define XQ_ASSEMBLE_F16 2
+int xq_vit_assemble_fwd(const void *src, int src_type, const float *table, int B, int Ls, int T, int D, int t0, float *out,
                         void *stream);
-int xq_vit_assemble_bwd(const float *g, int B, int Ls, int T, int D, int t0, void *d_src, int src_is_bf16, float *d_table,
+int xq_vit_assemble_bwd(const float *g, int B, int Ls, int T, int D, int t0, void *d_src, int src_type, float *d_table,
                         void *stream);
 /*   y = GELU(x + bias) exact-erf form (timm Mlp act_layer=nn.GELU), x / y bf16 [M,C], bias fp32 [C] or NULL,
  *   C % 8 == 0.  Backward also returns g_bias [C] = column sums of gx (may be NULL). */
 int xq_vit_gelu_fwd(const void *x, const float *bias, void *y, int M, int C, void *stream);
 int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C,
                     void *stream);
+int xq_vit_gelu_fwd_f16(const void *x, const float *bias, void *y, int M, int C, void *stream);
+int xq_vit_gelu_bwd_f16(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C,
+                        void *stream);
 
 /*   Flash attention of the ViT blocks, head_dim 64, no mask, no dropout (Attention.forward,
  *   tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197: F.scaled_dot_product_attention on
@@ -254,6 +276,7 @@ int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, 
  *     lse2  fp32 [B,H,N]       base-2 log-sum-exp of the scaled scores (scale*log2(e)*q.k), saved for backward
  *   scale = head_dim^-0.5 (Attention.scale).  Any N >= 1; qkv / out 16-byte aligned. */
 int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream);
+int xq_vit_attn_fwd_f16(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream);
 
 /*   Backward of xq_vit_attn_fwd: d_out bf16 [B,N,H*64] -> dqkv bf16 [B,N,3,H,64] (the gradient of the packed projection,
  *   written in place of autograd's three permuted tensors + stack).  `out` and `lse2` are the forward's results.
@@ -263,6 +286,10 @@ int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
 size_t xq_vit_attn_bwd_workspace_bytes(int B, int N, int H);
 int xq_vit_attn_bwd(const void *qkv, const void *out, const void *d_out, const float *lse2, void *dqkv, float *g_bias, int B, int N,
                     int H, int head_dim, float scale, void *workspace, size_t workspace_bytes, void *stream);
+/*   fp16 twins: qkv / out / d_out / dqkv fp16; P and dS are rounded to fp16 as the operands of their MMAs (scores and the
+ *   dQ accumulator stay fp32).  The workspace is the same as the bf16 call's. */
+int xq_vit_attn_bwd_f16(const void *qkv, const void *out, const void *d_out, const float *lse2, void *dqkv, float *g_bias, int B,
+                        int N, int H, int head_dim, float scale, void *workspace, size_t workspace_bytes, void *stream);
 
 /*
  * ---- loss stack (SURVEY.md section 8 row f-1) -------------------------------------------------------------------
@@ -321,6 +348,15 @@ int xq_vit_fc1_lora_gelu_fwd(const void *x, const void *w, const void *u, const 
                              int M, int N, int K, int R, void *stream);
 int xq_vit_fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre, const float *bias,
                               void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream);
+/* fp16 twins of the four calls above: every 16-bit matrix is fp16 (fp16 autocast), everything else as above. */
+int xq_vit_fc1_gelu_fwd_f16(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K,
+                            void *stream);
+int xq_vit_fc2_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
+                             int M, int N, int K, void *stream);
+int xq_vit_fc1_lora_gelu_fwd_f16(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre,
+                                 void *act, int M, int N, int K, int R, void *stream);
+int xq_vit_fc2_lora_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre,
+                                  const float *bias, void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream);
 
 /* ---- input pipeline: the training / validation image transforms (SURVEY.md section 8 row f-4, csrc/img_kernels.cu) ---------
  * Replaces the per-image CPU transform of the reference's DataLoader workers:
