@@ -179,94 +179,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, typename E::T *__rest
     }
 }
 
-// The last (N mod 128) query rows when they are few (AT_TAIL_MAX): one warp per (batch*head, row) on the CUDA cores --
-// a 1-row tile would cost a full 128-row MMA tile in attn_fwd_kernel (S = 513: 20 % of its work).  Lanes split the keys,
-// each with its own online softmax, merged by shuffles at the end.  Same outputs as the tile kernel (out row, lse2).
-constexpr int AT_TAIL_MAX = 0;     // 0: ragged query tiles always run on the tile kernel (dead warps skip the softmax math)
-
-template <typename E>
-__global__ void __launch_bounds__(128)
-attn_fwd_tail_kernel(const typename E::T *__restrict__ qkv, typename E::T *__restrict__ out, float *__restrict__ lse2, int B, int N,
-                     int H, int n0 /* first tail row */, float c) {
-    const int lane = threadIdx.x & 31;
-    const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int nt = N - n0;
-    if (w >= (long long)B * H * nt) return;
-    const int r = (int)(w % nt);
-    const int bh = (int)(w / nt);
-    const int b = bh / H, h = bh - b * H;
-    const int n = n0 + r;
-    const size_t W = (size_t)3 * H * AT_D;
-    const typename E::T *qp = qkv + ((size_t)b * N + n) * W + h * AT_D;
-    float qf[AT_D];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-        const uint4 x = *reinterpret_cast<const uint4 *>(qp + u * 8);
-        const typename E::T2 *x2 = reinterpret_cast<const typename E::T2 *>(&x);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const float2 f = E::to2(x2[e]);
-            qf[u * 8 + 2 * e] = f.x * c;             // scores directly in the log2 domain
-            qf[u * 8 + 2 * e + 1] = f.y * c;
-        }
-    }
-    float m = -CUDART_INF_F, l = 0.f, o[AT_D];
-#pragma unroll
-    for (int i = 0; i < AT_D; ++i) o[i] = 0.f;
-    for (int key = lane; key < N; key += 32) {
-        const typename E::T *kp = qkv + ((size_t)b * N + key) * W + (H + h) * AT_D;
-        const typename E::T *vp = kp + (size_t)H * AT_D;
-        float s = 0.f;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            const uint4 x = *reinterpret_cast<const uint4 *>(kp + u * 8);
-            const typename E::T2 *x2 = reinterpret_cast<const typename E::T2 *>(&x);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = E::to2(x2[e]);
-                s = fmaf(qf[u * 8 + 2 * e], f.x, s);
-                s = fmaf(qf[u * 8 + 2 * e + 1], f.y, s);
-            }
-        }
-        const float m_new = fmaxf(m, s);
-        const float corr = ex2_approx(m - m_new);      // first key: ex2(-inf) = 0
-        const float p = ex2_approx(s - m_new);
-        l = fmaf(l, corr, p);
-        m = m_new;
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            const uint4 x = *reinterpret_cast<const uint4 *>(vp + u * 8);
-            const typename E::T2 *x2 = reinterpret_cast<const typename E::T2 *>(&x);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = E::to2(x2[e]);
-                o[u * 8 + 2 * e] = fmaf(o[u * 8 + 2 * e], corr, p * f.x);
-                o[u * 8 + 2 * e + 1] = fmaf(o[u * 8 + 2 * e + 1], corr, p * f.y);
-            }
-        }
-    }
-    float M = m;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) M = fmaxf(M, __shfl_xor_sync(0xffffffffu, M, off));
-    const float f = (m == -CUDART_INF_F) ? 0.f : ex2_approx(m - M);     // lanes without keys (N < 32) contribute nothing
-    l *= f;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) l += __shfl_xor_sync(0xffffffffu, l, off);
-    const float inv = 1.0f / l;
-    float mine0 = 0.f, mine1 = 0.f;
-#pragma unroll
-    for (int i = 0; i < AT_D; ++i) {
-        float x = o[i] * f;
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xffffffffu, x, off);
-        if (i == 2 * lane) mine0 = x;
-        if (i == 2 * lane + 1) mine1 = x;
-    }
-    typename E::T *op = out + ((size_t)b * N + n) * H * AT_D + h * AT_D;
-    *reinterpret_cast<uint32_t *>(op + 2 * lane) = E::pack(mine0 * inv, mine1 * inv);
-    if (lane == 0) lse2[(size_t)bh * N + n] = M + log2f(l);
-}
-
 // =====================================================================================================================
 // Backward.  One CTA per (batch, head, 128-key block), 288 threads: warpgroup wg owns keys 64 wg .. 64 wg + 63 of the block,
 // warp 8 is the TMA producer.  The CTA loops over the 64-query blocks i (Q_i, dO_i and the statistics through an AB_QS-stage
@@ -796,9 +708,7 @@ static int attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
     const uint64_t W = (uint64_t)3 * H * AT_D;
     CUtensorMap tmQKV;
     if (!tensor_map_16_3d(&tmQKV, E::TMAP, qkv, W, N, B, W * 2, (uint64_t)N * W * 2, AT_BM)) return XQ_ERR_UNSUPPORTED;
-    // query tiles: full 128-row tiles on the tensor cores; a short remainder (<= AT_TAIL_MAX rows) on the CUDA cores
-    const int n_tail = (N % AT_BM != 0 && N % AT_BM <= AT_TAIL_MAX && N > AT_BM) ? N % AT_BM : 0;
-    const int nQ = n_tail ? N / AT_BM : (N + AT_BM - 1) / AT_BM;
+    const int nQ = (N + AT_BM - 1) / AT_BM;       // query tiles; the last one may be ragged (its rows beyond N are not stored)
     const size_t smem = AttnFwdSmem::BYTES + 1024;
     if (int rc = smem_optin(attn_fwd_kernel<E>, smem)) return rc;
     const long long tiles = (long long)B * H * nQ;
@@ -806,12 +716,6 @@ static int attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
     const float c = scale * 1.4426950408889634f;
     attn_fwd_kernel<E><<<(unsigned)tiles, AT_THREADS, smem, (cudaStream_t)stream>>>(tmQKV, (T *)out, lse2, N, H, nQ, c);
     XQ_LAUNCH_CHECK("attn_fwd_kernel");
-    if (n_tail) {
-        const long long warps = (long long)B * H * n_tail;
-        attn_fwd_tail_kernel<E><<<(unsigned)((warps + 3) / 4), 128, 0, (cudaStream_t)stream>>>((const T *)qkv, (T *)out, lse2, B,
-                                                                                                 N, H, N - n_tail, c);
-        XQ_LAUNCH_CHECK("attn_fwd_tail_kernel");
-    }
     return XQ_OK;
 }
 

@@ -158,12 +158,16 @@ def test_lora_f16_rank_stage_equals_plain_kernel_on_concatenated_operands(R):
 
     pre, act, pre2, act2 = (_nan((M, N), H16) for _ in range(4))
     _capi.check(L.xq_vit_fc1_lora_gelu_fwd_f16(p(x), p(w), p(u), p(bl), p(b1), p(pre), p(act), M, N, K, R, s), "lora fwd")
-    _capi.check(L.xq_vit_fc1_gelu_fwd_f16(p(cat(x, u)), p(cat(w, bl)), p(b1), p(pre2), p(act2), M, N, K + 64, s), "fwd")
+    # the concatenated operands are held by name until the kernels have run: a temporary would go back to the caching
+    # allocator as soon as its pointer is taken, and the next one could be built in the same memory before the launch
+    xu, wb = cat(x, u), cat(w, bl)
+    _capi.check(L.xq_vit_fc1_gelu_fwd_f16(p(xu), p(wb), p(b1), p(pre2), p(act2), M, N, K + 64, s), "fwd")
     _assert_bits(pre, pre2, "pre", zero_sign=True)
     _assert_bits(act, act2, "act", zero_sign=True)
     dp, db, dp2, db2 = _nan((M, N), H16), _nan((N,)), _nan((M, N), H16), _nan((N,))
     _capi.check(L.xq_vit_fc2_lora_dgelu_bwd_f16(p(g), p(w2t), p(v), p(a2t), p(pre), p(b1), p(dp), p(db), M, N, K, R, s), "bwd")
-    _capi.check(L.xq_vit_fc2_dgelu_bwd_f16(p(cat(g, v)), p(cat(w2t, a2t)), p(pre), p(b1), p(dp2), p(db2), M, N, K + 64, s), "b")
+    gv, wa = cat(g, v), cat(w2t, a2t)
+    _capi.check(L.xq_vit_fc2_dgelu_bwd_f16(p(gv), p(wa), p(pre), p(b1), p(dp2), p(db2), M, N, K + 64, s), "b")
     _assert_bits(dp, dp2, "d_pre", zero_sign=True)
     pos = b1 == SAT
     assert torch.equal(db[pos], db2[pos])
