@@ -92,8 +92,18 @@ def _depth(sd, prefix):
     return 1 + max(int(k[len(prefix) + 8:].split(".")[0]) for k in sd if k.startswith(prefix + ".blocks."))
 
 
+def _blocks(t, sd, prefix, num_heads, keep):
+    """the transformer blocks; keep[i] = None or the (attention, MLP) DropPath multipliers of block i, each [B] or None"""
+    for i in range(_depth(sd, prefix)):
+        k = keep[i] if keep is not None else None
+        if k is not None:
+            k = [torch.ones((), dtype=t.dtype, device=t.device) if m is None else m.to(t).view(-1, 1, 1) for m in k]
+        t = _block(t, sd, f"{prefix}.blocks.{i}", num_heads, k)
+    return t
+
+
 def encoder_forward(sd: Dict[str, torch.Tensor], x, num_heads: int, num_latent: int, product_quant: int,
-                    prefix="encoder", patch=16):
+                    prefix="encoder", patch=16, keep=None):
     w, b = sd[prefix + ".model.patch_embed.proj.weight"], sd[prefix + ".model.patch_embed.proj.bias"]
     t = F.conv2d(x, w, b, stride=patch).flatten(2).transpose(1, 2)
     t = _pos_embed(t, sd, prefix + ".model")
@@ -107,13 +117,12 @@ def encoder_forward(sd: Dict[str, torch.Tensor], x, num_heads: int, num_latent: 
         t = t + sd[prefix + ".lvl_embed.weight"][sd[prefix + ".lvl1LC"].long()].expand(t.shape[0], -1, -1)
     else:                                           # learned latent positions (dinov2.py:170-171)
         t = torch.cat([t, z + sd[prefix + ".latent_pos_embed"]], dim=1)
-    for i in range(_depth(sd, prefix + ".model")):
-        t = _block(t, sd, f"{prefix}.model.blocks.{i}", num_heads)
+    t = _blocks(t, sd, prefix + ".model", num_heads, keep)
     t = _ln(t, sd, prefix + ".model.norm")
     return t[:, -num_latent:]
 
 
-def decoder_forward(sd, z, num_heads: int, num_latent: int, num_img_tokens=256, prefix="decoder", patch=16):
+def decoder_forward(sd, z, num_heads: int, num_latent: int, num_img_tokens=256, prefix="decoder", patch=16, keep=None):
     B = z.shape[0]
     x = sd[prefix + ".mask_token"].expand(B, num_img_tokens, -1)
     x = _pos_embed(x, sd, prefix + ".model")
@@ -124,8 +133,7 @@ def decoder_forward(sd, z, num_heads: int, num_latent: int, num_img_tokens=256, 
         t = t + sd[prefix + ".lvl_embed.weight"][sd[prefix + ".lvl1LC"].long()].expand(B, -1, -1)
     else:                                           # dinov2.py:332-333
         t = torch.cat([x, z + sd[prefix + ".latent_pos_embed"]], dim=1)
-    for i in range(_depth(sd, prefix + ".model")):
-        t = _block(t, sd, f"{prefix}.model.blocks.{i}", num_heads)
+    t = _blocks(t, sd, prefix + ".model", num_heads, keep)
     t = _ln(t, sd, prefix + ".model.norm")
     t = t[:, 1:1 + num_img_tokens]
     t = F.linear(t, sd[prefix + ".to_pixel.model.weight"], sd[prefix + ".to_pixel.model.bias"])
@@ -194,18 +202,21 @@ class _LFQ(torch.autograd.Function):
 # the whole path
 # ----------------------------------------------------------------------------------------------
 class RefTokenizer:
-    """encode -> quantize -> decode on CPU from a VQModel state_dict (fp32).
+    """encode -> quantize -> decode from a VQModel state_dict, in fp32 on the CPU unless `dtype` / `device` say otherwise
+    (fp64 on a GPU is what the gradient tests use).  The quantizer stage always runs the fp32 C/numpy oracle on the CPU.
 
     cfg keys: codebook_size, codebook_embed_dim, product_quant, v_patch_nums, num_latent_tokens (per branch),
     lfq, num_heads, codebook_drop, beta, entropy_weight, codebook_l2_norm
+    `keep` (encode / decode / forward): per-block DropPath multipliers of that ViT, see `_blocks`.
     """
 
-    def __init__(self, state_dict: Dict[str, torch.Tensor], cfg: Dict, requires_grad: bool = False):
+    def __init__(self, state_dict: Dict[str, torch.Tensor], cfg: Dict, requires_grad: bool = False,
+                 dtype: torch.dtype = torch.float32, device="cpu"):
         self.cfg = dict(cfg)
         self.sd = {}
         for k, v in state_dict.items():
-            v = v.detach().to("cpu")
-            v = v.float().clone() if v.is_floating_point() else v.clone()
+            v = v.detach().to(device)
+            v = v.to(dtype).clone() if v.is_floating_point() else v.clone()
             if requires_grad and v.is_floating_point() and "ema_vocab_hit" not in k and "scaler" not in k:
                 v.requires_grad_(True)
             self.sd[k] = v
@@ -216,10 +227,10 @@ class RefTokenizer:
     def _qprefix(self, i):
         return f"quantizes.{i}" if self.cfg["product_quant"] > 1 else "quantize"
 
-    def encode(self, x):
+    def encode(self, x, keep=None):
         c = self.cfg
         PQ = c["product_quant"]
-        h = encoder_forward(self.sd, x, c["num_heads"], c["num_latent_tokens"] * PQ, PQ)
+        h = encoder_forward(self.sd, x, c["num_heads"], c["num_latent_tokens"] * PQ, PQ, keep=keep)
         b, l, d = h.shape
         if PQ > 1:
             h = h.reshape(b, l, 1, d).permute(0, 3, 1, 2)
@@ -243,41 +254,42 @@ class RefTokenizer:
         return w, b
 
     def quantize(self, h, dropout=None):
-        """-> quant [B, PQ*C, s, s], (vq, commit, entropy)"""
+        """-> quant [B, PQ*C, s, s], (vq, commit, entropy) in h's dtype and device"""
         c = self.cfg
         pn = list(c["v_patch_nums"])
+        o = lambda t: t.float().cpu()           # the oracle's operands: fp32 on the CPU (no-ops for the fp32 CPU tokenizer)
         outs, vqs, cms, ens = [], [], [], []
         for i, hi in enumerate(self._branches(h)):
             q = self._qprefix(i)
-            hi = hi.contiguous()
+            hi = o(hi.contiguous())
             if len(pn) == 1:
-                out, vq, cm, _ = _VQ.apply(hi, self.sd[q + ".embedding.weight"], c.get("beta", 0.25),
+                out, vq, cm, _ = _VQ.apply(hi, o(self.sd[q + ".embedding.weight"]), c.get("beta", 0.25),
                                            c.get("codebook_l2_norm", True))
                 en = torch.zeros(())
             elif not c.get("lfq", False):
                 w, b = self._phi(q)
-                out, vq, cm = _VQ2.apply(hi, self.sd[q + ".embedding.weight"], w, b, pn, True, c.get("beta", 0.25),
-                                         c.get("codebook_drop", 0.0), dropout)
+                out, vq, cm = _VQ2.apply(hi, o(self.sd[q + ".embedding.weight"]), o(w), o(b), pn, True,
+                                         c.get("beta", 0.25), c.get("codebook_drop", 0.0), dropout)
                 en = torch.zeros(())
             else:
                 w, b = self._phi(q)
-                out, vq, cm, en = _LFQ.apply(hi, w, b, pn, c.get("codebook_l2_norm", True), c.get("beta", 0.25),
-                                             c.get("codebook_drop", 0.0), dropout, self.sd[q + ".scaler"].numpy(),
+                out, vq, cm, en = _LFQ.apply(hi, o(w), o(b), pn, c.get("codebook_l2_norm", True), c.get("beta", 0.25),
+                                             c.get("codebook_drop", 0.0), dropout, o(self.sd[q + ".scaler"]).numpy(),
                                              c.get("entropy_weight", 0.0))
-            outs.append(out), vqs.append(vq), cms.append(cm), ens.append(en)
+            outs.append(out.to(h)), vqs.append(vq.to(h)), cms.append(cm.to(h)), ens.append(en.to(h))
         n = len(outs)
         return torch.cat(outs, dim=1), (sum(vqs) / n, sum(cms) / n, sum(ens) / n)
 
-    def decode(self, quant):
+    def decode(self, quant, keep=None):
         c = self.cfg
         t = F.conv2d(quant, self.sd["post_quant_conv.weight"], self.sd["post_quant_conv.bias"])
         t = t.flatten(2).permute(0, 2, 1)
-        return decoder_forward(self.sd, t, c["num_heads"], c["num_latent_tokens"])
+        return decoder_forward(self.sd, t, c["num_heads"], c["num_latent_tokens"], keep=keep)
 
-    def forward(self, x, dropout=None):
-        h = self.encode(x)
+    def forward(self, x, dropout=None, enc_keep=None, dec_keep=None):
+        h = self.encode(x, enc_keep)
         quant, losses = self.quantize(h, dropout)
-        return self.decode(quant), losses, h
+        return self.decode(quant, dec_keep), losses, h
 
     def train_step(self, x, opt, dropout=None):
         """the in-scope generator step: fwd + bwd of (MSE rec + vq + commit + entropy) + optimizer."""

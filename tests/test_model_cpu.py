@@ -129,3 +129,61 @@ def test_cnn_encoder_decoder_match_reference_golden():
     with torch.no_grad():
         np.testing.assert_allclose(enc(torch.tensor(g["x"])).numpy(), g["h"], rtol=1e-4, atol=1e-5)
         np.testing.assert_allclose(dec(torch.tensor(g["z"])).numpy(), g["y"], rtol=1e-4, atol=1e-5)
+
+
+def _droppath_masks(vit, batch, gen):
+    """per block, the (attention, MLP) DropPath multipliers [B] the test imposes: keep / keep_prob or 0, at least one 0 in
+    each ViT; None for a branch without DropPath (block 0: drop_path_rate is linear from 0)"""
+    keep = []
+    for blk in vit.blocks:
+        pair = []
+        for dp in (blk.drop_path1, blk.drop_path2):
+            p = getattr(dp, "drop_prob", 0.0)
+            if p == 0.0:
+                pair.append(None)
+                continue
+            k = (torch.rand(batch, generator=gen) >= 0.5).double()
+            k[len(pair) % batch] = 0.0
+            pair.append(k / (1.0 - p))
+        keep.append(pair)
+    return keep
+
+
+def _impose_masks(vit, keep):
+    for blk, pair in zip(vit.blocks, keep):
+        for dp, k in zip((blk.drop_path1, blk.drop_path2), pair):
+            if k is not None:
+                dp.forward = lambda x, k=k: x * k.to(x.dtype).view(-1, *([1] * (x.dim() - 1)))
+
+
+@pytest.mark.parametrize("name", ["VQ-8192", "MSVR10P2-4096"])
+def test_fp64_reference_droppath_matches_module_path_in_train_mode(name):
+    """the fp64 RefTokenizer with per-block DropPath multipliers equals the product's fp32 module path in train mode with
+    its DropPath modules forced to the same multipliers; LayerScale gammas random in [0.25, 1] so that a dropped branch
+    changes the output"""
+    model, args = small_model(name)
+    model.train()
+    gen = torch.Generator().manual_seed(11)
+    with torch.no_grad():
+        for vit in (model.encoder.model, model.decoder.model):
+            for blk in vit.blocks:
+                blk.ls1.gamma.copy_(0.25 + 0.75 * torch.rand(blk.ls1.gamma.shape, generator=gen))
+                blk.ls2.gamma.copy_(0.25 + 0.75 * torch.rand(blk.ls2.gamma.shape, generator=gen))
+    enc_keep = _droppath_masks(model.encoder.model, 2, gen)
+    dec_keep = _droppath_masks(model.decoder.model, 2, gen)
+    _impose_masks(model.encoder.model, enc_keep)
+    _impose_masks(model.decoder.model, dec_keep)
+    cfg = vit_ref.cfg_from_model_args(model.config, num_heads=6)
+    ref = vit_ref.RefTokenizer(model.state_dict(), cfg, dtype=torch.float64)
+    x = torch.rand(2, 3, 256, 256, generator=gen) * 2 - 1
+    s = int(np.sqrt(model.config.num_latent_tokens // model.product_quant))
+    q = torch.randn(2, model.Cvae, s, s, generator=gen)
+    with torch.no_grad():
+        h, h_ref = model.encode(x), ref.encode(x.double(), enc_keep)
+        d, d_ref = model.decode(q), ref.decode(q.double(), dec_keep)
+        assert h_ref.dtype == d_ref.dtype == torch.float64
+        np.testing.assert_allclose(h.double().numpy(), h_ref.numpy(), rtol=1e-5, atol=1e-5 * float(h_ref.abs().max()))
+        np.testing.assert_allclose(d.double().numpy(), d_ref.numpy(), rtol=1e-5, atol=1e-5 * float(d_ref.abs().max()))
+        # the multipliers matter: without them the reference is far from the module path
+        assert float((ref.encode(x.double()) - h_ref).abs().max()) > 1e-2 * float(h_ref.abs().max())
+        assert float((ref.decode(q.double()) - d_ref).abs().max()) > 1e-2 * float(d_ref.abs().max())
