@@ -11,9 +11,15 @@
 //               canonical fp32 arithmetic (fmaf chain, d = (zz+ee) - 2 dot, first index on ties) -> the index
 //               equals the exact kernel's and the oracle's: the true argmin provably lies in a kept group.
 //
-// Error bound (codebook_norm=1, |z| = |c| = 1 up to 1e-6): TF32 operands carry <= 2^-10 relative error
-// each, so |dot_tf32 - dot| <= 2^-9 * sum|z_k c_k| <= 1.96e-3.  We use eps = 2.5e-3 and keep every code with
+// Error bound (codebook_norm=1): the screening score is the dot alone, which ranks codes like the canonical key
+// d = (zz + ee) - 2 dot only while every code has ee = |c|^2 = 1.  F.normalize leaves a codebook row of norm < XQ_EPS
+// shorter than 1 (a zero row at 0), so the prep kernel raises a flag when any real code has |ee - 1| > 1e-5, and then
+// EVERY row of the search takes the full canonical scan (degenerate codebooks only; the score tile is not touched).
+// Otherwise |z| <= 1, |c| = 1 up to 1e-5: TF32 operands carry <= 2^-10 relative error each, so
+// |dot_tf32 - dot| <= 2^-9 * sum|z_k c_k| <= 1.96e-3, and the ee spread moves a code's key by at most 1e-5 relative to
+// its score.  We use eps = 2.5e-3, whose margin over 1.96e-3 covers that spread, and keep every code with
 // score >= running_max - (2 eps + 2e-6)  (the 2e-6 covers the fp32 rounding of zz + ee in the canonical key).
+// Padded codes score 0; the last tile masks them.
 //
 // Roles (416 threads): warpgroups 0-1 = MMA (rows 64 wg .. 64 wg + 63), warpgroup 2 = epilogue (thread = row),
 // warp 12 = TMA producer.  Pipelines: full/empty mbarriers per smem stage (TMA <-> MMA), s_full/s_empty for the score
@@ -88,9 +94,9 @@ static size_t tc_smem_bytes(int C, int nstage) {
 template <int KC>   // 128-byte K chunks: C / 32
 __global__ void __launch_bounds__(TC_THREADS, 1)
 vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__restrict__ z, const float *__restrict__ E,
-                    const float *__restrict__ En, const float *__restrict__ ee, int N, int C, int HW, int V, int Vpad,
-                    int nstage, int ste_value, int64_t *__restrict__ idx_out, float *__restrict__ out,
-                    float *__restrict__ partial, float *__restrict__ hist) {
+                    const float *__restrict__ En, const float *__restrict__ ee, const int *__restrict__ ee_off_unit,
+                    int N, int C, int HW, int V, int Vpad, int nstage, int ste_value, int64_t *__restrict__ idx_out,
+                    float *__restrict__ out, float *__restrict__ partial, float *__restrict__ hist) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     TcSmem s;
@@ -201,7 +207,7 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
         const int q = warp & 3;
         const int row = q * 32 + lane;
         float runmax = -CUDART_INF_F, thr = -CUDART_INF_F;
-        int cnt = 0, overflow = 0;
+        int cnt = 0, overflow = *ee_off_unit;    // a code with ee != 1: the scores do not rank the key -> full scan
         float *cs = s.cand_s + row * TC_CAP;
         float *cs2 = s.cand_s2 + row * TC_CAP;
         int *cv = s.cand_v + row * TC_CAP;
@@ -340,9 +346,10 @@ vq_search_tc_kernel(const __grid_constant__ CUtensorMap tmB, const float *__rest
     if (tid == 0 && partial) partial[blockIdx.x] = sq;
 }
 
-// row-major normalised codebook En[Vpad][C] (+ ee[Vpad]); padded rows are zero
+// row-major normalised codebook En[Vpad][C] (+ ee[Vpad]); padded rows are zero.  *ee_off_unit (zeroed by the host)
+// is set when a real code has |ee - 1| > 1e-5 (a zero row, or one of norm < XQ_EPS)
 __global__ void codebook_prep_rowmajor_kernel(const float *__restrict__ E, int V, int C, int Vpad, float *__restrict__ En,
-                                              float *__restrict__ ee) {
+                                              float *__restrict__ ee, int *__restrict__ ee_off_unit) {
     int v = blockIdx.x * blockDim.x + threadIdx.x;
     if (v >= Vpad) return;
     if (v >= V) {
@@ -361,12 +368,14 @@ __global__ void codebook_prep_rowmajor_kernel(const float *__restrict__ E, int V
         s2 = fmaf(x, x, s2);
     }
     ee[v] = s2;
+    if (!(fabsf(s2 - 1.f) <= 1e-5f)) *ee_off_unit = 1;
 }
 
 size_t vq_tc_workspace_bytes(int B, int C, int HW, int V) {
     size_t Vp = ((size_t)V + TC_BN - 1) / TC_BN * TC_BN;
     size_t ctas = ((size_t)B * HW + TC_BM - 1) / TC_BM;
-    return align_up(sizeof(float) * Vp * C, 1024) + align_up(sizeof(float) * Vp, 256) + align_up(sizeof(float) * ctas, 256);
+    return align_up(sizeof(float) * Vp * C, 1024) + align_up(sizeof(float) * Vp, 256) + align_up(sizeof(float) * ctas, 256) +
+           256;                                                                                     // ee_off_unit
 }
 
 bool vq_tc_supported(int C, int V, int codebook_norm) {
@@ -387,6 +396,8 @@ int vq_tc_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     float *ee = (float *)ws;
     ws += align_up(sizeof(float) * (size_t)Vp, 256);
     float *partial = (float *)ws;
+    ws += align_up(sizeof(float) * (size_t)((N + TC_BM - 1) / TC_BM), 256);
+    int *ee_off_unit = (int *)ws;
     const int nstage = (C == 32) ? 4 : 3;
     const size_t smem = tc_smem_bytes(C, nstage);
     if (smem > 227 * 1024) return XQ_ERR_UNSUPPORTED;
@@ -398,12 +409,13 @@ int vq_tc_forward(const float *z, const float *E, int B, int C, int HW, int V, i
     if (!xqtc::tensor_map(&tm, En, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
         return XQ_ERR_UNSUPPORTED;
 
-    codebook_prep_rowmajor_kernel<<<(Vp + 127) / 128, 128, 0, stream>>>(E, V, C, Vp, En, ee);
+    XQ_CUDA_TRY(cudaMemsetAsync(ee_off_unit, 0, sizeof(int), stream));
+    codebook_prep_rowmajor_kernel<<<(Vp + 127) / 128, 128, 0, stream>>>(E, V, C, Vp, En, ee, ee_off_unit);
     XQ_LAUNCH_CHECK("codebook_prep_rowmajor_kernel");
     const int ctas = (N + TC_BM - 1) / TC_BM;
     auto kern = C == 32 ? vq_search_tc_kernel<1> : vq_search_tc_kernel<2>;
     if (int rc = smem_optin(kern, smem)) return rc;
-    kern<<<ctas, TC_THREADS, smem, stream>>>(tm, z, E, En, ee, N, C, HW, V, Vp, nstage, ste_value, idx, out,
+    kern<<<ctas, TC_THREADS, smem, stream>>>(tm, z, E, En, ee, ee_off_unit, N, C, HW, V, Vp, nstage, ste_value, idx, out,
                                              loss ? partial : nullptr, hist);
     XQ_LAUNCH_CHECK("vq_search_tc_kernel");
     if (loss) return launch_finalize_mse(partial, ctas, 1.0 / ((double)N * (double)C), beta, loss, stream);
