@@ -1464,6 +1464,9 @@ int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const flo
     const int C = d->C, H = d->H, W = d->W, HW = H * W;
     size_t smem = sizeof(float) * ms_fwd_smem_floats(C, H, W, d->SN, !bsq);
     if (smem > 227 * 1024) return XQ_ERR_UNSUPPORTED;
+    // a training forward is followed by xq_ms_backward, whose CTA holds more per image than the forward's: refuse the
+    // shape here rather than let loss.backward() fail after the forward has run
+    if (with_losses && saved && sizeof(float) * ms_bwd_smem_floats(C, H, W) > 227 * 1024) return XQ_ERR_UNSUPPORTED;
     MsSaved sv = {nullptr, nullptr, nullptr, nullptr, nullptr};
     if (saved) sv = ms_saved_layout(d, saved);
 

@@ -153,9 +153,13 @@ class _MSForward(torch.autograd.Function):
         saved = C.workspace(L.xq_ms_saved_bytes(desc), dev)
         ws = C.workspace(L.xq_ms_workspace_bytes(desc), dev)
         nk = 2 + (1 if desc.channel_norm else 0) + (1 if E is not None else 1) + (1 if desc.mode == C.XQ_MS_BSQ_HARD else 0)
-        C.call("xq_ms_forward", nk, L.xq_ms_forward, desc, C.ptr(f), C.ptr(E), C.ptr(phi_w), C.ptr(phi_b), C.ptr(nq), 1,
-               C.ptr(out), C.ptr(idx_all), None, C.ptr(loss), C.ptr(hist), C.ptr(saved), C.ptr(ws), ws.numel(),
-               C.stream_ptr(dev))
+        try:
+            C.call("xq_ms_forward", nk, L.xq_ms_forward, desc, C.ptr(f), C.ptr(E), C.ptr(phi_w), C.ptr(phi_b), C.ptr(nq),
+                   1, C.ptr(out), C.ptr(idx_all), None, C.ptr(loss), C.ptr(hist), C.ptr(saved), C.ptr(ws), ws.numel(),
+                   C.stream_ptr(dev))
+        except C.XqError as e:
+            # most refusals are shape limits (one image's forward or backward working set in shared memory)
+            raise C.XqError(f"{e} (B = {desc.B}, C = {desc.C}, last scale {desc.H} x {desc.W})") from None
         ctx.desc = desc
         ctx.has = (E is not None, phi_w is not None)
         ctx.save_for_backward(f, E, phi_w, phi_b, nq, idx_all, saved)

@@ -150,6 +150,9 @@ int64_t xq_ms_total_tokens(const xq_ms_desc *d); /* sum_si B*pn^2 */
  *   loss         [3] {vq, commit, entropy}
  *   hist         [SN,V] += bincount per scale, or NULL
  *   saved        xq_ms_saved_bytes(): state the backward needs (final masked f_hat, ...)
+ * Refusals: XQ_ERR_UNSUPPORTED when one image's working set exceeds 227 KB of shared memory; with losses and `saved`
+ * (training), also when the backward's would (it needs more: e.g. C = 32 fits the forward up to a 16 x 16 last
+ * scale but the backward only up to 13 x 13), so that a forward never succeeds whose backward is refused.
  */
 int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const float *phi_w, const float *phi_b,
                   const float *n_quantizers, int with_losses, float *out, int64_t *idx_all, float *fhat_scales,
