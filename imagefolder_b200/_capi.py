@@ -94,8 +94,6 @@ def lib() -> ctypes.CDLL:
     L.xq_ms_decode.argtypes = [dp, i64p, f32p, f32p, f32p, f32p, f32p, f32p, vp]
     L.xq_ms_embed.restype = c_int
     L.xq_ms_embed.argtypes = [dp, c_int, c_int, f32p, f32p, f32p, f32p, f32p, f32p, f32p, vp]
-    L.xq_usage_ema.restype = c_int
-    L.xq_usage_ema.argtypes = [f32p, f32p, c_int, c_int, c_int, c_float, f32p, vp]
     L.xq_usage_ema_dev.restype = c_int
     L.xq_usage_ema_dev.argtypes = [f32p, f32p, c_int, c_int, i64p, c_float, f32p, vp]
     L.xq_vit_residual_ln_fwd.restype = c_int
@@ -241,7 +239,7 @@ EXPORTED_SYMBOLS = [
     "xq_strerror", "xq_abi_version", "xq_last_cuda_error", "xq_vq_workspace_bytes", "xq_vq_forward",
     "xq_vq_backward", "xq_perturb_workspace_bytes", "xq_perturb_forward", "xq_perturb_backward",
     "xq_ms_workspace_bytes", "xq_ms_saved_bytes", "xq_ms_total_tokens", "xq_ms_forward", "xq_ms_backward",
-    "xq_ms_decode", "xq_ms_embed", "xq_usage_ema", "xq_usage_ema_dev", "xq_vit_residual_ln_fwd", "xq_vit_ln_bwd_workspace_bytes",
+    "xq_ms_decode", "xq_ms_embed", "xq_usage_ema_dev", "xq_vit_residual_ln_fwd", "xq_vit_ln_bwd_workspace_bytes",
     "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd", "xq_vit_fc2_lora_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",

@@ -483,16 +483,16 @@ __global__ void perturb_backward_kernel(const float *__restrict__ z, const float
     }
 }
 
-// ema rows update + usage (xqgan_model.py:777-788, quant.py:121-127,137-141).  One CTA per row;
-// row i uses record_hit + i (the reference increments record_hit once per scale).
-// record_hit_dev (optional): the step counter lives on the device (a graph-capturable / torch.compile-friendly variant: the
-// host never reads or writes it); the last block to finish bumps it by the number of rows, like the reference's per-scale `+= 1`
-__global__ void usage_ema_kernel(float *__restrict__ ema, const float *__restrict__ hit, int V, int record_hit,
-                                 float margin, float *__restrict__ usage_out, long long *__restrict__ record_hit_dev,
+// ema rows update + usage (xqgan_model.py:777-788, quant.py:121-127,137-141).  One CTA per row; row i uses
+// record_hit_dev[0] + i (the reference increments record_hit once per scale).  The step counter lives on the device, so the host
+// never reads or writes it (the call stays graph-capturable and torch.compile-friendly); the last block to finish advances it
+// by the number of rows, like the reference's per-scale `+= 1`.
+__global__ void usage_ema_kernel(float *__restrict__ ema, const float *__restrict__ hit, int V, float margin,
+                                 float *__restrict__ usage_out, long long *__restrict__ record_hit_dev,
                                  unsigned int *__restrict__ done_counter) {
     __shared__ float red[32];
     const int row = blockIdx.x;
-    const int rh = (record_hit_dev ? (int)min(*record_hit_dev, 1000000LL) : record_hit) + row;
+    const int rh = (int)min(*record_hit_dev, 1000000LL) + row;
     float *e_row = ema + (size_t)row * V;
     const float *h_row = hit + (size_t)row * V;
     float cnt = 0.f;
@@ -506,7 +506,7 @@ __global__ void usage_ema_kernel(float *__restrict__ ema, const float *__restric
     }
     cnt = block_sum(cnt, red);
     if (threadIdx.x == 0 && usage_out) usage_out[row] = cnt / (float)V * 100.f;
-    if (record_hit_dev && threadIdx.x == 0) {
+    if (threadIdx.x == 0) {
         __threadfence();
         if (atomicAdd(done_counter, 1u) == gridDim.x - 1) {      // every block has read the counter: safe to advance it
             *record_hit_dev += gridDim.x;
@@ -661,19 +661,11 @@ int xq_perturb_backward(const float *z, const float *g, int B, int C, int HW, in
     return XQ_OK;
 }
 
-int xq_usage_ema(float *ema, const float *hit, int rows, int V, int record_hit, float margin, float *usage_out,
-                 void *stream_) {
-    if (!ema || !hit || V <= 0 || rows <= 0) return XQ_ERR_ARG;
-    usage_ema_kernel<<<rows, 1024, 0, (cudaStream_t)stream_>>>(ema, hit, V, record_hit, margin, usage_out, nullptr, nullptr);
-    XQ_LAUNCH_CHECK("usage_ema_kernel");
-    return XQ_OK;
-}
-
 int xq_usage_ema_dev(float *ema, const float *hit, int rows, int V, int64_t *record_hit_dev, float margin, float *usage_out,
                      void *stream_) {
     if (!ema || !hit || !record_hit_dev || V <= 0 || rows <= 0) return XQ_ERR_ARG;
     // record_hit_dev[0] = the counter, record_hit_dev[1] = scratch for the last-block detection (must start at 0)
-    usage_ema_kernel<<<rows, 1024, 0, (cudaStream_t)stream_>>>(ema, hit, V, 0, margin, usage_out, (long long *)record_hit_dev,
+    usage_ema_kernel<<<rows, 1024, 0, (cudaStream_t)stream_>>>(ema, hit, V, margin, usage_out, (long long *)record_hit_dev,
                                                                (unsigned int *)(record_hit_dev + 1));
     XQ_LAUNCH_CHECK("usage_ema_kernel");
     return XQ_OK;

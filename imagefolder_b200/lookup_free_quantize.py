@@ -19,7 +19,7 @@ Reference behaviour that is kept on purpose:
 from __future__ import annotations
 
 from math import sqrt
-from typing import List, Optional, Sequence, Tuple, Union
+from typing import Tuple
 
 import torch
 from torch import nn as nn
@@ -54,7 +54,7 @@ class LFQ(_MultiScaleBase):
         self.quant_resi = build_quant_resi(Cvae, quant_resi, share_quant_resi, default_qresi_counts, self.v_patch_nums)
 
         self.register_buffer('ema_vocab_hit_SV', torch.full((len(self.v_patch_nums), self.vocab_size), fill_value=0.0))
-        self.record_hit = 0
+        self.register_buffer('_record_hit_dev', torch.zeros(2, dtype=torch.int64), persistent=False)
         self.register_buffer('mask', 2 ** torch.arange(self.Cvae), persistent=False)
         self.beta: float = beta
         self.codebook_drop = codebook_drop
@@ -131,40 +131,3 @@ class LFQ(_MultiScaleBase):
         if si is None:
             return x
         return torch.where(x, self.scaler[si], -self.scaler[si])
-
-    def f_to_idxBl_or_fhat(self, f_BChw: torch.Tensor, to_fhat: bool,
-                           v_patch_nums: Optional[Sequence[Union[int, Tuple[int, int]]]] = None):
-        """:345-380."""
-        B, Cc, H, W = f_BChw.shape
-        pns = [pn if isinstance(pn, int) else pn[0] for pn in (v_patch_nums or self.v_patch_nums)]
-        d, w, b, pns = self._desc(B, H, W, pns)
-        _, idx_all, fs = ops.ms_lookup(f_BChw.detach(), None, w, b, d, want_fhat_scales=to_fhat)
-        if to_fhat:
-            return list(fs.unbind(0))
-        return ops.split_scales(idx_all, B, pns)
-
-    def idx_to_fhat(self, gt_ms_idx_Bl: List[torch.Tensor], last_one=True):
-        B = gt_ms_idx_Bl[0].shape[0]
-        H = W = self.v_patch_nums[-1]
-        d, w, b, pns = self._desc(B, H, W)
-        d.channel_norm = 0
-        idx_all = torch.cat([t.reshape(-1) for t in gt_ms_idx_Bl]).to(torch.int64)
-        out, fs, _ = ops.ms_decode(idx_all, None, w, b, d, want_out=last_one, want_fhat_scales=not last_one)
-        return out if last_one else list(fs.unbind(0))
-
-    def idxBl_to_var_input(self, gt_ms_idx_Bl: List[torch.Tensor]) -> torch.Tensor:
-        """:383-401 (the reference's version reads a non-existent self.embedding; here the BSQ codes
-        +-scaler[si] are used, which is what indices_to_bits(idx, si) yields)."""
-        SN = len(self.v_patch_nums)
-        if SN < 2:
-            return None
-        B = gt_ms_idx_Bl[0].shape[0]
-        H = W = self.v_patch_nums[-1]
-        d, w, b, pns = self._desc(B, H, W)
-        d.channel_norm = 0
-        lists = list(gt_ms_idx_Bl)
-        if len(lists) < SN:
-            lists = lists + [torch.zeros(B, pns[-1] ** 2, dtype=torch.int64, device=lists[0].device)]
-        idx_all = torch.cat([t.reshape(-1) for t in lists]).to(torch.int64)
-        _, _, var = ops.ms_decode(idx_all, None, w, b, d, want_out=False, want_var_input=True)
-        return var

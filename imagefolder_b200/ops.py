@@ -1,4 +1,5 @@
-"""autograd.Function wrappers over the C ABI (include/xqb200.h).
+"""The quantizers' binding of the C ABI (include/xqb200.h): torch.library ops for the single-scale VQ and the usage EMA,
+autograd.Function wrappers for the latent perturbation and the multi-scale quantizers.
 
 PyTorch is plumbing here: it owns the device memory and the stream; every arithmetic step of the
 quantizer path happens inside libxqb200.so.  Gradients are the closed forms of SURVEY.md
@@ -9,69 +10,31 @@ from __future__ import annotations
 from typing import List, Sequence, Tuple
 
 import torch
+from torch import Tensor
 
 from . import _capi as C
 
 
-def _f32c(t: torch.Tensor) -> torch.Tensor:
+def _f32c(t):
+    """contiguous fp32 view or copy of t (None stays None)."""
+    if t is None:
+        return None
     if t.dtype != torch.float32:
         t = t.float()
     return t.contiguous()
 
 
 # ----------------------------------------------------------------------------------------------
-# single-scale VQ
+# single-scale VQ: torch.library ops, so that torch.compile(fullgraph=True) traces VectorQuantizer.forward without graph
+# breaks and CUDA graphs capture it (SURVEY.md section 8b: "loaded as PyTorch custom ops through a thin C-ABI")
+#
+#     torch.ops.xqb200.vq_forward(z, E, beta, codebook_norm)                       -> (out, loss[2], idx, hist)
+#     torch.ops.xqb200.vq_backward(z, E, idx, g_out, g_loss, beta, codebook_norm)  -> (gz, gE)
+#     torch.ops.xqb200.usage_ema_(ema, hit, counter, margin)                       -> usage[rows]  (mutates ema and counter)
 # ----------------------------------------------------------------------------------------------
-class _VQForward(torch.autograd.Function):
-    """(z[B,C,H,W], E[V,C]) -> out, vq_loss, commit_loss, idx, hist   (xqgan_model.py:745-801)."""
-
-    @staticmethod
-    def forward(ctx, z, E, beta: float, codebook_norm: bool, want_hist: bool):
-        z, E = _f32c(z), _f32c(E)
-        B, Cc = z.shape[0], z.shape[1]
-        HW = z[0, 0].numel()
-        V = E.shape[0]
-        dev = z.device
-        idx = torch.empty(B * HW, dtype=torch.int64, device=dev)
-        out = torch.empty_like(z)
-        loss = torch.empty(2, dtype=torch.float32, device=dev)
-        hist = torch.zeros(V, dtype=torch.float32, device=dev) if want_hist else None
-        L = C.lib()
-        ws = C.workspace(L.xq_vq_workspace_bytes(B, Cc, HW, V), dev)
-        C.call("xq_vq_forward", 3, L.xq_vq_forward, C.ptr(z), C.ptr(E), B, Cc, HW, V, int(codebook_norm), 1,
-               float(beta), C.ptr(idx), C.ptr(out), C.ptr(loss), C.ptr(hist), C.ptr(ws), ws.numel(), C.stream_ptr(dev))
-        ctx.save_for_backward(z, E, idx)
-        ctx.beta, ctx.codebook_norm = float(beta), bool(codebook_norm)
-        ctx.mark_non_differentiable(idx)
-        if hist is not None:
-            ctx.mark_non_differentiable(hist)
-        return out, loss[0], loss[1], idx, hist
-
-    @staticmethod
-    def backward(ctx, g_out, g_vq, g_commit, _gi, _gh):
-        z, E, idx = ctx.saved_tensors
-        B, Cc = z.shape[0], z.shape[1]
-        HW = z[0, 0].numel()
-        V = E.shape[0]
-        g_out = _f32c(g_out) if g_out is not None else None
-        g_vq = _f32c(g_vq) if g_vq is not None else None
-        g_commit = _f32c(g_commit) if g_commit is not None else None
-        gz = torch.empty_like(z)
-        gE = torch.empty_like(E)
-        L = C.lib()
-        C.call("xq_vq_backward", 1, L.xq_vq_backward, C.ptr(z), C.ptr(E), C.ptr(idx), C.ptr(g_out), C.ptr(g_vq),
-               C.ptr(g_commit), B, Cc, HW, V, int(ctx.codebook_norm), ctx.beta, C.ptr(gz), C.ptr(gE),
-               C.stream_ptr(z.device))
-        return gz, gE, None, None, None
-
-
-def vq_forward(z, E, beta=0.25, codebook_norm=True, want_hist=True):
-    return _VQForward.apply(z, E, beta, codebook_norm, want_hist)
-
-
-@torch.no_grad()
-def vq_lookup(z, E, codebook_norm=True) -> Tuple[torch.Tensor, torch.Tensor]:
-    """inference: (q[B,C,H,W], idx[N])  (xqgan_model.py:803-833)."""
+def _vq_search(z, E, codebook_norm: bool, train: bool, beta: float = 0.0):
+    """one xq_vq_forward call.  train: straight-through output, {vq, commit} losses and code histogram
+    (xqgan_model.py:745-801); otherwise the codes themselves, no losses (xqgan_model.py:803-833)."""
     z, E = _f32c(z), _f32c(E)
     B, Cc = z.shape[0], z.shape[1]
     HW = z[0, 0].numel()
@@ -79,11 +42,97 @@ def vq_lookup(z, E, codebook_norm=True) -> Tuple[torch.Tensor, torch.Tensor]:
     dev = z.device
     idx = torch.empty(B * HW, dtype=torch.int64, device=dev)
     out = torch.empty_like(z)
+    loss = torch.empty(2, dtype=torch.float32, device=dev) if train else None
+    hist = torch.zeros(V, dtype=torch.float32, device=dev) if train else None
     L = C.lib()
     ws = C.workspace(L.xq_vq_workspace_bytes(B, Cc, HW, V), dev)
-    C.call("xq_vq_lookup", 2, L.xq_vq_forward, C.ptr(z), C.ptr(E), B, Cc, HW, V, int(codebook_norm), 0, 0.0,
-           C.ptr(idx), C.ptr(out), None, None, C.ptr(ws), ws.numel(), C.stream_ptr(dev))
+    name, nk = ("xq_vq_forward", 3) if train else ("xq_vq_lookup", 2)
+    C.call(name, nk, L.xq_vq_forward, C.ptr(z), C.ptr(E), B, Cc, HW, V, int(codebook_norm), int(train), float(beta),
+           C.ptr(idx), C.ptr(out), C.ptr(loss), C.ptr(hist), C.ptr(ws), ws.numel(), C.stream_ptr(dev))
+    return out, loss, idx, hist
+
+
+@torch.library.custom_op("xqb200::vq_forward", mutates_args=())
+def _vq_forward(z: Tensor, E: Tensor, beta: float, codebook_norm: bool) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+    return _vq_search(z, E, codebook_norm, train=True, beta=beta)
+
+
+@_vq_forward.register_fake
+def _(z, E, beta, codebook_norm):
+    n = z.shape[0] * z[0, 0].numel()
+    return (torch.empty_like(z, dtype=torch.float32, memory_format=torch.contiguous_format), z.new_empty(2, dtype=torch.float32),
+            z.new_empty(n, dtype=torch.int64), z.new_empty(E.shape[0], dtype=torch.float32))
+
+
+@torch.library.custom_op("xqb200::vq_backward", mutates_args=())
+def _vq_backward(z: Tensor, E: Tensor, idx: Tensor, g_out: Tensor, g_loss: Tensor, beta: float,
+                codebook_norm: bool) -> Tuple[Tensor, Tensor]:
+    z, E, g_out, g_loss = _f32c(z), _f32c(E), _f32c(g_out), _f32c(g_loss)
+    B, Cc = z.shape[0], z.shape[1]
+    HW = z[0, 0].numel()
+    V = E.shape[0]
+    gz = torch.empty_like(z)
+    gE = torch.empty_like(E)
+    L = C.lib()
+    C.call("xq_vq_backward", 1, L.xq_vq_backward, C.ptr(z), C.ptr(E), C.ptr(idx), C.ptr(g_out), C.ptr(g_loss),
+           C.ptr(g_loss) + 4, B, Cc, HW, V, int(codebook_norm), float(beta), C.ptr(gz), C.ptr(gE), C.stream_ptr(z.device))
+    return gz, gE
+
+
+@_vq_backward.register_fake
+def _(z, E, idx, g_out, g_loss, beta, codebook_norm):
+    return (torch.empty_like(z, dtype=torch.float32, memory_format=torch.contiguous_format),
+            torch.empty_like(E, dtype=torch.float32, memory_format=torch.contiguous_format))
+
+
+def _vq_setup(ctx, inputs, output):
+    z, E, beta, codebook_norm = inputs
+    ctx.save_for_backward(z, E, output[2])
+    ctx.beta, ctx.codebook_norm = beta, codebook_norm
+
+
+def _vq_bwd(ctx, g_out, g_loss, _g_idx, _g_hist):
+    z, E, idx = ctx.saved_tensors
+    if g_out is None:
+        g_out = torch.zeros_like(z, dtype=torch.float32)
+    if g_loss is None:
+        g_loss = z.new_zeros(2, dtype=torch.float32)
+    gz, gE = torch.ops.xqb200.vq_backward(z, E, idx, g_out, g_loss, ctx.beta, ctx.codebook_norm)
+    return gz, gE, None, None
+
+
+torch.library.register_autograd("xqb200::vq_forward", _vq_bwd, setup_context=_vq_setup)
+
+
+def vq_forward(z, E, beta=0.25, codebook_norm=True, want_hist=True):
+    """(z[B,C,H,W], E[V,C]) -> out, vq_loss, commit_loss, idx, hist|None   (xqgan_model.py:745-801)."""
+    out, loss, idx, hist = torch.ops.xqb200.vq_forward(z, E, beta, codebook_norm)
+    return out, loss[0], loss[1], idx, (hist.detach() if want_hist else None)    # statistics only: no gradient
+
+
+@torch.no_grad()
+def vq_lookup(z, E, codebook_norm=True) -> Tuple[torch.Tensor, torch.Tensor]:
+    """inference: (q[B,C,H,W], idx[N])  (xqgan_model.py:803-833)."""
+    out, _, idx, _ = _vq_search(z, E, codebook_norm, train=False)
     return out, idx
+
+
+@torch.library.custom_op("xqb200::usage_ema_", mutates_args=("ema", "counter"))
+def usage_ema_(ema: Tensor, hit: Tensor, counter: Tensor, margin: float) -> Tensor:
+    """in-place EMA update of ema [rows, V] or [V] from hit (same shape) + usage percentages (device tensor [rows]).
+    counter: int64 [2] on the device, the quantizer's step counter and the kernel's scratch word (see xq_usage_ema_dev)."""
+    rows = 1 if ema.dim() == 1 else ema.shape[0]
+    V = ema.shape[-1]
+    usage = torch.empty(rows, dtype=torch.float32, device=ema.device)
+    L = C.lib()
+    C.call("xq_usage_ema", 1, L.xq_usage_ema_dev, C.ptr(ema), C.ptr(hit.contiguous()), rows, V, C.ptr(counter),
+           float(margin), C.ptr(usage), C.stream_ptr(ema.device))
+    return usage
+
+
+@usage_ema_.register_fake
+def _(ema, hit, counter, margin):
+    return ema.new_empty(1 if ema.dim() == 1 else ema.shape[0], dtype=torch.float32)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -131,22 +180,23 @@ def perturb(z, z_q, E, rand_u, rand_j, codebook_norm, alpha, n_perturb, delta):
 # ----------------------------------------------------------------------------------------------
 # multi-scale residual (VQ2 / BSQ)
 # ----------------------------------------------------------------------------------------------
+def _ms_idx_buffer(L, desc, dev) -> torch.Tensor:
+    """the int64 token buffer of every scale (checks the descriptor)."""
+    total = L.xq_ms_total_tokens(desc)
+    if total < 0:
+        raise ValueError("xq_ms_forward: invalid multi-scale descriptor")
+    return torch.empty(total, dtype=torch.int64, device=dev)
+
+
 class _MSForward(torch.autograd.Function):
     """(f, E|None, phi_w|None, phi_b|None) -> out, vq, commit, entropy, idx_all, hist."""
 
     @staticmethod
     def forward(ctx, f, E, phi_w, phi_b, n_quantizers, desc, want_hist: bool):
-        f = _f32c(f)
-        E = _f32c(E) if E is not None else None
-        phi_w = _f32c(phi_w) if phi_w is not None else None
-        phi_b = _f32c(phi_b) if phi_b is not None else None
-        nq = n_quantizers.float().contiguous() if n_quantizers is not None else None
+        f, E, phi_w, phi_b, nq = map(_f32c, (f, E, phi_w, phi_b, n_quantizers))
         dev = f.device
         L = C.lib()
-        total = L.xq_ms_total_tokens(desc)
-        if total < 0:
-            raise ValueError("xq_ms_forward: invalid multi-scale descriptor")
-        idx_all = torch.empty(total, dtype=torch.int64, device=dev)
+        idx_all = _ms_idx_buffer(L, desc, dev)
         out = torch.empty_like(f)
         loss = torch.empty(3, dtype=torch.float32, device=dev)
         hist = torch.zeros(desc.SN, desc.V, dtype=torch.float32, device=dev) if want_hist else None
@@ -174,10 +224,7 @@ class _MSForward(torch.autograd.Function):
         desc = ctx.desc
         dev = f.device
         L = C.lib()
-        g_out = _f32c(g_out) if g_out is not None else None
-        g_vq = _f32c(g_vq) if g_vq is not None else None
-        g_commit = _f32c(g_commit) if g_commit is not None else None
-        g_ent = _f32c(g_ent) if g_ent is not None else None
+        g_out, g_vq, g_commit, g_ent = map(_f32c, (g_out, g_vq, g_commit, g_ent))
         gf = torch.empty_like(f)
         gE = torch.empty_like(E) if E is not None else None
         gw = torch.empty_like(phi_w) if phi_w is not None else None
@@ -207,16 +254,10 @@ def split_scales(idx_all: torch.Tensor, B: int, patch_nums: Sequence[int]) -> Li
 @torch.no_grad()
 def ms_lookup(f, E, phi_w, phi_b, desc, want_fhat_scales: bool):
     """inference loop (quant.py:182-223): returns (f_hat_last, idx_all, fhat_scales|None)."""
-    f = _f32c(f)
-    E = _f32c(E) if E is not None else None
-    phi_w = _f32c(phi_w) if phi_w is not None else None
-    phi_b = _f32c(phi_b) if phi_b is not None else None
+    f, E, phi_w, phi_b = map(_f32c, (f, E, phi_w, phi_b))
     dev = f.device
     L = C.lib()
-    total = L.xq_ms_total_tokens(desc)
-    if total < 0:
-        raise ValueError("xq_ms_forward: invalid multi-scale descriptor")
-    idx_all = torch.empty(total, dtype=torch.int64, device=dev)
+    idx_all = _ms_idx_buffer(L, desc, dev)
     out = torch.empty_like(f)
     fs = torch.empty((desc.SN,) + tuple(f.shape), dtype=torch.float32, device=dev) if want_fhat_scales else None
     ws = C.workspace(L.xq_ms_workspace_bytes(desc), dev)
@@ -230,9 +271,7 @@ def ms_lookup(f, E, phi_w, phi_b, desc, want_fhat_scales: bool):
 def ms_decode(idx_all, E, phi_w, phi_b, desc, want_out=True, want_fhat_scales=False, want_var_input=False):
     """indices -> f_hat / per-scale f_hat / next-scale inputs (quant.py:148-180, 226-244)."""
     dev = idx_all.device
-    E = _f32c(E) if E is not None else None
-    phi_w = _f32c(phi_w) if phi_w is not None else None
-    phi_b = _f32c(phi_b) if phi_b is not None else None
+    E, phi_w, phi_b = map(_f32c, (E, phi_w, phi_b))
     shape = (desc.B, desc.C, desc.H, desc.W)
     out = torch.empty(shape, dtype=torch.float32, device=dev) if want_out else None
     fs = torch.empty((desc.SN,) + shape, dtype=torch.float32, device=dev) if want_fhat_scales else None
@@ -250,8 +289,7 @@ def ms_embed(h_all, phi_w, phi_b, desc, si0: int, si1: int, f_hat=None, want_sca
     f_hat += Phi_si(bicubic_up(h_si)).  `f_hat` (fp32 [B,C,H,W], contiguous) is updated IN PLACE when given, as the
     reference's f_hat.add_ does.  -> (f_hat, per-scale cumulative f_hat [si1-si0,B,C,H,W] | None, next | None)"""
     dev = h_all.device
-    phi_w = _f32c(phi_w) if phi_w is not None else None
-    phi_b = _f32c(phi_b) if phi_b is not None else None
+    phi_w, phi_b = _f32c(phi_w), _f32c(phi_b)
     shape = (desc.B, desc.C, desc.H, desc.W)
     if f_hat is not None:
         if tuple(f_hat.shape) != shape or f_hat.dtype != torch.float32 or not f_hat.is_contiguous():
@@ -268,14 +306,3 @@ def ms_embed(h_all, phi_w, phi_b, desc, si0: int, si1: int, f_hat=None, want_sca
     C.call("xq_ms_embed", 1, L.xq_ms_embed, desc, int(si0), int(si1), C.ptr(h_all), C.ptr(phi_w), C.ptr(phi_b),
            C.ptr(fin), C.ptr(out), C.ptr(fs), C.ptr(nxt), C.stream_ptr(dev))
     return out, fs, nxt
-
-
-def usage_ema_(ema: torch.Tensor, hit: torch.Tensor, record_hit: int, margin: float) -> torch.Tensor:
-    """in-place EMA update of all rows + usage percentages (device tensor [rows])."""
-    rows = 1 if ema.dim() == 1 else ema.shape[0]
-    V = ema.shape[-1]
-    usage = torch.empty(rows, dtype=torch.float32, device=ema.device)
-    L = C.lib()
-    C.call("xq_usage_ema", 1, L.xq_usage_ema, C.ptr(ema), C.ptr(hit.contiguous()), rows, V, int(record_hit),
-           float(margin), C.ptr(usage), C.stream_ptr(ema.device))
-    return usage

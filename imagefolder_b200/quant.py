@@ -11,6 +11,7 @@ Differences from the reference, all host-side:
   * `usages` are 0-dim device tensors unless `sync_usages=True` (the reference calls .item() per
     scale = SN host syncs per forward, quant.py:140); float(u) gives the reference value;
   * a process group is optional (the reference requires one even on 1 GPU, quant.py:137).
+  * `record_hit` reads and writes a device counter that the usage-EMA kernel advances by SN per training forward.
 """
 from __future__ import annotations
 
@@ -34,6 +35,16 @@ def _world_size() -> int:
 def _allreduce_hist_(hist: torch.Tensor) -> None:
     if tdist.is_available() and tdist.is_initialized() and tdist.get_world_size() > 1:
         tdist.all_reduce(hist)
+
+
+def _set_record_hit(self, value: int) -> None:
+    self._record_hit_dev.copy_(torch.tensor([int(value), 0]))
+
+
+# The reference's `record_hit` (the usage EMA's step counter) as a view of the device buffer `_record_hit_dev` = [counter,
+# kernel scratch word], which the usage-EMA kernel reads and advances without the host.  Reading it synchronises with the
+# device, so no forward does; like the reference's plain attribute it is not part of the state_dict.
+record_hit_property = property(lambda self: int(self._record_hit_dev[0]), _set_record_hit)
 
 
 class Phi(nn.Conv2d):
@@ -117,6 +128,7 @@ class _MultiScaleBase(nn.Module):
     """host logic shared by VectorQuantizer2 and LFQ (descriptor, Phi stacking, EMA, usages)."""
 
     sync_usages: bool = False
+    record_hit = record_hit_property
 
     def _phi_params(self):
         mods = self.quant_resi.modules_list()
@@ -150,8 +162,7 @@ class _MultiScaleBase(nn.Module):
         margin = _world_size() * numel_per_channel / self.vocab_size * 0.08
         if self.training:
             _allreduce_hist_(hist)
-            usage = ops.usage_ema_(self.ema_vocab_hit_SV, hist, self.record_hit, margin)
-            self.record_hit += SN
+            usage = torch.ops.xqb200.usage_ema_(self.ema_vocab_hit_SV, hist, self._record_hit_dev, margin)
         else:
             usage = (self.ema_vocab_hit_SV >= margin).float().mean(dim=-1) * 100
         if not ret_usages:
@@ -162,12 +173,18 @@ class _MultiScaleBase(nn.Module):
 
 
     # ===================== feature-map helpers shared by VectorQuantizer2 and LFQ =====================
-    def _embed_steps(self, hs, si0: int, f_hat, want_scales: bool, want_next: bool):
-        """scales [si0, si0+len(hs)) of  f_hat += Phi_si(bicubic_up(h_si))  in ONE fused kernel (xq_ms_embed)."""
-        B = hs[0].shape[0]
+    def _decode_desc(self, B: int):
+        """descriptor for building f_hat at the module's scales from codes or feature maps, which are used as they are
+        (no channel normalisation)."""
         H = W = self.v_patch_nums[-1]
         d, w, b, pns = self._desc(B, H, W)
         d.channel_norm = 0
+        return d, w, b, pns
+
+    def _embed_steps(self, hs, si0: int, f_hat, want_scales: bool, want_next: bool):
+        """scales [si0, si0+len(hs)) of  f_hat += Phi_si(bicubic_up(h_si))  in ONE fused kernel (xq_ms_embed)."""
+        B = hs[0].shape[0]
+        d, w, b, pns = self._decode_desc(B)
         for k, h in enumerate(hs):
             want = (B, self.Cvae, pns[si0 + k], pns[si0 + k])
             if tuple(h.shape) != want:
@@ -213,6 +230,48 @@ class _MultiScaleBase(nn.Module):
         _, _, nxt = self._embed_steps([h_BChw], si, f_hat, want_scales=False, want_next=si != SN - 1)
         return f_hat, (nxt if si != SN - 1 else f_hat)
 
+    # ===================== inference (VectorQuantizer2 / LFQ) =====================
+    def _codebook(self) -> Optional[torch.Tensor]:
+        """the codebook the kernels read: None for LFQ, whose codes are +-scaler per bit; VectorQuantizer2 returns its
+        embedding."""
+        return None
+
+    def f_to_idxBl_or_fhat(self, f_BChw: torch.Tensor, to_fhat: bool,
+                           v_patch_nums: Optional[Sequence[Union[int, Tuple[int, int]]]] = None):
+        """quant.py:182-223 / lookup_free_quantize.py:345-380: list over scales of idx [B, pn*pn] (int64) or cumulative
+        f_hat [B,C,H,W]."""
+        B, Cc, H, W = f_BChw.shape
+        pns = [pn if isinstance(pn, int) else pn[0] for pn in (v_patch_nums or self.v_patch_nums)]
+        d, w, b, pns = self._desc(B, H, W, pns)
+        _, idx_all, fs = ops.ms_lookup(f_BChw.detach(), self._codebook(), w, b, d, want_fhat_scales=to_fhat)
+        if to_fhat:
+            return list(fs.unbind(0))
+        return ops.split_scales(idx_all, B, pns)
+
+    def idx_to_fhat(self, gt_ms_idx_Bl: List[torch.Tensor], last_one=True):
+        """token lists -> f_hat (fused decode kernel; used by VQModel.decode_tokens)."""
+        d, w, b, _ = self._decode_desc(gt_ms_idx_Bl[0].shape[0])
+        idx_all = torch.cat([t.reshape(-1) for t in gt_ms_idx_Bl]).to(torch.int64)
+        out, fs, _ = ops.ms_decode(idx_all, self._codebook(), w, b, d, want_out=last_one, want_fhat_scales=not last_one)
+        return out if last_one else list(fs.unbind(0))
+
+    # ===================== idxBl_to_var_input: only used in VAR training =====================
+    def idxBl_to_var_input(self, gt_ms_idx_Bl: List[torch.Tensor]) -> torch.Tensor:
+        """quant.py:226-244 / lookup_free_quantize.py:383-401 -> [B, sum_{si>=1} pn^2, C] float32 (None for a single
+        scale).  The reference's LFQ version reads a non-existent self.embedding; here LFQ uses its BSQ codes +-scaler[si],
+        which is what indices_to_bits(idx, si) yields."""
+        SN = len(self.v_patch_nums)
+        if SN < 2:
+            return None
+        B = gt_ms_idx_Bl[0].shape[0]
+        d, w, b, pns = self._decode_desc(B)
+        lists = list(gt_ms_idx_Bl)
+        if len(lists) < SN:  # the last scale's tokens are not needed for teacher forcing
+            lists = lists + [torch.zeros(B, pns[-1] ** 2, dtype=torch.int64, device=lists[0].device)]
+        idx_all = torch.cat([t.reshape(-1) for t in lists]).to(torch.int64)
+        _, _, var = ops.ms_decode(idx_all, self._codebook(), w, b, d, want_out=False, want_var_input=True)
+        return var
+
 
 class VectorQuantizer2(_MultiScaleBase):
     # VQGAN originally use beta=1.0, never tried 0.25; SD seems using 0.25
@@ -232,7 +291,7 @@ class VectorQuantizer2(_MultiScaleBase):
         self.quant_resi = build_quant_resi(Cvae, quant_resi, share_quant_resi, default_qresi_counts, self.v_patch_nums)
 
         self.register_buffer('ema_vocab_hit_SV', torch.full((len(self.v_patch_nums), self.vocab_size), fill_value=0.0))
-        self.record_hit = 0
+        self.register_buffer('_record_hit_dev', torch.zeros(2, dtype=torch.int64), persistent=False)
 
         self.beta: float = beta
         self.embedding = nn.Embedding(self.vocab_size, self.Cvae)
@@ -263,6 +322,9 @@ class VectorQuantizer2(_MultiScaleBase):
                            resi_ratio=abs(self.quant_resi_ratio), beta=self.beta, loss_div_sn_all=False)
         return d, w, b, pns
 
+    def _codebook(self):
+        return self.embedding.weight.data
+
     # ===================== `forward` is only used in VAE training =====================
     def forward(self, f_BChw: torch.Tensor, ret_usages=False, dropout=None):
         """-> (f_hat, usages|None, mean_vq_loss, mean_commit_loss, 0)   (quant.py:64-144)"""
@@ -276,41 +338,3 @@ class VectorQuantizer2(_MultiScaleBase):
         usages = self._update_usage(hist, f_BChw.numel() / f_BChw.shape[1], ret_usages)
         self.last_idx_Bl = ops.split_scales(idx_all, B, pns)
         return f_hat, usages, vq, commit, 0
-
-    # ===================== inference =====================
-    def f_to_idxBl_or_fhat(self, f_BChw: torch.Tensor, to_fhat: bool,
-                           v_patch_nums: Optional[Sequence[Union[int, Tuple[int, int]]]] = None):
-        """quant.py:182-223: list over scales of idx [B, pn*pn] (int64) or cumulative f_hat [B,C,H,W]."""
-        B, Cc, H, W = f_BChw.shape
-        pns = [pn if isinstance(pn, int) else pn[0] for pn in (v_patch_nums or self.v_patch_nums)]
-        d, w, b, pns = self._desc(B, H, W, pns)
-        _, idx_all, fs = ops.ms_lookup(f_BChw.detach(), self.embedding.weight.data, w, b, d, want_fhat_scales=to_fhat)
-        if to_fhat:
-            return list(fs.unbind(0))
-        return ops.split_scales(idx_all, B, pns)
-
-    def idx_to_fhat(self, gt_ms_idx_Bl: List[torch.Tensor], last_one=True):
-        """token lists -> f_hat (fused decode kernel; used by VQModel.decode_tokens)."""
-        B = gt_ms_idx_Bl[0].shape[0]
-        H = W = self.v_patch_nums[-1]
-        d, w, b, pns = self._desc(B, H, W)
-        idx_all = torch.cat([t.reshape(-1) for t in gt_ms_idx_Bl]).to(torch.int64)
-        out, fs, _ = ops.ms_decode(idx_all, self.embedding.weight.data, w, b, d, want_out=last_one,
-                                   want_fhat_scales=not last_one)
-        return out if last_one else list(fs.unbind(0))
-
-    # ===================== idxBl_to_var_input: only used in VAR training =====================
-    def idxBl_to_var_input(self, gt_ms_idx_Bl: List[torch.Tensor]) -> torch.Tensor:
-        """quant.py:226-244 -> [B, sum_{si>=1} pn^2, C] float32 (None for a single scale)."""
-        SN = len(self.v_patch_nums)
-        if SN < 2:
-            return None
-        B = gt_ms_idx_Bl[0].shape[0]
-        H = W = self.v_patch_nums[-1]
-        d, w, b, pns = self._desc(B, H, W)
-        lists = list(gt_ms_idx_Bl)
-        if len(lists) < SN:  # the last scale's tokens are not needed for teacher forcing
-            lists = lists + [torch.zeros(B, pns[-1] ** 2, dtype=torch.int64, device=lists[0].device)]
-        idx_all = torch.cat([t.reshape(-1) for t in lists]).to(torch.int64)
-        _, _, var = ops.ms_decode(idx_all, self.embedding.weight.data, w, b, d, want_out=False, want_var_input=True)
-        return var

@@ -12,17 +12,14 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import ops
-from .quant import _allreduce_hist_, _world_size
+from .quant import _allreduce_hist_, _world_size, record_hit_property
 
 __all__ = ["VectorQuantizer"]
 
 
 class VectorQuantizer(nn.Module):
     sync_usages: bool = False  # True: usages are python floats like the reference (one host sync)
-    # True: go through the torch.library registrations of the same C entry points (imagefolder_b200/custom_ops.py:
-    # torch.ops.xqb200.*), with the usage-EMA step counter on the device -- the form torch.compile(fullgraph=True) traces
-    # and CUDA graphs capture.  False: the autograd.Function wrappers of ops.py (step counter = the Python int `record_hit`).
-    use_custom_ops: bool = False
+    record_hit = record_hit_property
 
     def __init__(self, vocab_size=8192, z_channels=32, beta=0.25, codebook_norm=True):
         super().__init__()
@@ -37,8 +34,6 @@ class VectorQuantizer(nn.Module):
             self.embedding.weight.data = F.normalize(self.embedding.weight.data, p=2, dim=-1)
 
         self.register_buffer("ema_vocab_hit_SV", torch.full((self.vocab_size,), fill_value=0.0))
-        self.record_hit = 0
-        # device twin of `record_hit` (+ one scratch word) for the custom-op path; not part of the checkpoint, like record_hit
         self.register_buffer("_record_hit_dev", torch.zeros(2, dtype=torch.int64), persistent=False)
 
     def no_weight_decay(self):
@@ -48,25 +43,11 @@ class VectorQuantizer(nn.Module):
         """-> (z_q, [codebook_usage], vq_loss, commit_loss, 0.0)      (xqgan_model.py:745-801)"""
         assert z.shape[1] == self.z_channels
         margin = _world_size() * (z.numel() / self.z_channels) / self.vocab_size * 0.08
-        if self.use_custom_ops:
-            from . import custom_ops  # noqa: F401  (registers torch.ops.xqb200.*)
-            z_q, loss2, idx, hist = torch.ops.xqb200.vq_forward(z, self.embedding.weight, self.beta, self.codebook_norm)
-            vq_loss, commit_loss = loss2[0], loss2[1]
-            self.last_idx = idx
-            if ret_usages and self.training:
-                hist = hist.detach()                 # statistics only: no gradient flows through the usage EMA
-                _allreduce_hist_(hist)
-                usage = torch.ops.xqb200.usage_ema_(self.ema_vocab_hit_SV, hist, self._record_hit_dev, margin)[0]
-            else:
-                usage = (self.ema_vocab_hit_SV >= margin).float().mean() * 100
-            return z_q, [usage], vq_loss, commit_loss, 0.0
-        z_q, vq_loss, commit_loss, idx, hist = ops.vq_forward(z, self.embedding.weight, self.beta, self.codebook_norm,
-                                                              want_hist=True)
+        z_q, vq_loss, commit_loss, idx, hist = ops.vq_forward(z, self.embedding.weight, self.beta, self.codebook_norm)
         self.last_idx = idx
         if ret_usages and self.training:
             _allreduce_hist_(hist)
-            usage = ops.usage_ema_(self.ema_vocab_hit_SV, hist, self.record_hit, margin)[0]
-            self.record_hit += 1
+            usage = torch.ops.xqb200.usage_ema_(self.ema_vocab_hit_SV, hist, self._record_hit_dev, margin)[0]
         else:
             # the reference leaves `codebook_usage` unbound here (NameError); report the current EMA instead
             usage = (self.ema_vocab_hit_SV >= margin).float().mean() * 100

@@ -197,12 +197,10 @@ int xq_ms_embed(const xq_ms_desc *d, int si0, int si1, const float *h_all, const
  *   ema[rows,V], hit[rows,V]: row i <- copy | 0.9/0.1 | 0.99/0.01 blend of hit[i], chosen by
  *   (record_hit + i) == 0 | < 100 | otherwise  (the reference bumps record_hit once per scale).
  *   usage_out[rows] (device, may be NULL) = 100 * mean(ema[i] >= margin)
- * ------------------------------------------------------------------------------------------ */
-int xq_usage_ema(float *ema, const float *hit, int rows, int V, int record_hit, float margin,
-                 float *usage_out, void *stream);
-/* same, with the step counter on the device: record_hit_dev[0] = `record_hit` (read, then advanced by `rows` by the kernel),
+ * The step counter is on the device: record_hit_dev[0] = `record_hit` (read, then advanced by `rows` by the kernel),
  * record_hit_dev[1] = scratch (zero-initialised once).  The host neither reads nor writes the counter, which keeps the call
- * CUDA-graph capturable and lets torch.compile trace the module without specialising on a Python int. */
+ * CUDA-graph capturable and lets torch.compile trace the module without specialising on a Python int.
+ * ------------------------------------------------------------------------------------------ */
 int xq_usage_ema_dev(float *ema, const float *hit, int rows, int V, int64_t *record_hit_dev, float margin,
                      float *usage_out, void *stream);
 

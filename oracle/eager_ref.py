@@ -14,12 +14,28 @@ Follows: VectorQuantizer.forward            tokenizer/tokenizer_image/xqgan_mode
 """
 from __future__ import annotations
 
+import weakref
+
 import torch
 import torch.nn.functional as F
+
+# module -> the restatement's own `record_hit`.  The product modules keep theirs on the device, where reading it costs a host
+# sync the reference does not make: it is read once per module, at the module's first update, and counted here from then on
+# (the module's own counter does not advance).
+_record_hit = weakref.WeakKeyDictionary()
 
 
 def _sync_usage(ema, margin):
     return (ema >= margin).float().mean().item() * 100       # the reference's host sync
+
+
+def _next_record_hit(mod):
+    """the reference's `record_hit` for this update, then `record_hit += 1`."""
+    rh = _record_hit.get(mod)
+    if rh is None:
+        rh = mod.record_hit
+    _record_hit[mod] = rh + 1
+    return rh
 
 
 def _ema_(ema_row, hit, record_hit):
@@ -49,8 +65,7 @@ def vq_forward(mod, z):
     usage = None
     if mod.training:
         hit = idx.bincount(minlength=mod.vocab_size).float()
-        _ema_(mod.ema_vocab_hit_SV, hit, mod.record_hit)
-        mod.record_hit += 1
+        _ema_(mod.ema_vocab_hit_SV, hit, _next_record_hit(mod))
         usage = _sync_usage(mod.ema_vocab_hit_SV, flat.shape[0] / mod.vocab_size * 0.08)
     commit = mod.beta * (zq.detach() - zt).pow(2).mean()
     vq = (zq - zt.detach()).pow(2).mean()
@@ -122,8 +137,7 @@ def vq2_forward(mod, f, dropout=None):
             fhat = fhat + h * mask
             rest = rest - h
             if mod.training:
-                _ema_(mod.ema_vocab_hit_SV[si], hit, mod.record_hit)
-                mod.record_hit += 1
+                _ema_(mod.ema_vocab_hit_SV[si], hit, _next_record_hit(mod))
             ratio = mask.sum() / B
             vq = vq + F.mse_loss(fhat, f_ng, reduction="none").mul(mask).mean() / ratio
             commit = commit + F.mse_loss(fhat.detach(), f, reduction="none").mul(mask).mul(mod.beta / ratio).mean()
@@ -166,8 +180,7 @@ def lfq_forward(mod, f, dropout):
             fhat = fhat + h * mask
             rest = rest - h
             if mod.training:
-                _ema_(mod.ema_vocab_hit_SV[si], hit, mod.record_hit)
-                mod.record_hit += 1
+                _ema_(mod.ema_vocab_hit_SV[si], hit, _next_record_hit(mod))
             ratio = mask.sum() / B
             zsel = x[mask.view(B)]                                         # INT-mask gather of batch rows 0 / 1
             p = torch.sigmoid(-4 * zsel * s)

@@ -634,42 +634,45 @@ def test_msvr_unscreened_seed_counts_mismatches_on_gpu():
 
 
 # ------------------------------------------------------------------------------------------
-# torch.library registration (SURVEY.md section 8b): torch.compile(fullgraph=True) and CUDA-graph capture
+# torch.library registration (SURVEY.md section 8b): the usage-EMA step counter on the device, torch.compile(fullgraph=True)
+# and CUDA-graph capture
 # ------------------------------------------------------------------------------------------
-def test_vq_custom_ops_compile_fullgraph_and_cuda_graph():
+def test_vq_library_ops_compile_fullgraph_and_cuda_graph():
     from imagefolder_b200 import VectorQuantizer
     rng = np.random.default_rng(5)
     V, C, B, hw = 512, 32, 4, 8
     E = (rng.standard_normal((V, C)) * 0.3).astype(np.float32)
     zs = [rng.standard_normal((B, C, hw, hw)).astype(np.float32) for _ in range(3)]
 
-    def make(custom):
+    def make():
         q = VectorQuantizer(V, C).cuda().train()
         q.embedding.weight.data.copy_(dev(E))
-        q.use_custom_ops = custom
         return q
 
-    # (1) eager custom-op path == autograd.Function path, bit for bit, over several steps (EMA schedule on the device counter)
-    qa, qb = make(False), make(True)
-    for z in zs:
-        za, zb = dev(z, grad=True), dev(z, grad=True)
+    # (1) three training steps against the oracle: indices and z_q bit for bit, gradients, the EMA schedule on the device counter
+    qa = make()
+    ema = np.zeros(V, np.float32)
+    margin = B * hw * hw / V * 0.08
+    for step, z in enumerate(zs):
+        za = dev(z, grad=True)
         oa, ua, va, ca, _ = qa(za)
-        ob, ub, vb, cb, _ = qb(zb)
         (oa.sum() * 0.3 + va + ca).backward()
-        (ob.sum() * 0.3 + vb + cb).backward()
-        assert torch.equal(oa, ob) and torch.equal(qa.last_idx, qb.last_idx) and float(va) == float(vb) and float(ca) == float(cb)
-        assert torch.equal(za.grad, zb.grad)
-        # the codebook gradient is a float atomic scatter-add: deterministic values, run-to-run summation order
-        assert torch.allclose(qa.embedding.weight.grad, qb.embedding.weight.grad, rtol=1e-5, atol=1e-8)
-        assert torch.equal(qa.ema_vocab_hit_SV, qb.ema_vocab_hit_SV) and float(ua[0]) == float(ub[0])
+        fwd = xo.vq_forward(z, E)
+        np.testing.assert_array_equal(npy(qa.last_idx), fwd["idx"])
+        np.testing.assert_array_equal(npy(oa), fwd["out"])
+        gz, gE = xo.vq_backward(fwd, E, np.full(z.shape, 0.3, np.float32), 1.0, 1.0, 0.25, True)
+        close(za.grad, gz, rtol=1e-4)
+        close(qa.embedding.weight.grad, gE, rtol=1e-4)
         qa.embedding.weight.grad = None
-        qb.embedding.weight.grad = None
-    assert int(qb._record_hit_dev[0]) == 3 and qa.record_hit == 3
+        ema = xo.ema_update(ema, np.bincount(fwd["idx"], minlength=V).astype(np.float32), step)
+        np.testing.assert_array_equal(npy(qa.ema_vocab_hit_SV), ema)
+        assert abs(float(ua[0]) - float((ema >= margin).mean() * 100)) < 1e-4
+    assert qa.record_hit == 3
 
     # (2) torch.compile(fullgraph=True): no graph breaks, same numbers
-    qc = make(True)
+    qc = make()
     fn = torch.compile(lambda zz: qc(zz)[0:4], fullgraph=True, backend="aot_eager")
-    qd = make(True)
+    qd = make()
     for z in zs:
         oc, uc, vc, cc = fn(dev(z, grad=True))
         od, ud, vd, cd, _ = qd(dev(z, grad=True))
@@ -677,7 +680,7 @@ def test_vq_custom_ops_compile_fullgraph_and_cuda_graph():
     assert torch.equal(qc.ema_vocab_hit_SV, qd.ema_vocab_hit_SV)
 
     # (3) CUDA-graph capture of forward + backward of the quantizer (static buffers; replay == eager)
-    qg = make(True)
+    qg = make()
     z_static = dev(zs[0], grad=True)
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -685,7 +688,7 @@ def test_vq_custom_ops_compile_fullgraph_and_cuda_graph():
         o, u, v, c, _ = qg(z_static)
         (o.sum() * 0.3 + v + c).backward()
     torch.cuda.current_stream().wait_stream(s)
-    qg2 = make(True)
+    qg2 = make()
     qg.load_state_dict(qg2.state_dict())
     qg._record_hit_dev.zero_()
     z_static.grad = None
@@ -694,7 +697,7 @@ def test_vq_custom_ops_compile_fullgraph_and_cuda_graph():
     with torch.cuda.graph(graph):
         o, u, v, c, _ = qg(z_static)
         (o.sum() * 0.3 + v + c).backward()
-    qe = make(True)
+    qe = make()
     for z in zs:
         z_static.data.copy_(dev(z))
         graph.replay()
@@ -706,3 +709,26 @@ def test_vq_custom_ops_compile_fullgraph_and_cuda_graph():
         assert torch.equal(o, oe) and float(v) == float(ve) and torch.equal(z_static.grad, ze.grad)
         assert torch.allclose(qg.embedding.weight.grad, qe.embedding.weight.grad, rtol=1e-5, atol=1e-8)
     assert torch.equal(qg.ema_vocab_hit_SV, qe.ema_vocab_hit_SV)
+
+
+def test_multiscale_usage_counter_crosses_the_schedule_boundary():
+    """one training forward of 4 scales from record_hit = 98: row i uses 98 + i, so rows 0-1 blend 0.9/0.1 and rows 2-3
+    blend 0.99/0.01, and the device counter advances by SN"""
+    from imagefolder_b200 import LFQ, VectorQuantizer2
+    pn = [1, 2, 3, 4]
+    B = 3
+    torch.manual_seed(0)
+    for q in (VectorQuantizer2(64, 8, v_patch_nums=pn, num_latent_tokens=16).cuda().train(),
+              LFQ(64, 6, v_patch_nums=pn, num_latent_tokens=16).cuda().train()):
+        V = q.vocab_size
+        ema0 = (torch.rand(len(pn), V, device="cuda") * 50).round()
+        q.ema_vocab_hit_SV.copy_(ema0)
+        q.record_hit = 98
+        q(torch.randn(B, q.Cvae, 4, 4, device="cuda"), ret_usages=True, dropout=torch.full((B,), len(pn) + 1))
+        for si in range(len(pn)):
+            hit = np.bincount(npy(q.last_idx_Bl[si]).reshape(-1), minlength=V).astype(np.float32)
+            want = xo.ema_update(npy(ema0[si]), hit, 98 + si)
+            np.testing.assert_array_equal(npy(q.ema_vocab_hit_SV[si]), want)
+            w = 0.9 if si < 2 else 0.99
+            close(q.ema_vocab_hit_SV[si], npy(ema0[si]) * w + hit * (1 - w), rtol=1e-6)
+        assert q.record_hit == 102
