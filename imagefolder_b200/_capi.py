@@ -16,6 +16,8 @@ LIB_PATH = os.path.join(_HERE, "lib", "libxqb200.so")
 XQ_MAX_SCALES = 32
 XQ_EMA_MAX_TENSORS = 1020      # entries of one xq_ema_update launch (include/xqb200.h)
 XQ_ADAMW_MAX_TENSORS = 584     # entries of one xq_adamw_step launch (include/xqb200.h)
+XQ_CLIP_MAX_TENSORS = 1360     # entries of one xq_grad_norm / xq_grad_scale table (include/xqb200.h)
+XQ_GRAD_NORM_CHUNK = 65536     # floats per partial of xq_grad_norm: torch's _foreach_norm chunk (csrc/clip_kernel.cu)
 XQ_METRIC_STRIP_ROWS = 32      # image rows per CTA of xq_recon_psnr_ssim (include/xqb200.h)
 
 XQ_MS_VQ_ZNORM, XQ_MS_VQ_L2, XQ_MS_BSQ, XQ_MS_BSQ_HARD = 0, 1, 2, 3
@@ -156,6 +158,13 @@ def lib() -> ctypes.CDLL:
     # AdamW step (csrc/adamw_kernel.cu): every array is a HOST array (of device pointers, sizes or per-tensor doubles)
     L.xq_adamw_step.restype = c_int
     L.xq_adamw_step.argtypes = [vp, vp, vp, vp, vp, vp, vp, c_int, c_double, c_double, c_double, c_double, c_double, vp]
+    # gradient-norm clipping (csrc/clip_kernel.cu): grad / numel are HOST arrays of device pointers and sizes
+    L.xq_grad_norm_workspace_bytes.restype = c_size_t
+    L.xq_grad_norm_workspace_bytes.argtypes = [c_int, vp]
+    L.xq_grad_norm.restype = c_int
+    L.xq_grad_norm.argtypes = [vp, vp, c_int, f32p, vp, c_size_t, vp]
+    L.xq_grad_scale.restype = c_int
+    L.xq_grad_scale.argtypes = [vp, vp, c_int, f32p, vp]
     # reconstruction metrics (csrc/metric_kernels.cu)
     L.xq_recon_psnr_ssim_workspace_bytes.restype = c_size_t
     L.xq_recon_psnr_ssim_workspace_bytes.argtypes = [c_int] * 4
@@ -243,5 +252,5 @@ EXPORTED_SYMBOLS = [
     "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd", "xq_vit_fc2_lora_dgelu_bwd",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
-    "xq_ema_update", "xq_adamw_step", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
+    "xq_ema_update", "xq_adamw_step", "xq_grad_norm_workspace_bytes", "xq_grad_norm", "xq_grad_scale", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
 ] + [n + "_f16" for n in F16_TWINS]

@@ -15,6 +15,8 @@ nvcc $FLAGS -c "$HERE/img_kernels.cu" -o "$OUT/img_kernels.o" "$@" &
 nvcc $FLAGS -c "$HERE/ema_kernel.cu" -o "$OUT/ema_kernel.o" "$@" &
 # AdamW step: the same, intrinsics throughout
 nvcc $FLAGS -c "$HERE/adamw_kernel.cu" -o "$OUT/adamw_kernel.o" "$@" &
+# gradient-norm clipping: the same, intrinsics throughout
+nvcc $FLAGS -c "$HERE/clip_kernel.cu" -o "$OUT/clip_kernel.o" "$@" &
 # PSNR / SSIM: every step of scikit-image's fp32 arithmetic, uncontracted
 nvcc $FLAGS -c "$HERE/metric_kernels.cu" -o "$OUT/metric_kernels.o" "$@" &
 # ViT glue kernels carry no index decisions: default contraction (-fmad=true)
@@ -23,5 +25,5 @@ nvcc ${FLAGS/-fmad=false/} -c "$HERE/loss_kernels.cu" -o "$OUT/loss_kernels.o" "
 nvcc ${FLAGS/-fmad=false/} -c "$HERE/attn_kernel.cu" -o "$OUT/attn_kernel.o" "$@" &
 nvcc ${FLAGS/-fmad=false/} -c "$HERE/gemm_kernel.cu" -o "$OUT/gemm_kernel.o" "$@" &
 for job in $(jobs -p); do wait "$job"; done     # a failed compile stops the build (a bare `wait` would ignore it)
-nvcc $ARCH -shared -o "$OUT/libxqb200.so" "$OUT/vq_kernels.o" "$OUT/vq_tc_kernel.o" "$OUT/ms_kernels.o" "$OUT/vit_kernels.o" "$OUT/loss_kernels.o" "$OUT/attn_kernel.o" "$OUT/gemm_kernel.o" "$OUT/img_kernels.o" "$OUT/ema_kernel.o" "$OUT/adamw_kernel.o" "$OUT/metric_kernels.o" -lcudart
+nvcc $ARCH -shared -o "$OUT/libxqb200.so" "$OUT/vq_kernels.o" "$OUT/vq_tc_kernel.o" "$OUT/ms_kernels.o" "$OUT/vit_kernels.o" "$OUT/loss_kernels.o" "$OUT/attn_kernel.o" "$OUT/gemm_kernel.o" "$OUT/img_kernels.o" "$OUT/ema_kernel.o" "$OUT/adamw_kernel.o" "$OUT/clip_kernel.o" "$OUT/metric_kernels.o" -lcudart
 echo "$OUT/libxqb200.so"

@@ -1,9 +1,10 @@
-// xq_chunks.cuh -- the tensor-table walk shared by the multi-tensor elementwise kernels (ema_kernel.cu, adamw_kernel.cu).
+// xq_chunks.cuh -- the tensor-table walk shared by the multi-tensor kernels (ema_kernel.cu, adamw_kernel.cu, clip_kernel.cu).
 //
 // A call hands a host table of tensors to one launch through the kernel's parameter space (__grid_constant__, up to
-// 32 764 bytes on sm_90 with CUDA >= 12.1), so there is no host-to-device copy.  Every tensor is cut into 64 KiB chunks; a
-// persistent grid takes the chunks in a grid stride and finds each chunk's tensor by a binary search over the inclusive
-// chunk prefix.  CHUNK is a multiple of 4, so a tensor whose base is 16-byte aligned stays float4-aligned in every chunk.
+// 32 764 bytes on sm_90 with CUDA >= 12.1), so there is no host-to-device copy.  Every tensor is cut into chunks of CH floats
+// (CHUNK = 64 KiB by default; the gradient norm uses torch's 65 536-float chunk); a persistent grid takes the chunks in a grid
+// stride and finds each chunk's tensor by a binary search over the inclusive chunk prefix.  CH is a multiple of 4, so a tensor
+// whose base is 16-byte aligned stays float4-aligned in every chunk.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,6 +24,7 @@ struct Chunk {
 };
 
 // chunk c of a table whose tensors 0..i hold chunk_end[i] chunks together
+template <int CH = CHUNK>
 __device__ __forceinline__ Chunk locate_chunk(const int64_t *chunk_end, const int64_t *numel, int n, int64_t c) {
     int lo = 0, hi = n - 1;                  // first tensor whose chunk_end exceeds c
     while (lo < hi) {
@@ -33,16 +35,18 @@ __device__ __forceinline__ Chunk locate_chunk(const int64_t *chunk_end, const in
     const int64_t first = lo ? chunk_end[lo - 1] : 0;
     Chunk k;
     k.t = lo;
-    k.start = (c - first) * CHUNK;
-    k.count = (int)min((int64_t)CHUNK, numel[lo] - k.start);
+    k.start = (c - first) * CH;
+    k.count = (int)min((int64_t)CH, numel[lo] - k.start);
     return k;
 }
 
 // inclusive chunk prefix of n tensors; returns the total number of chunks
+template <int CH = CHUNK>
 static inline int64_t chunk_prefix(const int64_t *numel, int n, int64_t *chunk_end) {
+    static_assert(CH % 4 == 0, "a chunk must keep float4 alignment");
     int64_t chunks = 0;
     for (int j = 0; j < n; ++j) {
-        chunks += (numel[j] + CHUNK - 1) / CHUNK;
+        chunks += (numel[j] + CH - 1) / CH;
         chunk_end[j] = chunks;
     }
     return chunks;

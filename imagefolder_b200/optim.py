@@ -10,17 +10,25 @@ param, grad and both moments, with the same bits:
 
 The class keeps torch's constructor, `param_groups`, `state` layout and `state_dict` / `load_state_dict`, so checkpoints move
 both ways between it and torch.optim.AdamW, and LR schedulers that write `group['lr']` work unchanged.
+
+With --max_grad_norm set, the trainer clips between `scaler.unscale_` and `scaler.step` (:456-458, 471-473).
+`clip_grad_norm_` is torch.nn.utils.clip_grad_norm_ with the same signature, return value and bits; its two passes over the
+grads are csrc/clip_kernel.cu launches instead of torch's foreach chains:
+
+    from imagefolder_b200.optim import clip_grad_norm_  # instead of: torch.nn.utils.clip_grad_norm_
 """
 from __future__ import annotations
 
 import math
+import types
+import warnings
 
 import numpy as np
 import torch
 
 from . import _capi
 
-__all__ = ["AdamW"]
+__all__ = ["AdamW", "clip_grad_norm_"]
 
 _UNSUPPORTED = ("amsgrad", "maximize", "capturable", "differentiable")
 
@@ -148,3 +156,90 @@ class AdamW(torch.optim.AdamW):
             # the kernel writes through raw pointers: bump the version counters as torch's in-place foreach ops do
             torch.autograd.graph.increment_version(ps + ms + vs)
         return loss
+
+
+def _clip_tables(numels):
+    """(start, stop, launches of xq_grad_norm, launches of xq_grad_scale) of each XQ_CLIP_MAX_TENSORS-entry table of a call"""
+    T = _capi.XQ_CLIP_MAX_TENSORS
+    tables = []
+    for i0 in range(0, len(numels), T):
+        nonempty = any(int(k) > 0 for k in numels[i0:i0 + T])
+        tables.append((i0, min(i0 + T, len(numels)), 1 + nonempty, int(nonempty)))
+    return tables
+
+
+def _check_grads(grads):
+    """the device of `grads`, after refusing anything the kernels do not reproduce; nothing is written"""
+    for i, g in enumerate(grads):
+        if g.is_sparse or g.layout != torch.strided:
+            raise ValueError(f"clip_grad_norm_: grad {i}: sparse grads are not supported")
+        if g.dtype != torch.float32:
+            raise ValueError(f"clip_grad_norm_: grad {i}: fp32 grads are required (got {g.dtype})")
+        if not g.is_contiguous():
+            raise ValueError(f"clip_grad_norm_: grad {i}: contiguous grads are required")
+    for i, g in enumerate(grads):
+        if not g.is_cuda:
+            raise _capi.XqError(f"clip_grad_norm_: grad {i}: CUDA tensors are required, there is no CPU path "
+                                f"(grad on {g.device})")
+        if g.device != grads[0].device:
+            raise ValueError(f"clip_grad_norm_: grad {i} is on {g.device}, expected {grads[0].device}: one device "
+                             "per call")
+    return grads[0].device
+
+
+@torch.no_grad()
+def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=False, foreach=None):
+    """torch.nn.utils.clip_grad_norm_ (torch 2.11) for fp32 CUDA grads on one device, with the same bits.
+
+    The per-tensor norms are one xq_grad_norm call (bit-identical to torch._foreach_norm), the total norm and the clip
+    coefficient are torch's own ops on them, and the grads are scaled by one xq_grad_scale call that reads the coefficient on
+    the device, so nothing synchronises unless `error_if_nonfinite` asks to.  Returns the total norm, as torch does.
+
+    Raises before anything is written on norm_type != 2, foreach=False, non-fp32, sparse or non-contiguous grads, grads on more
+    than one device, and CPU grads (_capi.XqError: there is no CPU path)."""
+    if isinstance(parameters, torch.Tensor):
+        parameters = [parameters]
+    else:
+        is_generator = isinstance(parameters, types.GeneratorType)
+        parameters = list(parameters)                  # a generator is consumed once
+        if is_generator and len(parameters) == 0:
+            warnings.warn("`parameters` is an empty generator, no gradient clipping will occur.", stacklevel=3)
+    grads = [p.grad for p in parameters if p.grad is not None]
+    norm_type = float(norm_type)
+    if norm_type != 2.0:
+        raise ValueError(f"clip_grad_norm_: norm_type {norm_type} is not supported; the kernels reproduce the L2 norm")
+    if foreach is False:
+        raise ValueError("clip_grad_norm_: foreach=False (torch's per-tensor vector_norm loop) rounds differently; the kernels "
+                         "reproduce the foreach implementation that torch picks for CUDA grads by default")
+    if len(grads) == 0:
+        return torch.tensor(0.0)
+    max_norm = float(max_norm)
+    device = _check_grads(grads)
+    ptrs = np.array([g.data_ptr() for g in grads], dtype=np.uint64)
+    numel = np.array([g.numel() for g in grads], dtype=np.int64)
+    n = len(grads)
+    tables = _clip_tables(numel)
+    L = _capi.lib()
+    with torch.cuda.device(device):
+        stream = _capi.stream_ptr(device)
+        ws_bytes = L.xq_grad_norm_workspace_bytes(n, numel.ctypes.data)
+        ws = _capi.workspace(ws_bytes, device)
+        norms = torch.empty(n, dtype=torch.float32, device=device)    # what torch.stack(torch._foreach_norm(grads)) holds
+        _capi.call("xq_grad_norm", sum(t[2] for t in tables), L.xq_grad_norm, ptrs.ctypes.data, numel.ctypes.data, n,
+                   norms.data_ptr(), ws.data_ptr(), ws.numel(), stream, nbytes=4 * int(numel.sum()))
+        # torch/nn/utils/clip_grad.py, _get_total_norm and _clip_grads_with_norm_, op for op
+        total_norm = torch.linalg.vector_norm(norms, norm_type)
+        if error_if_nonfinite and torch.logical_or(total_norm.isnan(), total_norm.isinf()):
+            raise RuntimeError(
+                f"The total norm of order {norm_type} for gradients from "
+                "`parameters` is non-finite, so it cannot be clipped. To disable "
+                "this error and scale the gradients by the non-finite norm anyway, "
+                "set `error_if_nonfinite=False`"
+            )
+        clip_coef = max_norm / (total_norm + 1e-6)
+        clip_coef_clamped = torch.clamp(clip_coef, max=1.0)
+        _capi.call("xq_grad_scale", sum(t[3] for t in tables), L.xq_grad_scale, ptrs.ctypes.data, numel.ctypes.data, n,
+                   clip_coef_clamped.data_ptr(), stream, nbytes=8 * int(numel.sum()))
+    # the kernel writes through raw pointers: bump the version counters as torch's in-place _foreach_mul_ does
+    torch.autograd.graph.increment_version(grads)
+    return total_norm

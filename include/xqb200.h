@@ -423,6 +423,28 @@ int xq_adamw_step(float *const *param, const float *const *grad, float *const *e
                   const int64_t *numel, const double *step_size, const double *bc2_sqrt, int n, double wd_factor,
                   double one_minus_beta1, double beta2, double one_minus_beta2, double eps, void *stream);
 
+/* ---- gradient-norm clipping of the trainer (csrc/clip_kernel.cu) ----------------------------------------------------------
+ * The two streaming passes of torch.nn.utils.clip_grad_norm_(params, max_norm) (xqgan_train.py:456-458, 471-473, with
+ * --max_grad_norm set); the steps between them are torch's own ops on `norms` (imagefolder_b200/optim.py::clip_grad_norm_).
+ *
+ * xq_grad_norm: norms[i] = ||grad[i]||_2 for i < n, fp32, bit-identical to torch.stack(torch._foreach_norm(grads)) on the same
+ *   GPU (the same per-chunk partials, trees and sqrt).  norms is a device array of n floats (4-byte aligned); entries with
+ *   numel 0 get 0.  The per-chunk partials go to the caller's workspace of xq_grad_norm_workspace_bytes(n, numel) bytes.
+ *   Two launches per XQ_CLIP_MAX_TENSORS entries (chunk partials, then one block per tensor), in order, on `stream`.
+ * xq_grad_scale: grad[i][k] <- grad[i][k] * (*coef) for i < n, k < numel[i]: torch's _foreach_mul_(grads, coef) with coef a
+ *   0-dim fp32 device tensor, read on the device (the host never synchronises).  One launch per XQ_CLIP_MAX_TENSORS entries.
+ *   grad, numel   HOST arrays of n entries; the pointers in grad are fp32 device pointers (4-byte aligned).
+ * n == 0 is a no-op; entries with numel 0 are not read (their pointers may be NULL).  Every entry is validated before the first
+ * launch, so XQ_ERR_ARG (n < 0, NULL arrays, a negative numel, a NULL or misaligned pointer) and XQ_ERR_WORKSPACE mean nothing
+ * was written.
+ * ------------------------------------------------------------------------------------------------------------------------------ */
+#define XQ_CLIP_MAX_TENSORS 1360
+/* bytes of the partial-sum workspace of xq_grad_norm (4 per 65 536-float chunk); 0 when an argument is out of range */
+size_t xq_grad_norm_workspace_bytes(int n, const int64_t *numel);
+int xq_grad_norm(const float *const *grad, const int64_t *numel, int n, float *norms, void *workspace, size_t workspace_bytes,
+                 void *stream);
+int xq_grad_scale(float *const *grad, const int64_t *numel, int n, const float *coef, void *stream);
+
 /* ---- reconstruction metrics: PSNR and SSIM per image (csrc/metric_kernels.cu) ---------------------------------------------
  * Replaces the scikit-image calls of the reference's reconstruction evaluation (tokenizer/vqgan/reconstruction_vqgan_ddp.py:
  * 155-169), per image b of rec [B,C,H,W] (the clamped reconstruction, fp32, or bf16 when rec_is_bf16) and x [B,C,H,W] fp32 (the
