@@ -27,8 +27,10 @@
 // Each step is written with intrinsics, so the -fmad flag of this translation unit cannot change it.  step_size = -(lr / (1 - beta1**t)) and bc2_sqrt = (1 - beta2**t) ** 0.5 are evaluated by the caller in
 // Python doubles, per tensor, because a parameter whose grad is None skips a step and its count falls behind.
 //
-// Work split: the table walk of xq_chunks.cuh, as in ema_kernel.cu; float4 streaming accesses when all four bases are
-// 16-byte aligned, scalar code otherwise.
+// Work split: the table and chunk walk of xq_chunks.cuh, as in ema_kernel.cu: two float4 quadruples in flight per thread when
+// all four bases are 16-byte aligned, four floats otherwise.  The loop is this kernel's own, not xqc::stream_table: that
+// routine hands its op a copy of the loaded values, and this op updates the loaded values in place; moved there, either form
+// changes the register allocation of one of the kernels (78 registers each today).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -38,25 +40,18 @@
 
 namespace xqa {
 
-using xqc::CHUNK;
 using xqc::THREADS;
 constexpr int U4 = 2;                        // float4 quadruples in flight per thread (4 x 32 B)
 constexpr int U1 = 4;                        // floats in flight per thread on the scalar path
 constexpr int TABLE = XQ_ADAMW_MAX_TENSORS;
 
-struct AdamwTable {
-    float *p[TABLE];
-    const float *g[TABLE];
-    float *m[TABLE];
-    float *v[TABLE];
-    int64_t numel[TABLE];
-    int64_t chunk_end[TABLE];                // chunks of tensors 0..i (inclusive prefix)
-    float step_size[TABLE];                  // -(lr / (1 - beta1**t)) of tensor i
-    float bc2_sqrt[TABLE];                   // (1 - beta2**t) ** 0.5 of tensor i
-    int n;
+struct Scalars {
     int decay;                               // multiply p by wd_factor first
     float wd_factor, w, beta2, c, eps;       // 1 - lr*wd, 1 - beta1, beta2, 1 - beta2, eps
+    float step_size[TABLE];                  // -(lr / (1 - beta1**t)) of tensor i
+    float bc2_sqrt[TABLE];                   // (1 - beta2**t) ** 0.5 of tensor i
 };
+using AdamwTable = xqc::Table<4, TABLE, Scalars>;   // arrays: p, g, m, v; all but g written
 static_assert(sizeof(AdamwTable) <= xqc::PARAM_BYTES, "the tensor table must fit in the kernel parameter space");
 
 struct Hyper {
@@ -82,28 +77,29 @@ __device__ __forceinline__ void adamw_op4(float4 &p, float4 g, float4 &m, float4
 }
 
 __global__ void __launch_bounds__(THREADS) adamw_step_kernel(const __grid_constant__ AdamwTable tab) {
+    const Scalars &sc = tab.own;
     const int tid = threadIdx.x;
     const int64_t nchunks = tab.chunk_end[tab.n - 1];
     Hyper h;
-    h.decay = tab.decay != 0;
-    h.wd_factor = tab.wd_factor;
-    h.w = tab.w;
-    h.omw = __fsub_rn(1.0f, tab.w);
-    h.small_w = fabsf(tab.w) < 0.5f;
-    h.beta2 = tab.beta2;
-    h.c = tab.c;
-    h.unit_c = tab.c == 1.0f;
-    h.eps = tab.eps;
+    h.decay = sc.decay != 0;
+    h.wd_factor = sc.wd_factor;
+    h.w = sc.w;
+    h.omw = __fsub_rn(1.0f, sc.w);
+    h.small_w = fabsf(sc.w) < 0.5f;
+    h.beta2 = sc.beta2;
+    h.c = sc.c;
+    h.unit_c = sc.c == 1.0f;
+    h.eps = sc.eps;
     for (int64_t c = blockIdx.x; c < nchunks; c += gridDim.x) {
         const xqc::Chunk k = xqc::locate_chunk(tab.chunk_end, tab.numel, tab.n, c);
         const int count = k.count;
-        h.ss = tab.step_size[k.t];
-        h.bc2 = tab.bc2_sqrt[k.t];
-        float *p = tab.p[k.t] + k.start;
-        const float *g = tab.g[k.t] + k.start;
-        float *m = tab.m[k.t] + k.start;
-        float *v = tab.v[k.t] + k.start;
-        if ((((uintptr_t)tab.p[k.t] | (uintptr_t)tab.g[k.t] | (uintptr_t)tab.m[k.t] | (uintptr_t)tab.v[k.t]) & 15) == 0) {
+        h.ss = sc.step_size[k.t];
+        h.bc2 = sc.bc2_sqrt[k.t];
+        float *p = tab.x[0][k.t] + k.start;
+        const float *g = tab.x[1][k.t] + k.start;
+        float *m = tab.x[2][k.t] + k.start;
+        float *v = tab.x[3][k.t] + k.start;
+        if ((((uintptr_t)tab.x[0][k.t] | (uintptr_t)tab.x[1][k.t] | (uintptr_t)tab.x[2][k.t] | (uintptr_t)tab.x[3][k.t]) & 15) == 0) {
             float4 *p4 = reinterpret_cast<float4 *>(p);
             const float4 *g4 = reinterpret_cast<const float4 *>(g);
             float4 *m4 = reinterpret_cast<float4 *>(m);
@@ -167,8 +163,6 @@ __global__ void __launch_bounds__(THREADS) adamw_step_kernel(const __grid_consta
     }
 }
 
-static bool bad_ptr(const void *q) { return !q || ((uintptr_t)q & 3); }
-
 }  // namespace xqa
 
 using namespace xqa;
@@ -180,47 +174,30 @@ int xq_adamw_step(float *const *param, const float *const *grad, float *const *e
                   double one_minus_beta1, double beta2, double one_minus_beta2, double eps, void *stream) {
     if (n < 0) return XQ_ERR_ARG;
     if (n == 0) return XQ_OK;
-    if (!param || !grad || !exp_avg || !exp_avg_sq || !numel || !step_size || !bc2_sqrt) return XQ_ERR_ARG;
+    if (!step_size || !bc2_sqrt) return XQ_ERR_ARG;
     for (double x : {wd_factor, one_minus_beta1, beta2, one_minus_beta2, eps})
         if (!std::isfinite(x)) return XQ_ERR_ARG;
-    bool any = false;
-    for (int i = 0; i < n; ++i) {            // every entry is checked before the first launch: a refused call writes nothing
-        if (numel[i] < 0) return XQ_ERR_ARG;
-        if (numel[i] == 0) continue;
-        if (bad_ptr(param[i]) || bad_ptr(grad[i]) || bad_ptr(exp_avg[i]) || bad_ptr(exp_avg_sq[i])) return XQ_ERR_ARG;
-        if (!std::isfinite(step_size[i]) || !std::isfinite(bc2_sqrt[i])) return XQ_ERR_ARG;
-        any = true;
-    }
-    if (!any) return XQ_OK;
-    int max_grid = 0;
-    const int rc = xq::persistent_grid(adamw_step_kernel, THREADS, &max_grid);
-    if (rc != XQ_OK) return rc;
+    int64_t chunks = 0;                      // every entry is checked before the first launch: a refused call writes nothing
+    if (xqc::check_entries({param, grad, exp_avg, exp_avg_sq}, numel, n, &chunks) != XQ_OK) return XQ_ERR_ARG;
+    for (int i = 0; i < n; ++i)
+        if (numel[i] > 0 && (!std::isfinite(step_size[i]) || !std::isfinite(bc2_sqrt[i]))) return XQ_ERR_ARG;
+    if (chunks == 0) return XQ_OK;
     AdamwTable tab;
+    Scalars &sc = tab.own;
     // each scalar rounded once to fp32, as the foreach kernels receive it
-    tab.decay = wd_factor != 1.0;            // weight_decay == 0 (torch skips the multiply), or a multiply by 1, which is exact
-    tab.wd_factor = (float)wd_factor;
-    tab.w = (float)one_minus_beta1;
-    tab.beta2 = (float)beta2;
-    tab.c = (float)one_minus_beta2;
-    tab.eps = (float)eps;
-    for (int i0 = 0; i0 < n; i0 += TABLE) {
-        tab.n = n - i0 < TABLE ? n - i0 : TABLE;
-        for (int j = 0; j < tab.n; ++j) {
-            tab.p[j] = param[i0 + j];
-            tab.g[j] = grad[i0 + j];
-            tab.m[j] = exp_avg[i0 + j];
-            tab.v[j] = exp_avg_sq[i0 + j];
-            tab.numel[j] = numel[i0 + j];
-            tab.step_size[j] = (float)step_size[i0 + j];
-            tab.bc2_sqrt[j] = (float)bc2_sqrt[i0 + j];
-        }
-        const int64_t chunks = xqc::chunk_prefix(tab.numel, tab.n, tab.chunk_end);
-        if (chunks == 0) continue;
-        const unsigned grid = (unsigned)(chunks < max_grid ? chunks : max_grid);
-        adamw_step_kernel<<<grid, THREADS, 0, (cudaStream_t)stream>>>(tab);
-        XQ_LAUNCH_CHECK("adamw_step_kernel");
-    }
-    return XQ_OK;
+    sc.decay = wd_factor != 1.0;             // weight_decay == 0 (torch skips the multiply), or a multiply by 1, which is exact
+    sc.wd_factor = (float)wd_factor;
+    sc.w = (float)one_minus_beta1;
+    sc.beta2 = (float)beta2;
+    sc.c = (float)one_minus_beta2;
+    sc.eps = (float)eps;
+    return xqc::launch_tables(adamw_step_kernel, THREADS, "adamw_step_kernel", tab, {param, grad, exp_avg, exp_avg_sq}, numel,
+                              n, stream, [&](int i0) {
+                                  for (int j = 0; j < tab.n; ++j) {
+                                      sc.step_size[j] = (float)step_size[i0 + j];
+                                      sc.bc2_sqrt[j] = (float)bc2_sqrt[i0 + j];
+                                  }
+                              });
 }
 
 }  // extern "C"
