@@ -47,6 +47,8 @@ F16_TWINS = [
     "xq_vit_attn_fwd", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd",
     "xq_vit_fc2_lora_dgelu_bwd",
 ]
+# the SwiGLU entry points of the giant backbones' MLP, with `_f16` twins in the same sense
+SWIGLU_ENTRIES = ["xq_vit_swiglu_fwd", "xq_vit_swiglu_bwd", "xq_vit_fc1_swiglu_fwd", "xq_vit_fc2_dswiglu_bwd"]
 
 
 def lib() -> ctypes.CDLL:
@@ -130,8 +132,16 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_fc1_lora_gelu_fwd.argtypes = [vp, vp, vp, vp, f32p, vp, vp, c_int, c_int, c_int, c_int, vp]
     L.xq_vit_fc2_lora_dgelu_bwd.restype = c_int
     L.xq_vit_fc2_lora_dgelu_bwd.argtypes = [vp, vp, vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, c_int, vp]
+    L.xq_vit_swiglu_fwd.restype = c_int
+    L.xq_vit_swiglu_fwd.argtypes = [vp, f32p, vp, c_int, c_int, vp]
+    L.xq_vit_swiglu_bwd.restype = c_int
+    L.xq_vit_swiglu_bwd.argtypes = [vp, f32p, vp, vp, f32p, c_int, c_int, vp]
+    L.xq_vit_fc1_swiglu_fwd.restype = c_int
+    L.xq_vit_fc1_swiglu_fwd.argtypes = [vp, vp, f32p, vp, vp, c_int, c_int, c_int, vp]
+    L.xq_vit_fc2_dswiglu_bwd.restype = c_int
+    L.xq_vit_fc2_dswiglu_bwd.argtypes = [vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, vp]
     # fp16 twins of the 16-bit ViT entry points: the same argument lists
-    for name in F16_TWINS:
+    for name in F16_TWINS + SWIGLU_ENTRIES:
         twin = getattr(L, name + "_f16")
         twin.restype = c_int
         twin.argtypes = getattr(L, name).argtypes
@@ -253,4 +263,4 @@ EXPORTED_SYMBOLS = [
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
     "xq_ema_update", "xq_adamw_step", "xq_grad_norm_workspace_bytes", "xq_grad_norm", "xq_grad_scale", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
-] + [n + "_f16" for n in F16_TWINS]
+] + [n + "_f16" for n in F16_TWINS] + SWIGLU_ENTRIES + [n + "_f16" for n in SWIGLU_ENTRIES]

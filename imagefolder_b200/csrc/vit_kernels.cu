@@ -11,6 +11,7 @@
 //   residual_ln_bwd : G = g_xnew + LN^T(g_y);  g_branch = G * rowscale * gamma_ls -> bf16;
 //                     d ln_w, d ln_b, d gamma_ls column sums (per-CTA partials, reduced deterministically)
 //   gelu_fwd / gelu_bwd : exact (erf) GELU on bf16, 16-byte vectors
+//   swiglu_fwd / swiglu_bwd : SwiGLU of timm's GluMlp (the giant backbones' MLP) on the same 16-byte vectors
 //
 // Algorithmic bytes per element (row x channel): fwd 4 (x) + 2 (branch) + 4 (x_new) + 2 (y) = 12 B;
 // bwd 4 (g_xnew) + 2 (g_y) + 4 (x_new) + 2 (branch) + 4 (G) + 2 (g_branch) = 18 B.
@@ -138,7 +139,11 @@ constexpr int NACC = 4;
 constexpr int LNB_TR = 8;
 constexpr int LNB_THREADS = (LNB_TR + 1) * 32;
 __host__ __device__ inline size_t lnb_stage_bytes(int D) { return (size_t)LNB_TR * D * 12 + 128; }
-__host__ __device__ inline int lnb_stages(int D) { return lnb_stage_bytes(D) * 3 <= 225 * 1024 ? 3 : 2; }
+// D = 1536 (ViT-g): one stage of 8 rows is 144 KB, so two do not fit and the producer refills the single stage only once
+// every consumer has released it
+__host__ __device__ inline int lnb_stages(int D) {
+    return lnb_stage_bytes(D) * 3 <= 225 * 1024 ? 3 : (lnb_stage_bytes(D) * 2 <= 225 * 1024 ? 2 : 1);
+}
 
 template <typename E, int NV>
 __global__ void __launch_bounds__(LNB_THREADS, 1)
@@ -431,6 +436,74 @@ __global__ void gelu_bwd_kernel(const uint4 *__restrict__ x, const float *__rest
     }
 }
 
+// SwiGLU of timm's GluMlp (gate_last=False) on the fc1 GEMM output WITHOUT its bias, pre [M, 2H] (gate columns [0, H), up
+// columns [H, 2H)), bias fp32 [2H]:  act[:, j] = silu(pre[:, j] + b[j]) * (pre[:, H+j] + b[H+j]), rounded once.
+// Same layout of work as gelu_fwd_kernel: a thread owns the 8-column chunk c of act (and of both halves of pre).
+template <typename E>
+__global__ void swiglu_fwd_kernel(const uint4 *__restrict__ pre, const float *__restrict__ bias, uint4 *__restrict__ act,
+                                  int M, int H8) {
+    const int row0 = blockIdx.x * GELU_RU;
+    for (int c = threadIdx.x; c < H8; c += blockDim.x) {
+        float ba[8], bc[8];
+        load_bias8(bias, c, ba);
+        load_bias8(bias ? bias + 8 * H8 : nullptr, c, bc);
+        uint4 va[GELU_RU], vc[GELU_RU];
+#pragma unroll
+        for (int u = 0; u < GELU_RU; ++u)
+            if (row0 + u < M) { va[u] = pre[(size_t)(row0 + u) * 2 * H8 + c]; vc[u] = pre[(size_t)(row0 + u) * 2 * H8 + H8 + c]; }
+#pragma unroll
+        for (int u = 0; u < GELU_RU; ++u) {
+            if (row0 + u >= M) continue;
+            typename E::T2 *p = reinterpret_cast<typename E::T2 *>(&va[u]);
+            const typename E::T2 *q = reinterpret_cast<const typename E::T2 *>(&vc[u]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float2 a = E::to2(p[k]), cc = E::to2(q[k]);
+                p[k] = E::from2(swiglu_f(a.x + ba[2 * k], cc.x + bc[2 * k]), swiglu_f(a.y + ba[2 * k + 1], cc.y + bc[2 * k + 1]));
+            }
+            act[(size_t)(row0 + u) * H8 + c] = va[u];
+        }
+    }
+}
+
+// d_pre[:, j] = g silu'(a) c, d_pre[:, H+j] = g silu(a) (each rounded once, g = g_act); column sums of the ROUNDED d_pre
+// (= d bias [2H]) per thread, one atomicAdd per column per CTA at the end (g_bias zeroed by the caller).  Persistent, like
+// gelu_bwd_kernel, so that the sums stay in registers.
+template <typename E>
+__global__ void swiglu_bwd_kernel(const uint4 *__restrict__ pre, const float *__restrict__ bias, const uint4 *__restrict__ gy,
+                                  uint4 *__restrict__ d_pre, float *__restrict__ g_bias, int M, int H8) {
+    for (int c = threadIdx.x; c < H8; c += blockDim.x) {
+        float ba[8], bc[8], sa[8] = {}, sc[8] = {};
+        load_bias8(bias, c, ba);
+        load_bias8(bias ? bias + 8 * H8 : nullptr, c, bc);
+        for (int row = blockIdx.x; row < M; row += gridDim.x) {
+            uint4 va = pre[(size_t)row * 2 * H8 + c], vc = pre[(size_t)row * 2 * H8 + H8 + c];
+            const uint4 vg = gy[(size_t)row * H8 + c];
+            typename E::T2 *p = reinterpret_cast<typename E::T2 *>(&va);
+            typename E::T2 *q = reinterpret_cast<typename E::T2 *>(&vc);
+            const typename E::T2 *h = reinterpret_cast<const typename E::T2 *>(&vg);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float2 a = E::to2(p[k]), cc = E::to2(q[k]), g = E::to2(h[k]);
+                float da0, dc0, da1, dc1;
+                dswiglu_f(g.x, a.x + ba[2 * k], cc.x + bc[2 * k], da0, dc0);
+                dswiglu_f(g.y, a.y + ba[2 * k + 1], cc.y + bc[2 * k + 1], da1, dc1);
+                p[k] = E::from2(da0, da1);
+                q[k] = E::from2(dc0, dc1);
+                const float2 ra = E::to2(p[k]), rc = E::to2(q[k]);
+                sa[2 * k] += ra.x; sa[2 * k + 1] += ra.y;
+                sc[2 * k] += rc.x; sc[2 * k + 1] += rc.y;
+            }
+            d_pre[(size_t)row * 2 * H8 + c] = va;
+            d_pre[(size_t)row * 2 * H8 + H8 + c] = vc;
+        }
+        if (g_bias) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) { atomicAdd(g_bias + c * 8 + k, sa[k]); atomicAdd(g_bias + 8 * H8 + c * 8 + k, sc[k]); }
+        }
+    }
+}
+
 // Patch embedding as a GEMM (timm PatchEmbed: Conv2d(kernel = stride = p) -> flatten -> NLC, vision_transformer.py:
 // patch_embed): non-overlapping patches make im2col a pure permutation, so the conv is
 //   tokens[B*gh*gw, D] = patches[B*gh*gw, Cin*p*p] @ W[D, Cin*p*p]^T + b .
@@ -519,6 +592,7 @@ using namespace xqv;
         case 384: { constexpr int NV = 3; __VA_ARGS__; break; }   \
         case 768: { constexpr int NV = 6; __VA_ARGS__; break; }   \
         case 1024: { constexpr int NV = 8; __VA_ARGS__; break; }  \
+        case 1536: { constexpr int NV = 12; __VA_ARGS__; break; } \
         default: return XQ_ERR_UNSUPPORTED;    \
     }
 
@@ -610,6 +684,32 @@ static int gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, 
     if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, sizeof(float) * (size_t)C, st));
     gelu_bwd_kernel<E><<<grid, threads, 0, st>>>((const uint4 *)x, bias, (const uint4 *)gy, (uint4 *)gx, g_bias, M, C8);
     XQ_LAUNCH_CHECK("gelu_bwd_kernel");
+    return XQ_OK;
+}
+
+template <typename E>
+static int swiglu_fwd(const void *pre, const float *bias, void *act, int M, int H, void *stream) {
+    if (!pre || !act || M <= 0 || H <= 0 || (H & 7)) return XQ_ERR_ARG;
+    const int H8 = H / 8;
+    const int threads = H8 >= 384 ? 384 : (H8 >= 192 ? 192 : 128);
+    swiglu_fwd_kernel<E><<<(M + GELU_RU - 1) / GELU_RU, threads, 0, (cudaStream_t)stream>>>((const uint4 *)pre, bias, (uint4 *)act,
+                                                                                           M, H8);
+    XQ_LAUNCH_CHECK("swiglu_fwd_kernel");
+    return XQ_OK;
+}
+
+template <typename E>
+static int swiglu_bwd(const void *pre, const float *bias, const void *gy, void *d_pre, float *g_bias, int M, int H, void *stream) {
+    if (!pre || !gy || !d_pre || M <= 0 || H <= 0 || (H & 7)) return XQ_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H8 = H / 8;
+    const int threads = H8 >= 384 ? 384 : (H8 >= 192 ? 192 : 128);
+    int grid = 0;
+    if (int rc = xq::persistent_grid(swiglu_bwd_kernel<E>, threads, &grid)) return rc;
+    if (M < grid) grid = M;
+    if (g_bias) XQ_CUDA_TRY(cudaMemsetAsync(g_bias, 0, sizeof(float) * 2 * (size_t)H, st));
+    swiglu_bwd_kernel<E><<<grid, threads, 0, st>>>((const uint4 *)pre, bias, (const uint4 *)gy, (uint4 *)d_pre, g_bias, M, H8);
+    XQ_LAUNCH_CHECK("swiglu_bwd_kernel");
     return XQ_OK;
 }
 
@@ -705,6 +805,22 @@ int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, 
 }
 int xq_vit_gelu_bwd_f16(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C, void *stream) {
     return gelu_bwd<F16>(x, bias, gy, gx, g_bias, M, C, stream);
+}
+
+
+int xq_vit_swiglu_fwd(const void *pre, const float *bias, void *act, int M, int H, void *stream) {
+    return swiglu_fwd<Bf16>(pre, bias, act, M, H, stream);
+}
+int xq_vit_swiglu_fwd_f16(const void *pre, const float *bias, void *act, int M, int H, void *stream) {
+    return swiglu_fwd<F16>(pre, bias, act, M, H, stream);
+}
+
+int xq_vit_swiglu_bwd(const void *pre, const float *bias, const void *gy, void *d_pre, float *g_bias, int M, int H, void *stream) {
+    return swiglu_bwd<Bf16>(pre, bias, gy, d_pre, g_bias, M, H, stream);
+}
+int xq_vit_swiglu_bwd_f16(const void *pre, const float *bias, const void *gy, void *d_pre, float *g_bias, int M, int H,
+                          void *stream) {
+    return swiglu_bwd<F16>(pre, bias, gy, d_pre, g_bias, M, H, stream);
 }
 
 }  // extern "C"

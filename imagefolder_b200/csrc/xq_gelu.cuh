@@ -1,6 +1,8 @@
-// xq_gelu.cuh -- the exact-erf GELU and its derivative as ONE set of device functions, shared by the stand-alone bias + GELU
-// kernels (vit_kernels.cu) and the fused GEMM epilogues (gemm_kernel.cu), so that both paths produce the same bits.
-// Reference op: nn.GELU() (erf form) inside timm's Mlp, tokenizer/tokenizer_image/dino_enc/vision_transformer.py:336-339.
+// xq_gelu.cuh -- the exact-erf GELU, SiLU / SwiGLU and their derivatives as ONE set of device functions, shared by the
+// stand-alone element-wise kernels (vit_kernels.cu) and the fused GEMM epilogues (gemm_kernel.cu), so that both paths produce
+// the same bits.
+// Reference ops: nn.GELU() (erf form) inside timm's Mlp, tokenizer/tokenizer_image/dino_enc/vision_transformer.py:336-339, and
+// nn.SiLU inside timm's SwiGLUPacked (GluMlp, gate_last=False) of the giant backbones, vision_transformer.py:2925-2937.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -38,6 +40,24 @@ __device__ __forceinline__ float dgelu_f(float x) {
     const float pe = q * t * e;                                          // 1 - erf(|x| / sqrt2)
     const float half = fmaf(-0.5f, pe, 0.5f);                           // Phi(|x|) - 1/2
     return fmaf(x * 0.3989422804014327f, e, 0.5f + copysignf(half, x));
+}
+
+// silu(x) = x / (1 + exp(-x)) with the accurate expf and an IEEE division: the formula and the fp32 operations of
+// torch.nn.functional.silu's CUDA kernel.  Large negative x: exp overflows to +inf and the result is -0; x = -inf gives NaN,
+// as torch does.
+__device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
+// silu'(x) = s (1 + x (1 - s)), s = sigmoid(x) = 1 / (1 + exp(-x))
+__device__ __forceinline__ float dsilu_f(float x) {
+    const float s = 1.0f / (1.0f + expf(-x));
+    return s * fmaf(x, 1.0f - s, 1.0f);
+}
+// SwiGLU on one column pair (timm GluMlp, gate_last=False: the first half of fc1's output is the gate):
+//   a = gate pre-activation + its bias, c = up pre-activation + its bias;  act = silu(a) * c
+__device__ __forceinline__ float swiglu_f(float a, float c) { return silu_f(a) * c; }
+// backward of act = silu(a) * c for the incoming gradient g:  d_a = g c silu'(a),  d_c = g silu(a)
+__device__ __forceinline__ void dswiglu_f(float g, float a, float c, float &d_a, float &d_c) {
+    d_a = g * c * dsilu_f(a);
+    d_c = g * silu_f(a);
 }
 
 }  // namespace xqv

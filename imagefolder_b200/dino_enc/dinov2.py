@@ -23,7 +23,9 @@ from .lora import LoraConfig, get_peft_model
 from .to_pixel import ToPixel
 from .vision_transformer import Attention, create_model, trunc_normal_
 
-_NAMES = ['vit_small_patch14_dinov2.lvd142m', 'vit_base_patch14_dinov2.lvd142m', 'vit_large_patch14_dinov2.lvd142m']
+_NAMES = ['vit_small_patch14_dinov2.lvd142m', 'vit_base_patch14_dinov2.lvd142m', 'vit_large_patch14_dinov2.lvd142m',
+          'vit_giant_patch14_dinov2.lvd142m', 'vit_small_patch14_reg4_dinov2.lvd142m', 'vit_base_patch14_reg4_dinov2.lvd142m',
+          'vit_large_patch14_reg4_dinov2.lvd142m', 'vit_giant_patch14_reg4_dinov2.lvd142m']
 # modules_to_save of the reference's two LoRA methods (dinov2.py:57, 63); both adapt exactly the MLP Linears
 _LORA_SAVE = {'lora': ['norm'], 'lora_unfreeze_patch_embed': ['patch_embed.proj', 'patch_embed.norm', 'norm']}
 _LORA_TARGETS = r".*\.mlp\.fc\d"
@@ -71,6 +73,16 @@ def _adopt_backbone(owner, model, tuning_method, tuning_kwargs):
     owner.num_prefix_tokens = model.num_prefix_tokens
 
 
+def _check_prefix(model_name, abs_pos_embed):
+    """abs_pos_embed sizes the level-embedding index row for ONE prefix token (dinov2.py:91, 98, 266); the reference's
+    forward then fails on a shape mismatch for the four-register backbones (five prefix tokens).  Refused here, at
+    construction, with the reason (DESIGN.md section 8)."""
+    if abs_pos_embed and '_reg4_' in model_name:
+        raise ValueError(f"{model_name} has 5 prefix tokens (cls + 4 registers), but abs_pos_embed=True sizes the level "
+                         "embedding for 1 (the reference's lvl1LC, dinov2.py:91/266) and fails in its forward; use "
+                         "abs_pos_embed=False with the reg4 backbones")
+
+
 def _level_embedding(owner, n_levels, dim, segment_lengths):
     """`lvl_embed` (trunc-normal, std sqrt(1/3D)) + the `lvl1LC` index row: segment i of the sequence gets level i."""
     owner.lvl_embed = nn.Embedding(n_levels, dim)
@@ -103,6 +115,7 @@ class DINOv2Encoder(_Tunable, nn.Module):
                  pretrained=True, tuning_method='lora', tuning_kwargs={'r': 8}, abs_pos_embed=False, product_quant=1):
         super().__init__()
         assert model_name in _NAMES, f"{model_name} not found"
+        _check_prefix(model_name, abs_pos_embed and bool(num_latent_tokens))
         self.num_latent_tokens, self.use_attn_mask = num_latent_tokens, use_attn_mask
         self.product_quant, self.abs_pos_embed = product_quant, abs_pos_embed
         _adopt_backbone(self, create_model(model_name, pretrained=pretrained, **model_kwargs), tuning_method, tuning_kwargs)
@@ -167,6 +180,7 @@ class DINOv2Decoder(_Tunable, nn.Module):
                  cond_latent=False, abs_pos_embed=False):
         super().__init__()
         assert model_name in _NAMES
+        _check_prefix(model_name, abs_pos_embed)
         for flag, name in ((use_rope, "use_rope=True (RoPEAttention)"), (cond_latent, "cond_latent=True")):
             if flag:
                 raise NotImplementedError(f"{name} is not selected by any shipped config; not built")

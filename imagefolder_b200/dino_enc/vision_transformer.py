@@ -3,10 +3,11 @@
 Restates the subset of timm==1.0.9's VisionTransformer that the reference instantiates through
 its vendored copy (tokenizer/tokenizer_image/dino_enc/vision_transformer.py): `Attention` (:145),
 `LayerScale` (:280), `Block` (:295), `VisionTransformer` (:587, `_pos_embed` :814-848), and the
-model-name registry entries the shipped configs use (`vit_*_patch14_dinov2.lvd142m`, :2893-2935).
+model-name registry entries the reference's DINOv2 encoder / decoder accept (`vit_{small,base,large,giant}_patch14_dinov2
+.lvd142m` and their `_reg4_` variants, :2893-2995).
 timm itself is not vendored in the reference nor installed here, so `PatchEmbed`, `Mlp`, `DropPath`
 and `resample_abs_pos_embed` follow timm 1.0.9's published behaviour (SURVEY.md section 8c:
-this boundary is "parity unpinned" by the reference).
+this boundary is "parity unpinned" by the reference); so does `GluMlp` (timm's SwiGLUPacked) of the giant backbones.
 
 Parameter names (= checkpoint keys) are identical to timm's: patch_embed.proj, cls_token,
 pos_embed, blocks.{i}.{norm1,attn.qkv,attn.proj,ls1.gamma,norm2,mlp.fc1,mlp.fc2,ls2.gamma}, norm.
@@ -56,6 +57,26 @@ class Mlp(nn.Module):
 
     def forward(self, x):
         return self.fc2(self.act(self.fc1(x)))
+
+
+class GluMlp(nn.Module):
+    """timm.layers.GluMlp with gate_last=False, as timm's SwiGLUPacked builds it for the giant backbones
+    (vision_transformer.py:2925-2937: mlp_layer=SwiGLUPacked, act_layer=nn.SiLU, norm Identity): fc1 -> [gate | up] halves ->
+    act(gate) * up -> fc2.  Attribute and checkpoint key names are timm's (mlp.fc1 / mlp.fc2)."""
+
+    def __init__(self, in_features, hidden_features=None, out_features=None, act_layer=nn.SiLU, drop=0.0, **_):
+        super().__init__()
+        out_features = out_features or in_features
+        hidden_features = hidden_features or in_features
+        assert hidden_features % 2 == 0
+        self.fc1 = nn.Linear(in_features, hidden_features)
+        self.act = act_layer()
+        self.norm = nn.Identity()
+        self.fc2 = nn.Linear(hidden_features // 2, out_features)
+
+    def forward(self, x):
+        x1, x2 = self.fc1(x).chunk(2, dim=-1)
+        return self.fc2(self.norm(self.act(x1) * x2))
 
 
 class DropPath(nn.Module):
@@ -169,7 +190,7 @@ class VisionTransformer(nn.Module):
     def __init__(self, img_size=224, patch_size=16, in_chans=3, num_classes=0, embed_dim=768, depth=12, num_heads=12,
                  mlp_ratio=4.0, qkv_bias=True, init_values=None, class_token=True, no_embed_class=False, reg_tokens=0,
                  pre_norm=False, drop_path_rate=0.0, attn_layer=Attention, num_latent_tokens=32, global_pool='token',
-                 norm_eps=1e-6, **unused):
+                 norm_eps=1e-6, mlp_layer=Mlp, act_layer=nn.GELU, **unused):
         super().__init__()
         norm_layer = partial(nn.LayerNorm, eps=norm_eps)     # timm: 1e-6 for the DINOv2 / plain ViTs, 1e-5 for the CLIP variants
         self.num_classes = num_classes
@@ -193,7 +214,8 @@ class VisionTransformer(nn.Module):
         dpr = [x.item() for x in torch.linspace(0, drop_path_rate, depth)]
         self.blocks = nn.Sequential(*[
             Block(dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias, init_values=init_values,
-                  drop_path=dpr[i], norm_layer=norm_layer, attn_layer=attn_layer) for i in range(depth)])
+                  drop_path=dpr[i], norm_layer=norm_layer, attn_layer=attn_layer, mlp_layer=mlp_layer, act_layer=act_layer)
+            for i in range(depth)])
         self.norm = norm_layer(embed_dim)
         self.fc_norm = nn.Identity()
         self.head_drop = nn.Dropout(0.0)
@@ -263,6 +285,19 @@ _ARCH = {
     'vit_small_patch14_dinov2.lvd142m': dict(patch_size=14, embed_dim=384, depth=12, num_heads=6, init_values=1e-5, img_size=518),
     'vit_base_patch14_dinov2.lvd142m': dict(patch_size=14, embed_dim=768, depth=12, num_heads=12, init_values=1e-5, img_size=518),
     'vit_large_patch14_dinov2.lvd142m': dict(patch_size=14, embed_dim=1024, depth=24, num_heads=16, init_values=1e-5, img_size=518),
+    # hidden_features = int(1536 * 5.33334) = 8192: the packed [gate | up] width of fc1 (fc2 takes 4096)
+    'vit_giant_patch14_dinov2.lvd142m': dict(patch_size=14, embed_dim=1536, depth=40, num_heads=24, init_values=1e-5,
+                                             mlp_ratio=2.66667 * 2, mlp_layer=GluMlp, act_layer=nn.SiLU, img_size=518),
+    # four register tokens; pos_embed covers the patch tokens only (:2942-2995)
+    'vit_small_patch14_reg4_dinov2.lvd142m': dict(patch_size=14, embed_dim=384, depth=12, num_heads=6, init_values=1e-5,
+                                                  reg_tokens=4, no_embed_class=True, img_size=518),
+    'vit_base_patch14_reg4_dinov2.lvd142m': dict(patch_size=14, embed_dim=768, depth=12, num_heads=12, init_values=1e-5,
+                                                 reg_tokens=4, no_embed_class=True, img_size=518),
+    'vit_large_patch14_reg4_dinov2.lvd142m': dict(patch_size=14, embed_dim=1024, depth=24, num_heads=16, init_values=1e-5,
+                                                  reg_tokens=4, no_embed_class=True, img_size=518),
+    'vit_giant_patch14_reg4_dinov2.lvd142m': dict(patch_size=14, embed_dim=1536, depth=40, num_heads=24, init_values=1e-5,
+                                                  mlp_ratio=2.66667 * 2, mlp_layer=GluMlp, act_layer=nn.SiLU, reg_tokens=4,
+                                                  no_embed_class=True, img_size=518),
     'vit_base_patch16_clip_224.openai': dict(patch_size=16, embed_dim=768, depth=12, num_heads=12, pre_norm=True, img_size=224),
 }
 

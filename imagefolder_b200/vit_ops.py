@@ -21,7 +21,7 @@ import torch.nn.functional as F
 from . import _capi as C
 from ._capi import call as _call, lib as _lib, ptr as _ptr, stream_ptr as _stream
 
-_SUPPORTED_D = (384, 768, 1024)
+_SUPPORTED_D = (384, 768, 1024, 1536)
 _HALF = (torch.bfloat16, torch.float16)       # the GEMM operand dtypes the kernels are instantiated for
 
 
@@ -232,6 +232,106 @@ class _FusedMLP(torch.autograd.Function):
         return dy, dW1, (db1 if ctx.needs_input_grad[2] else None), dW2
 
 
+class _SwiGLUBias(torch.autograd.Function):
+    """act = silu(a) * c with a = x[..., :H] + bias[:H], c = x[..., H:] + bias[H:], x bf16 or fp16 [..., 2H] (the fc1 GEMM
+    output WITHOUT its bias), bias fp32 [2H] (timm GluMlp, gate_last=False)."""
+
+    @staticmethod
+    def forward(ctx, x, bias):
+        x = x.contiguous()
+        H = x.shape[-1] // 2
+        M = x.numel() // (2 * H)
+        act = torch.empty(x.shape[:-1] + (H,), dtype=x.dtype, device=x.device)
+        name, fn = _entry("xq_vit_swiglu_fwd", x.dtype)
+        C.call(name, 1, fn, C.ptr(x), C.ptr(bias), C.ptr(act), M, H, C.stream_ptr(x.device), nbytes=M * H * 6)
+        ctx.save_for_backward(x, bias)
+        return act
+
+    @staticmethod
+    def backward(ctx, g):
+        x, bias = ctx.saved_tensors
+        g = g.contiguous()
+        if g.dtype != x.dtype:
+            g = g.to(x.dtype)
+        H = x.shape[-1] // 2
+        M = x.numel() // (2 * H)
+        gx = torch.empty_like(x)
+        gb = torch.empty_like(bias) if bias is not None else None
+        name, fn = _entry("xq_vit_swiglu_bwd", x.dtype)
+        C.call(name, 1, fn, C.ptr(x), C.ptr(bias), C.ptr(g), C.ptr(gx), C.ptr(gb), M, H, C.stream_ptr(x.device),
+               nbytes=M * H * 10)
+        return gx, gb
+
+
+def swiglu_bias(x, bias=None):
+    return _SwiGLUBias.apply(x, bias)
+
+
+# The wgmma GEMMs with fused SwiGLU / SwiGLU' epilogues (csrc/gemm_kernel.cu, EPI 3 / 4).  Off by default: at the giant
+# training shape they are slower than the library GEMM + stand-alone kernel (tools/bench_swiglu_mlp.py, DESIGN.md section 0).
+SWIGLU_TC_ENABLED = [False]
+
+
+def swiglu_tc_ok(y, fc1, fc2) -> bool:
+    """xq_vit_fc1_swiglu_fwd / xq_vit_fc2_dswiglu_bwd (and their _f16 twins) cover: bf16 or fp16 CUDA tokens, an fc1 bias,
+    H = fc1 width / 2 with H % 128 == 0 (the backward's 128-column tiles; the forward needs H % 64), embed % 64 == 0, out % 64
+    == 0 (the K of the backward GEMM) and H / 64 <= SM count (the forward's column blocks; the backward has half as many).
+    Mirrors every refusal of the C wrappers, so neither call fails inside forward or backward."""
+    N1, K = fc1.weight.shape
+    return (SWIGLU_TC_ENABLED[0] and y.is_cuda and y.dtype in _HALF and fc1.bias is not None
+            and N1 % 256 == 0 and K % 64 == 0 and fc2.weight.shape[1] == N1 // 2 and fc2.weight.shape[0] % 64 == 0
+            and (N1 // 2) // 64 <= _sm_count(y.device))
+
+
+class _FusedSwiGLU(torch.autograd.Function):
+    """branch = fc2(silu(a) * c), [a | c] = fc1(y), WITHOUT the fc2 bias (folded into the next residual_ln): timm GluMlp as
+    called from Block.forward.  The fc1 GEMM carries bias + SwiGLU in its epilogue, the fc2 input-gradient GEMM carries the
+    SwiGLU derivative and the fc1-bias gradient; the other GEMMs are library calls.  Same bits as F.linear + swiglu_bias."""
+
+    @staticmethod
+    def forward(ctx, y, W1, b1, W2):
+        N1, K = W1.shape
+        H = N1 // 2
+        y2 = y.reshape(-1, K)
+        if not y2.is_contiguous():
+            y2 = y2.contiguous()
+        M = y2.shape[0]
+        dt = y.dtype
+        W1b, W2b, b1f = W1.to(dt), W2.to(dt), b1.float()
+        pre = torch.empty(M, N1, dtype=dt, device=y.device)
+        act = torch.empty(M, H, dtype=dt, device=y.device)
+        name, fn = _entry("xq_vit_fc1_swiglu_fwd", dt)
+        C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(b1f), C.ptr(pre), C.ptr(act), M, H, K,
+               C.stream_ptr(y.device), nbytes=M * K * 2 + N1 * K * 2 + M * N1 * 2 + M * H * 2, nflops=2.0 * M * N1 * K)
+        branch = act @ W2b.t()
+        ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
+        ctx.out_shape = y.shape[:-1] + (W2.shape[0],)
+        ctx.in_shape = y.shape
+        return branch.view(ctx.out_shape)
+
+    @staticmethod
+    def backward(ctx, g):
+        y2, pre, act, W1b, W2b, b1f = ctx.saved_tensors
+        M, N1 = pre.shape
+        H = N1 // 2
+        Ko = W2b.shape[0]
+        g2 = g.reshape(M, Ko)
+        if g2.dtype != pre.dtype:
+            g2 = g2.to(pre.dtype)
+        if not g2.is_contiguous():
+            g2 = g2.contiguous()
+        dW2 = (g2.t() @ act).float() if ctx.needs_input_grad[3] else None
+        W2t = W2b.t().contiguous()                      # [H, out]: the K-major B operand of g_act = g W2
+        dpre = torch.empty_like(pre)
+        db1 = torch.empty(N1, dtype=torch.float32, device=pre.device)
+        name, fn = _entry("xq_vit_fc2_dswiglu_bwd", pre.dtype)
+        C.call(name, 1, fn, C.ptr(g2), C.ptr(W2t), C.ptr(pre), C.ptr(b1f), C.ptr(dpre), C.ptr(db1),
+               M, H, Ko, C.stream_ptr(pre.device), nbytes=M * Ko * 2 + H * Ko * 2 + M * N1 * 4, nflops=2.0 * M * H * Ko)
+        dW1 = (dpre.t() @ y2).float() if ctx.needs_input_grad[1] else None
+        dy = (dpre @ W1b).view(ctx.in_shape) if ctx.needs_input_grad[0] else None
+        return dy, dW1, (db1 if ctx.needs_input_grad[2] else None), dW2
+
+
 def _scaled_mm(a, b, s: float):
     """16-bit(s * (a @ b)) in a's dtype: the scale applied to the fp32 accumulator, one rounding"""
     return torch.addmm(a.new_zeros(()), a, b, beta=0, alpha=s)
@@ -329,11 +429,18 @@ def _linear_no_bias(fc, x):
 
 
 def mlp_forward(mlp, y):
-    """timm Mlp (fc1 -> GELU -> fc2, drop = 0) without the fc2 bias; fused wgmma path when the shapes allow, else library GEMMs +
-    the stand-alone bias / GELU kernel.  LoRA-wrapped fc1 and fc2 with inactive lora_dropout and r <= 64 take the LoRA form of
+    """timm Mlp (fc1 -> GELU -> fc2, drop = 0) or GluMlp (fc1 -> SwiGLU -> fc2) without the fc2 bias; fused wgmma path when the
+    shapes allow, else library GEMMs + the stand-alone bias / GELU (SwiGLU) kernel.  LoRA-wrapped fc1 and fc2 with inactive lora_dropout and r <= 64 take the LoRA form of
     the fused path; any other LoRA Linear adds its `lora_delta` to a library GEMM."""
     fc1, fc2 = mlp.fc1, mlp.fc2
     lora = _lora()
+    from .dino_enc.vision_transformer import GluMlp      # imported here: dino_enc imports this module
+    if isinstance(mlp, GluMlp):
+        # timm GluMlp (the giant backbones): fused SwiGLU GEMMs for plain Linears, else library GEMMs + the stand-alone
+        # SwiGLU kernel (LoRA-wrapped fc1 / fc2 included: there is no fused LoRA form of the SwiGLU GEMMs)
+        if not (isinstance(fc1, lora.Linear) or isinstance(fc2, lora.Linear)) and swiglu_tc_ok(y, fc1, fc2):
+            return _FusedSwiGLU.apply(y, fc1.weight, fc1.bias, fc2.weight)
+        return _linear_no_bias(fc2, swiglu_bias(_linear_no_bias(fc1, y), fc1.bias))
     if isinstance(fc1, lora.Linear) or isinstance(fc2, lora.Linear):
         if (isinstance(fc1, lora.Linear) and isinstance(fc2, lora.Linear) and _lora_off(fc1) and _lora_off(fc2)
                 and fc1.r[fc1.active_adapter] <= 64 and fc2.r[fc2.active_adapter] == fc1.r[fc1.active_adapter]

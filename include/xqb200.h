@@ -268,6 +268,18 @@ int xq_vit_gelu_bwd(const void *x, const float *bias, const void *gy, void *gx, 
 int xq_vit_gelu_fwd_f16(const void *x, const float *bias, void *y, int M, int C, void *stream);
 int xq_vit_gelu_bwd_f16(const void *x, const float *bias, const void *gy, void *gx, float *g_bias, int M, int C,
                         void *stream);
+/*   SwiGLU of timm's GluMlp (gate_last=False), the MLP of the giant backbones (SwiGLUPacked, act_layer=nn.SiLU,
+ *   tokenizer/tokenizer_image/dino_enc/vision_transformer.py:2925-2937): pre [M,2H] is the fc1 GEMM output WITHOUT its bias
+ *   (gate columns [0,H), up columns [H,2H)), bias fp32 [2H] or NULL, H % 8 == 0 (else XQ_ERR_ARG, nothing written).
+ *     forward   act [M,H]:   act[:, j] = silu(pre[:, j] + b[j]) * (pre[:, H+j] + b[H+j]), rounded once
+ *     backward  gy [M,H] -> d_pre [M,2H]:  d_pre[:, j] = gy silu'(a) c,  d_pre[:, H+j] = gy silu(a),  and g_bias [2H] = column
+ *               sums of the rounded d_pre (may be NULL; fp32 atomics, in no fixed order).
+ *   silu is x / (1 + exp(-x)) in fp32 with the accurate exp, torch.nn.functional.silu's formula.  Allocates nothing. */
+int xq_vit_swiglu_fwd(const void *pre, const float *bias, void *act, int M, int H, void *stream);
+int xq_vit_swiglu_bwd(const void *pre, const float *bias, const void *gy, void *d_pre, float *g_bias, int M, int H, void *stream);
+int xq_vit_swiglu_fwd_f16(const void *pre, const float *bias, void *act, int M, int H, void *stream);
+int xq_vit_swiglu_bwd_f16(const void *pre, const float *bias, const void *gy, void *d_pre, float *g_bias, int M, int H,
+                          void *stream);
 
 /*   Flash attention of the ViT blocks, head_dim 64, no mask, no dropout (Attention.forward,
  *   tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197: F.scaled_dot_product_attention on
@@ -358,6 +370,24 @@ int xq_vit_fc1_lora_gelu_fwd_f16(const void *x, const void *w, const void *u, co
                                  void *act, int M, int N, int K, int R, void *stream);
 int xq_vit_fc2_lora_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre,
                                   const float *bias, void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream);
+
+/* SwiGLU forms of xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd for timm's GluMlp (vision_transformer.py:2925-2937):
+ *   forward   F.linear(y, W1) [cuBLAS] + xq_vit_swiglu_fwd                       -> xq_vit_fc1_swiglu_fwd
+ *   backward  g = d_out W2 [cuBLAS] + xq_vit_swiglu_bwd                          -> xq_vit_fc2_dswiglu_bwd
+ *   x [M,K], w [2H,K] (fc1.weight), bias [2H]  ->  pre [M,2H] = x w^T ,  act [M,H] as xq_vit_swiglu_fwd computes it from pre
+ *   d_out [M,K], w2t [H,K] (fc2.weight TRANSPOSED), pre [M,2H], bias [2H]
+ *     ->  d_pre [M,2H] as xq_vit_swiglu_bwd computes it from g = 16-bit(d_out w2t^T),  d_bias [2H] (required)
+ * Equal, bit for bit, to those two-call sequences up to the GEMM's fp32 accumulation order (d_bias: fp32 atomics, in no fixed
+ * order).  The forward needs H % 64 == 0 and H / 64 <= SM count, the backward H % 128 == 0 and H / 128 <= SM count; both
+ * K % 64 == 0 (else XQ_ERR_UNSUPPORTED); NULL or misaligned pointers give XQ_ERR_ARG.  A refused call writes nothing; no call
+ * allocates. */
+int xq_vit_fc1_swiglu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K, void *stream);
+int xq_vit_fc2_dswiglu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
+                           int M, int H, int K, void *stream);
+int xq_vit_fc1_swiglu_fwd_f16(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K,
+                              void *stream);
+int xq_vit_fc2_dswiglu_bwd_f16(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre,
+                               float *d_bias, int M, int H, int K, void *stream);
 
 /* ---- input pipeline: the training / validation image transforms (SURVEY.md section 8 row f-4, csrc/img_kernels.cu) ---------
  * Replaces the per-image CPU transform of the reference's DataLoader workers:
