@@ -49,6 +49,8 @@ F16_TWINS = [
 ]
 # the SwiGLU entry points of the giant backbones' MLP, with `_f16` twins in the same sense
 SWIGLU_ENTRIES = ["xq_vit_swiglu_fwd", "xq_vit_swiglu_bwd", "xq_vit_fc1_swiglu_fwd", "xq_vit_fc2_dswiglu_bwd"]
+# the RoPE decoder's q / k rotation (csrc/rope_kernel.cu), with `_f16` twins in the same sense
+ROPE_ENTRIES = ["xq_vit_rope_fwd", "xq_vit_rope_bwd"]
 
 
 def lib() -> ctypes.CDLL:
@@ -140,8 +142,14 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_fc1_swiglu_fwd.argtypes = [vp, vp, f32p, vp, vp, c_int, c_int, c_int, vp]
     L.xq_vit_fc2_dswiglu_bwd.restype = c_int
     L.xq_vit_fc2_dswiglu_bwd.argtypes = [vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, vp]
+    L.xq_vit_rope_fwd.restype = c_int
+    L.xq_vit_rope_fwd.argtypes = [vp, vp, f32p, f32p] + [c_int] * 7 + [vp]
+    L.xq_vit_rope_bwd_workspace_bytes.restype = c_size_t
+    L.xq_vit_rope_bwd_workspace_bytes.argtypes = [c_int] * 4
+    L.xq_vit_rope_bwd.restype = c_int
+    L.xq_vit_rope_bwd.argtypes = [vp, vp, f32p, f32p] + [c_int] * 7 + [vp, f32p, f32p, f32p, vp, c_size_t, vp]
     # fp16 twins of the 16-bit ViT entry points: the same argument lists
-    for name in F16_TWINS + SWIGLU_ENTRIES:
+    for name in F16_TWINS + SWIGLU_ENTRIES + ROPE_ENTRIES:
         twin = getattr(L, name + "_f16")
         twin.restype = c_int
         twin.argtypes = getattr(L, name).argtypes
@@ -263,4 +271,6 @@ EXPORTED_SYMBOLS = [
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
     "xq_ema_update", "xq_adamw_step", "xq_grad_norm_workspace_bytes", "xq_grad_norm", "xq_grad_scale", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
-] + [n + "_f16" for n in F16_TWINS] + SWIGLU_ENTRIES + [n + "_f16" for n in SWIGLU_ENTRIES]
+    "xq_vit_rope_bwd_workspace_bytes",
+] + [n + "_f16" for n in F16_TWINS] + SWIGLU_ENTRIES + [n + "_f16" for n in SWIGLU_ENTRIES] + ROPE_ENTRIES + [
+    n + "_f16" for n in ROPE_ENTRIES]

@@ -1,6 +1,7 @@
 """DINOv2Encoder / DINOv2Decoder -- drop-in for tokenizer/tokenizer_image/dino_enc/dinov2.py
 (:18 and :201): ViT backbone + learnable latent tokens, level embedding, mask tokens, ToPixel.
 
+DINOv2Decoder(use_rope=True) builds its blocks with RoPEAttention (rotary q / k, no latent positional embedding).
 tuning_method 'full', 'frozen', 'lora' and 'lora_unfreeze_patch_embed' are built, in the constructors and in `finetine`; the
 LoRA ones wrap the ViT with lora.py, a restatement of the peft 0.13.0 calls the reference makes.  'lat_lora' is not built.
 Sub-module / parameter names match the reference so released checkpoints load unchanged.
@@ -21,7 +22,7 @@ import torch.nn as nn
 from ..vit_ops import assemble_tokens, patch_embed, run_blocks
 from .lora import LoraConfig, get_peft_model
 from .to_pixel import ToPixel
-from .vision_transformer import Attention, create_model, trunc_normal_
+from .vision_transformer import Attention, RoPEAttention, create_model, trunc_normal_
 
 _NAMES = ['vit_small_patch14_dinov2.lvd142m', 'vit_base_patch14_dinov2.lvd142m', 'vit_large_patch14_dinov2.lvd142m',
           'vit_giant_patch14_dinov2.lvd142m', 'vit_small_patch14_reg4_dinov2.lvd142m', 'vit_base_patch14_reg4_dinov2.lvd142m',
@@ -180,13 +181,17 @@ class DINOv2Decoder(_Tunable, nn.Module):
                  cond_latent=False, abs_pos_embed=False):
         super().__init__()
         assert model_name in _NAMES
+        if use_rope and abs_pos_embed:
+            # the reference builds no level embedding with use_rope (dinov2.py:264) but its forward still adds one (:342)
+            raise ValueError("use_rope=True with abs_pos_embed=True: the reference's forward adds lvl_embed[lvl1LC], which "
+                             "it does not create for use_rope, and fails; use abs_pos_embed=False with use_rope")
         _check_prefix(model_name, abs_pos_embed)
-        for flag, name in ((use_rope, "use_rope=True (RoPEAttention)"), (cond_latent, "cond_latent=True")):
-            if flag:
-                raise NotImplementedError(f"{name} is not selected by any shipped config; not built")
+        if cond_latent:
+            raise NotImplementedError("cond_latent=True is not selected by any shipped config; not built")
         self.use_rope, self.cond_latent = use_rope, cond_latent
         self.num_latent_tokens, self.abs_pos_embed = num_latent_tokens, abs_pos_embed
-        vit_kwargs = dict(model_kwargs, num_latent_tokens=num_latent_tokens, attn_layer=Attention)
+        vit_kwargs = dict(model_kwargs, num_latent_tokens=num_latent_tokens,
+                          attn_layer=RoPEAttention if use_rope else Attention)
         model = create_model(model_name, pretrained=pretrained, **vit_kwargs)
         # the decoder never embeds pixels: drop the unused projection so that it is neither trained nor checkpointed (before
         # any LoRA wrapping, so that a saved copy of patch_embed.proj holds no parameters either)
@@ -196,7 +201,9 @@ class DINOv2Decoder(_Tunable, nn.Module):
         D = self.embed_dim
         self.mask_token = nn.Parameter(torch.zeros(1, 1, D))
         nn.init.normal_(self.mask_token, std=1e-6)
-        if abs_pos_embed:
+        if use_rope:
+            pass                                 # positions enter through the rotary embedding only (dinov2.py:264)
+        elif abs_pos_embed:
             # level 0 = [cls | mask tokens], level 1 = the latents WITH the cls slot _pos_embed gives them (dinov2.py:266-272)
             _level_embedding(self, 2, D, [model_kwargs['patch_size'] ** 2 + 1, num_latent_tokens + 1])
         else:
@@ -213,8 +220,13 @@ class DINOv2Decoder(_Tunable, nn.Module):
         return self.to_pixel.model.weight
 
     def _assemble(self, z):
-        """dinov2.py:318-336.  z: latents [B, L, D] -> fp32 [B, prefix + N_img + (prefix if abs_pos_embed) + L, D]."""
+        """dinov2.py:318-344.  z: latents [B, L, D] -> fp32 [B, prefix + N_img + (prefix if abs_pos_embed) + L, D]."""
         masks = self.mask_token.expand(z.size(0), self.num_img_tokens, -1)
+        if self.use_rope:                        # prefix tokens, mask tokens and latents, no positional terms (:336-344)
+            with _autocast_off(masks):
+                vit = self.model
+                prefix = [t.expand(z.size(0), -1, -1) for t in (vit.cls_token, vit.reg_token) if t is not None]
+                return torch.cat([vit.patch_drop(torch.cat(prefix + [masks], dim=1)), z.float()], dim=1)
         with _autocast_off(masks):
             front = self.model._pos_embed(masks)
             if self.abs_pos_embed:

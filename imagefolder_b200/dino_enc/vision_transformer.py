@@ -2,7 +2,7 @@
 
 Restates the subset of timm==1.0.9's VisionTransformer that the reference instantiates through
 its vendored copy (tokenizer/tokenizer_image/dino_enc/vision_transformer.py): `Attention` (:145),
-`LayerScale` (:280), `Block` (:295), `VisionTransformer` (:587, `_pos_embed` :814-848), and the
+`RoPEAttention` (:200, helpers :58-142), `LayerScale` (:280), `Block` (:295), `VisionTransformer` (:587, `_pos_embed` :814-848), and the
 model-name registry entries the reference's DINOv2 encoder / decoder accept (`vit_{small,base,large,giant}_patch14_dinov2
 .lvd142m` and their `_reg4_` variants, :2893-2995).
 timm itself is not vendored in the reference nor installed here, so `PatchEmbed`, `Mlp`, `DropPath`
@@ -151,6 +151,103 @@ class Attention(nn.Module):
         return self.proj_drop(self.proj(x))
 
 
+def init_1d_freqs(dim: int, end: int, theta: float = 10000.0):
+    """vision_transformer.py:58-79: complex64 [end, dim/2], polar(1, t * theta^(-2k/dim))."""
+    freqs = 1.0 / (theta ** (torch.arange(0, dim, 2)[: (dim // 2)].float() / dim))
+    t = torch.arange(end, device=freqs.device)
+    freqs = torch.outer(t, freqs).float()
+    return torch.polar(torch.ones_like(freqs), freqs)
+
+
+def init_2d_freqs(dim: int, num_heads: int, theta: float = 10.0, rotate: bool = True):
+    """vision_transformer.py:82-95: [2, H, dim/2] (fx, fy); one torch.rand(1) angle per head, in head order."""
+    freqs_x, freqs_y = [], []
+    mag = 1 / (theta ** (torch.arange(0, dim, 4)[: (dim // 4)].float() / dim))
+    for _ in range(num_heads):
+        angles = torch.rand(1) * 2 * torch.pi if rotate else torch.zeros(1)
+        freqs_x.append(torch.cat([mag * torch.cos(angles), mag * torch.cos(torch.pi / 2 + angles)], dim=-1))
+        freqs_y.append(torch.cat([mag * torch.sin(angles), mag * torch.sin(torch.pi / 2 + angles)], dim=-1))
+    return torch.stack([torch.stack(freqs_x, dim=0), torch.stack(freqs_y, dim=0)], dim=0)
+
+
+def init_t_xy(end_x: int, end_y: int):
+    """vision_transformer.py:98-102: t_x = n mod end_x, t_y = n div end_x (fp32)."""
+    t = torch.arange(end_x * end_y, dtype=torch.float32)
+    return (t % end_x).float(), torch.div(t, end_x, rounding_mode='floor').float()
+
+
+def compute_mixed_cis(freqs, t_x, t_y, num_heads: int):
+    """vision_transformer.py:105-112: polar(1, t_x fx + t_y fy) -> complex64 [H, N, dim/2], with autocast off."""
+    N = t_x.shape[0]
+    with torch.autocast(device_type=freqs.device.type, enabled=False):
+        freqs_x = (t_x.unsqueeze(-1) @ freqs[0].unsqueeze(-2)).view(N, num_heads, -1).permute(1, 0, 2)
+        freqs_y = (t_y.unsqueeze(-1) @ freqs[1].unsqueeze(-2)).view(N, num_heads, -1).permute(1, 0, 2)
+        return torch.polar(torch.ones_like(freqs_x), freqs_x + freqs_y)
+
+
+def apply_rotary_emb(xq, xk, freqs_cis):
+    """vision_transformer.py:134-142: q / k [..., T, dim] as dim/2 complex pairs times freqs_cis ([T, dim/2] or
+    [H, T, dim/2]) in fp32, returned in the input dtype."""
+    xq_ = torch.view_as_complex(xq.float().reshape(*xq.shape[:-1], -1, 2))
+    xk_ = torch.view_as_complex(xk.float().reshape(*xk.shape[:-1], -1, 2))
+    shape = [1] * (xq_.ndim - freqs_cis.ndim) + list(freqs_cis.shape)
+    freqs_cis = freqs_cis.view(*shape)
+    return (torch.view_as_real(xq_ * freqs_cis).flatten(3).type_as(xq),
+            torch.view_as_real(xk_ * freqs_cis).flatten(3).type_as(xk))
+
+
+class RoPEAttention(Attention):
+    """vision_transformer.py:200-270: Attention with rotary position embeddings on q and k -- 2-D mixed frequencies
+    (`freqs`, learnable fp32 [2, H*dim/2]) for the image tokens, a learnable complex64 table (`freqs_1d`, [L, dim/2]) for the
+    latent tokens, prefix tokens untouched.  Token order [prefix | image | latent].
+
+    The forward here is the module path (CPU, fp32, autocast dtypes the fused kernels do not cover); vit_ops runs the
+    bf16 / fp16 CUDA path on csrc/rope_kernel.cu.  It writes the rotated slices into new tensors instead of into the qkv view
+    in place, so its fp32 backward works; the reference's fails there (DESIGN.md section 8).  rope_mixed=False (the axial
+    branch) is not reachable from DINOv2Decoder and is refused."""
+
+    def __init__(self, *args, num_prefix_tokens=1, num_latent_tokens=32, num_image_tokens=256, rope_theta=10.0,
+                 rope_mixed=True, **kwargs):
+        super().__init__(*args, **kwargs)
+        if not rope_mixed:
+            raise NotImplementedError("RoPEAttention(rope_mixed=False) (axial frequencies) is not reachable from "
+                                      "DINOv2Decoder; not built")
+        self.rope_mixed = rope_mixed
+        self.num_prefix_tokens = num_prefix_tokens
+        self.num_latent_tokens = num_latent_tokens
+        self.num_image_tokens = num_image_tokens
+        self.num_axis_tokens = int(num_image_tokens ** 0.5)
+        freqs = init_2d_freqs(dim=self.head_dim, num_heads=self.num_heads, theta=rope_theta, rotate=True).view(2, -1)
+        self.freqs = nn.Parameter(freqs, requires_grad=True)
+        t_x, t_y = init_t_xy(end_x=self.num_axis_tokens, end_y=self.num_axis_tokens)
+        self.register_buffer('freqs_t_x', t_x)
+        self.register_buffer('freqs_t_y', t_y)
+        self.freqs_1d = nn.Parameter(init_1d_freqs(dim=self.head_dim, end=self.num_latent_tokens), requires_grad=True)
+
+    def forward(self, x, attn_mask=None):
+        B, N, C = x.shape
+        P, L = self.num_prefix_tokens, self.num_latent_tokens
+        qkv = self.qkv(x).reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
+        q, k, v = qkv[0], qkv[1], qkv[2]
+        t_x, t_y = self.freqs_t_x, self.freqs_t_y
+        if t_x.shape[0] != N - P - L:                     # :237-240
+            side = math.sqrt(N - 1)
+            t_x, t_y = init_t_xy(end_x=side, end_y=side)
+            t_x, t_y = t_x.to(x.device), t_y.to(x.device)
+        freqs_cis = compute_mixed_cis(self.freqs, t_x, t_y, self.num_heads)
+        dtype = x.dtype
+        with torch.autocast(device_type=x.device.type, enabled=False):
+            qi, ki = apply_rotary_emb(q[:, :, P:N - L], k[:, :, P:N - L], freqs_cis)
+            ql, kl = apply_rotary_emb(q[:, :, N - L:], k[:, :, N - L:], self.freqs_1d)
+            q = torch.cat([q[:, :, :P], qi, ql], dim=2)
+            k = torch.cat([k[:, :, :P], ki, kl], dim=2)
+        q, k = q.to(dtype), k.to(dtype)
+        attn = (q * self.scale) @ k.transpose(-2, -1)          # attn_mask is ignored, as in the reference
+        attn = self.attn_drop(attn.softmax(dim=-1))
+        x = (attn @ v).transpose(1, 2).reshape(B, N, C)
+        return self.proj_drop(self.proj(x))
+
+
 class LayerScale(nn.Module):
     def __init__(self, dim, init_values=1e-5, inplace=False):
         super().__init__()
@@ -214,7 +311,9 @@ class VisionTransformer(nn.Module):
         dpr = [x.item() for x in torch.linspace(0, drop_path_rate, depth)]
         self.blocks = nn.Sequential(*[
             Block(dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias, init_values=init_values,
-                  drop_path=dpr[i], norm_layer=norm_layer, attn_layer=attn_layer, mlp_layer=mlp_layer, act_layer=act_layer)
+                  drop_path=dpr[i], norm_layer=norm_layer, mlp_layer=mlp_layer, act_layer=act_layer,
+                  attn_layer=partial(attn_layer, num_prefix_tokens=self.num_prefix_tokens,        # :728-731
+                                     num_latent_tokens=num_latent_tokens, patch_size=patch_size))
             for i in range(depth)])
         self.norm = norm_layer(embed_dim)
         self.fc_norm = nn.Identity()

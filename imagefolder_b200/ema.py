@@ -25,7 +25,10 @@ def update_ema(ema_model, model, decay=0.9999):
     """Step the EMA model towards the current model: for every parameter name of `model`,
     ema = ema * decay + (1 - decay) * param, bit-identical to the reference's `mul_(decay).add_(param, alpha=1 - decay)`.
 
-    Every pair is checked before anything is launched (same shape, fp32, contiguous CUDA tensors on one device), so a refused
+    A complex64 parameter (the RoPE decoder's `freqs_1d`) is averaged through its real view, component by component
+    (DESIGN.md section 8 states where that differs from torch's complex mul_ / add_: signed zeros and non-finite values).
+    Every pair is checked before anything is launched (same shape and dtype, fp32 or complex64, contiguous CUDA tensors on
+    one device), so a refused
     call leaves the EMA model unchanged.  The pointer table is rebuilt on every call: `.to()`, `load_state_dict` or a wrapper
     that rebinds parameters can all move the storage between calls."""
     ema_params = OrderedDict(ema_model.named_parameters())
@@ -35,9 +38,12 @@ def update_ema(ema_model, model, decay=0.9999):
         e = ema_params[name]
         if e.shape != param.shape:
             raise ValueError(f"update_ema: {name}: ema shape {tuple(e.shape)} != model shape {tuple(param.shape)}")
-        if e.dtype != torch.float32 or param.dtype != torch.float32:
-            raise ValueError(f"update_ema: {name}: fp32 tensors are required (ema {e.dtype}, model {param.dtype})")
+        if e.dtype not in (torch.float32, torch.complex64) or param.dtype != e.dtype:
+            raise ValueError(f"update_ema: {name}: fp32 or complex64 tensors of one dtype are required (ema {e.dtype}, "
+                             f"model {param.dtype})")
         if e.numel():
+            if e.dtype == torch.complex64:
+                e, param = torch.view_as_real(e), torch.view_as_real(param)
             pairs.append((name, e, param))
     emas, params, numels = [], [], []
     device = None

@@ -25,12 +25,19 @@ import warnings
 
 import numpy as np
 import torch
+from torch.utils._foreach_utils import _group_tensors_by_device_and_dtype
 
 from . import _capi
 
 __all__ = ["AdamW", "clip_grad_norm_"]
 
 _UNSUPPORTED = ("amsgrad", "maximize", "capturable", "differentiable")
+
+
+def _real(t):
+    """t itself when fp32; its fp32 [..., 2] view when complex64 -- how torch's foreach AdamW (`_view_as_real`) and the
+    kernels see a complex tensor, element for element"""
+    return torch.view_as_real(t) if t.dtype == torch.complex64 else t
 
 
 def _check_group(group):
@@ -62,8 +69,9 @@ def _check_group(group):
 class AdamW(torch.optim.AdamW):
     """torch.optim.AdamW whose step() runs one sm_90a kernel per param group, bit-identical to torch's foreach step.
 
-    Supported: fp32 dense CUDA params on one device per group, with contiguous grads and state.  Anything else raises
-    before any tensor is written: there is no CPU or eager fallback."""
+    Supported: fp32 or complex64 dense CUDA params on one device per group, with contiguous grads and state.  A complex64
+    param (the RoPE decoder's `freqs_1d`) is stepped through its real view, as torch's foreach step does.  Anything else
+    raises before any tensor is written: there is no CPU or eager fallback."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2, amsgrad=False, *,
                  maximize=False, foreach=None, capturable=False, differentiable=False, fused=None):
@@ -81,8 +89,9 @@ class AdamW(torch.optim.AdamW):
                 continue
             if g.is_sparse or g.layout != torch.strided or p.layout != torch.strided:
                 raise ValueError(f"AdamW: param {i}: sparse params or grads are not supported")
-            if p.dtype != torch.float32 or g.dtype != torch.float32:
-                raise ValueError(f"AdamW: param {i}: fp32 params and grads are required (param {p.dtype}, grad {g.dtype})")
+            if p.dtype not in (torch.float32, torch.complex64) or g.dtype != p.dtype:
+                raise ValueError(f"AdamW: param {i}: fp32 or complex64 params with grads of the same dtype are required "
+                                 f"(param {p.dtype}, grad {g.dtype})")
             if not p.is_cuda or not g.is_cuda:
                 raise _capi.XqError(f"AdamW: param {i}: CUDA tensors are required, there is no CPU path "
                                     f"(param on {p.device}, grad on {g.device})")
@@ -96,7 +105,7 @@ class AdamW(torch.optim.AdamW):
             for t in tensors:
                 if t.device != device:
                     raise ValueError(f"AdamW: param {i}: tensors on {t.device}, expected {device}")
-                if t.dtype != torch.float32 or t.shape != p.shape:
+                if t.dtype != p.dtype or t.shape != p.shape:
                     raise ValueError(f"AdamW: param {i}: state {tuple(t.shape)} {t.dtype} does not match the param")
                 if not t.is_contiguous():
                     raise ValueError(f"AdamW: param {i}: param, grad and state must be contiguous")
@@ -129,10 +138,10 @@ class AdamW(torch.optim.AdamW):
                     st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                     st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                 steps.append(st["step"])
-                ps.append(p)
-                gs.append(g)
-                ms.append(st["exp_avg"])
-                vs.append(st["exp_avg_sq"])
+                ps.append(_real(p))
+                gs.append(_real(g))
+                ms.append(_real(st["exp_avg"]))
+                vs.append(_real(st["exp_avg_sq"]))
             # the step counters and scalars exactly as torch/optim/adam.py::_multi_tensor_adam computes them
             if steps[0].is_cpu:
                 torch._foreach_add_(steps, torch.tensor(1.0, device="cpu"), alpha=1.0)
@@ -173,8 +182,8 @@ def _check_grads(grads):
     for i, g in enumerate(grads):
         if g.is_sparse or g.layout != torch.strided:
             raise ValueError(f"clip_grad_norm_: grad {i}: sparse grads are not supported")
-        if g.dtype != torch.float32:
-            raise ValueError(f"clip_grad_norm_: grad {i}: fp32 grads are required (got {g.dtype})")
+        if g.dtype not in (torch.float32, torch.complex64):
+            raise ValueError(f"clip_grad_norm_: grad {i}: fp32 or complex64 grads are required (got {g.dtype})")
         if not g.is_contiguous():
             raise ValueError(f"clip_grad_norm_: grad {i}: contiguous grads are required")
     for i, g in enumerate(grads):
@@ -191,11 +200,14 @@ def _check_grads(grads):
 def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=False, foreach=None):
     """torch.nn.utils.clip_grad_norm_ (torch 2.11) for fp32 CUDA grads on one device, with the same bits.
 
+    A complex64 grad counts as its real view (the norm of a complex tensor is that of its real and imaginary parts) and is
+    scaled component-wise (DESIGN.md section 8 states where that differs from torch's complex multiply).
     The per-tensor norms are one xq_grad_norm call (bit-identical to torch._foreach_norm), the total norm and the clip
     coefficient are torch's own ops on them, and the grads are scaled by one xq_grad_scale call that reads the coefficient on
     the device, so nothing synchronises unless `error_if_nonfinite` asks to.  Returns the total norm, as torch does.
 
-    Raises before anything is written on norm_type != 2, foreach=False, non-fp32, sparse or non-contiguous grads, grads on more
+    Raises before anything is written on norm_type != 2, foreach=False, grads neither fp32 nor complex64, sparse or
+    non-contiguous grads, grads on more
     than one device, and CPU grads (_capi.XqError: there is no CPU path)."""
     if isinstance(parameters, torch.Tensor):
         parameters = [parameters]
@@ -215,6 +227,8 @@ def clip_grad_norm_(parameters, max_norm, norm_type=2.0, error_if_nonfinite=Fals
         return torch.tensor(0.0)
     max_norm = float(max_norm)
     device = _check_grads(grads)
+    # the order of torch's per-dtype groups, which is the order of the norms its total norm sums (one group for fp32 grads)
+    grads = [_real(g) for ([gs], _) in _group_tensors_by_device_and_dtype([grads]).values() for g in gs]
     ptrs = np.array([g.data_ptr() for g in grads], dtype=np.uint64)
     numel = np.array([g.numel() for g in grads], dtype=np.int64)
     n = len(grads)

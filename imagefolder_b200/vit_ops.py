@@ -538,9 +538,98 @@ class _QKVAttention(torch.autograd.Function):
         return dy, dW, db, None
 
 
+_ROPE_IMG = 256                # image tokens xq_vit_rope_fwd / _bwd cover (a 16 x 16 grid)
+_ROPE_WS = {}
+
+
+def rope_forward(qkv, freqs, freqs_1d_real, num_heads: int, P: int):
+    """q / k of the packed qkv bf16 or fp16 [B,N,3*H*64] rotated (xq_vit_rope_fwd) into a new packed tensor; freqs fp32
+    [2,H*32], freqs_1d_real fp32 [L,32,2] (view_as_real of the complex table)."""
+    B, N, _ = qkv.shape
+    out = torch.empty_like(qkv)
+    name, fn = _entry("xq_vit_rope_fwd", qkv.dtype)
+    _call(name, 1, fn, _ptr(qkv), _ptr(out), _ptr(freqs), _ptr(freqs_1d_real), B, N, num_heads, 64, P, _ROPE_IMG,
+          freqs_1d_real.shape[0], _stream(qkv.device), nbytes=qkv.numel() * 4)
+    return out
+
+
+def rope_backward(qkv, g, freqs, freqs_1d_real, num_heads: int, P: int):
+    """d(rotated qkv) -> (d(qkv) in qkv's dtype, qkv-bias gradient fp32 [3*H*64], d freqs fp32 [2,H*32], d freqs_1d fp32
+    [L,32,2]) through xq_vit_rope_bwd: deterministic sums, no atomics."""
+    B, N, C3 = qkv.shape
+    L = freqs_1d_real.shape[0]
+    g = g.contiguous()
+    dqkv = torch.empty_like(qkv)
+    db = torch.empty(C3, dtype=torch.float32, device=qkv.device)
+    dfreqs = torch.empty_like(freqs)
+    d1 = torch.empty_like(freqs_1d_real)
+    nbytes = int(_lib().xq_vit_rope_bwd_workspace_bytes(B, N, num_heads, L))
+    key = (qkv.device.index, torch.cuda.current_stream(qkv.device).cuda_stream)
+    ws = _ROPE_WS.get(key)                      # one workspace per (device, stream): calls on a stream are ordered
+    if ws is None or ws.numel() < nbytes:
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=qkv.device)
+        _ROPE_WS[key] = ws
+    name, fn = _entry("xq_vit_rope_bwd", qkv.dtype)
+    _call(name, 2, fn, _ptr(qkv), _ptr(g), _ptr(freqs), _ptr(freqs_1d_real), B, N, num_heads, 64, P, _ROPE_IMG, L,
+          _ptr(dqkv), _ptr(db), _ptr(dfreqs), _ptr(d1), _ptr(ws), ws.numel(), _stream(qkv.device),
+          nbytes=qkv.numel() * 6 + ws.numel() * 2)
+    return dqkv, db, dfreqs, d1
+
+
+class _RoPEQKVAttention(torch.autograd.Function):
+    """RoPEAttention.forward (vision_transformer.py:238-270) up to the proj GEMM as one autograd node: qkv = y W^T (+ b)
+    [library GEMM] -> q / k rotated [xq_vit_rope_fwd] -> attention [xq_vit_attn_fwd]; the backward runs xq_vit_attn_bwd,
+    xq_vit_rope_bwd and the two library GEMMs.  The qkv-bias gradient is the column sum of the gradient BEFORE the rotation,
+    which the RoPE backward computes; the attention backward's column sums (of the rotated gradient) are not used.  Saves the
+    unrotated qkv next to the rotated one: one more [B,N,3C] 16-bit tensor per layer (DESIGN.md section 0)."""
+
+    @staticmethod
+    def forward(ctx, y, W, b, freqs, freqs_1d_real, num_heads: int, P: int):
+        B, N, C = y.shape
+        Wb = W.to(y.dtype)
+        y2 = y.reshape(B * N, C)
+        qkv = (torch.addmm(b.to(y.dtype), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * C)
+        freqs, freqs_1d_real = freqs.contiguous(), freqs_1d_real.contiguous()
+        rot = rope_forward(qkv, freqs, freqs_1d_real, num_heads, P)
+        out, lse2 = attn_tc_forward(rot, num_heads)
+        ctx.save_for_backward(y, Wb, qkv, rot, out, lse2, freqs, freqs_1d_real)
+        ctx.cfg = (num_heads, P)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        y, Wb, qkv, rot, out, lse2, freqs, freqs_1d_real = ctx.saved_tensors
+        H, P = ctx.cfg
+        B, N, C = y.shape
+        drot = attn_tc_backward(rot, out, lse2, g, H)
+        dqkv, db, dfreqs, d1 = rope_backward(qkv, drot, freqs, freqs_1d_real, H, P)
+        d2 = dqkv.view(B * N, 3 * C)
+        need = ctx.needs_input_grad
+        dy = (d2 @ Wb).view(B, N, C) if need[0] else None
+        dW = (d2.t() @ y.reshape(B * N, C)).float() if need[1] else None
+        return dy, dW, (db if need[2] else None), (dfreqs if need[3] else None), (d1 if need[4] else None), None, None
+
+
+def rope_tc_ok(attn, y) -> bool:
+    """the RoPE kernels cover what DINOv2Decoder(use_rope=True) builds: the attn_tc_ok gates, mixed frequencies, a 16 x 16
+    image grid and a sequence of exactly prefix + 256 + latent tokens"""
+    P, L = attn.num_prefix_tokens, attn.num_latent_tokens
+    return (attn_tc_ok(attn, y) and attn.rope_mixed and attn.num_image_tokens == _ROPE_IMG and P >= 0 and L >= 1
+            and y.shape[1] == P + _ROPE_IMG + L and attn.num_heads <= 64
+            and tuple(attn.freqs.shape) == (2, attn.num_heads * 32) and tuple(attn.freqs_1d.shape) == (L, 32))
+
+
 def attention_forward(attn, y):
-    """Attention.forward (vision_transformer.py:173-197, no mask) -> (branch, bias to fold into the next residual_ln).
-    On the wgmma kernels the proj GEMM leaves its bias to the caller; otherwise the module's own forward, bias included."""
+    """Attention.forward (vision_transformer.py:173-197, no mask) or RoPEAttention.forward (:238-270) -> (branch, bias to fold
+    into the next residual_ln).  On the wgmma (and RoPE) kernels the proj GEMM leaves its bias to the caller; otherwise the
+    module's own forward, bias included."""
+    from .dino_enc.vision_transformer import RoPEAttention      # imported here: dino_enc imports this module
+    if isinstance(attn, RoPEAttention):
+        if not rope_tc_ok(attn, y):
+            return attn(y), None
+        o = _RoPEQKVAttention.apply(y, attn.qkv.weight, attn.qkv.bias, attn.freqs, torch.view_as_real(attn.freqs_1d),
+                                    attn.num_heads, attn.num_prefix_tokens)
+        return F.linear(o, attn.proj.weight), attn.proj.bias
     if not attn_tc_ok(attn, y):
         return attn(y), None
     o = _QKVAttention.apply(y, attn.qkv.weight, attn.qkv.bias, attn.num_heads)

@@ -280,6 +280,36 @@ int xq_vit_swiglu_bwd(const void *pre, const float *bias, const void *gy, void *
 int xq_vit_swiglu_fwd_f16(const void *pre, const float *bias, void *act, int M, int H, void *stream);
 int xq_vit_swiglu_bwd_f16(const void *pre, const float *bias, const void *gy, void *d_pre, float *g_bias, int M, int H,
                           void *stream);
+/*   Rotary position embedding of the RoPE decoder (DINOv2Decoder(use_rope=True)): replaces the two apply_rotary_emb calls of
+ *   RoPEAttention.forward, tokenizer/tokenizer_image/dino_enc/vision_transformer.py:246-259 (helpers :58-142), with
+ *   rope_mixed=True.  Token order [prefix P | image I | latent L], P + I + L == N (else XQ_ERR_ARG), I == 256 and
+ *   head_dim == 64 (else XQ_ERR_UNSUPPORTED), 1 <= H <= 64, L >= 1; every pointer 16-byte aligned (else XQ_ERR_ARG).
+ *     qkv       bf16 [B,N,3,H,64]  the packed qkv projection (read only)
+ *     freqs     fp32 [2,H*32]      RoPEAttention.freqs: row 0 = fx, row 1 = fy (freqs.view(2,H,32))
+ *     freqs_1d  fp32 [L,32,2]      torch.view_as_real(RoPEAttention.freqs_1d)
+ *   forward:  out = qkv with q / k pair j of head h (elements 2j, 2j+1) multiplied by c in fp32 and rounded once:
+ *               image token i = n - P:   c = polar(1, fl(fl(i mod 16 * fx[h,j]) + fl(i div 16 * fy[h,j]))), sincosf
+ *               latent token l = n-P-I:  c = freqs_1d[l,j]
+ *             prefix tokens and v are copied bit for bit.  `out` is what xq_vit_attn_fwd consumes.
+ *   backward: d_out = d(out) (xq_vit_attn_bwd's dqkv) ->
+ *               d_qkv      [B,N,3,H,64]  conj(c) d_out for rotated q / k pairs (rounded once), d_out elsewhere
+ *               g_bias     fp32 [3*H*64] column sums of the rounded d_qkv (the qkv-bias gradient)
+ *               g_freqs    fp32 [2,H*32] sum_{b,n,q/k} t_{x|y}(n) (g_i y_r - g_r y_i),  y = x c in fp32
+ *               g_freqs_1d fp32 [L,32,2] sum_{b,h,q/k} conj(x) g  (torch's complex-gradient convention)
+ *             g_bias / g_freqs / g_freqs_1d may each be NULL.  Per-CTA partials go to the caller's workspace (16-byte
+ *             aligned, xq_vit_rope_bwd_workspace_bytes; 0 for invalid sizes) and are summed in a fixed order: no atomics,
+ *             every output is bitwise reproducible.  2 launches. */
+int xq_vit_rope_fwd(const void *qkv, void *out, const float *freqs, const float *freqs_1d, int B, int N, int H, int head_dim,
+                    int P, int I, int L, void *stream);
+int xq_vit_rope_fwd_f16(const void *qkv, void *out, const float *freqs, const float *freqs_1d, int B, int N, int H,
+                        int head_dim, int P, int I, int L, void *stream);
+size_t xq_vit_rope_bwd_workspace_bytes(int B, int N, int H, int L);
+int xq_vit_rope_bwd(const void *qkv, const void *d_out, const float *freqs, const float *freqs_1d, int B, int N, int H,
+                    int head_dim, int P, int I, int L, void *d_qkv, float *g_bias, float *g_freqs, float *g_freqs_1d,
+                    void *workspace, size_t workspace_bytes, void *stream);
+int xq_vit_rope_bwd_f16(const void *qkv, const void *d_out, const float *freqs, const float *freqs_1d, int B, int N, int H,
+                        int head_dim, int P, int I, int L, void *d_qkv, float *g_bias, float *g_freqs, float *g_freqs_1d,
+                        void *workspace, size_t workspace_bytes, void *stream);
 
 /*   Flash attention of the ViT blocks, head_dim 64, no mask, no dropout (Attention.forward,
  *   tokenizer/tokenizer_image/dino_enc/vision_transformer.py:173-197: F.scaled_dot_product_attention on
