@@ -51,6 +51,8 @@ F16_TWINS = [
 SWIGLU_ENTRIES = ["xq_vit_swiglu_fwd", "xq_vit_swiglu_bwd", "xq_vit_fc1_swiglu_fwd", "xq_vit_fc2_dswiglu_bwd"]
 # the RoPE decoder's q / k rotation (csrc/rope_kernel.cu), with `_f16` twins in the same sense
 ROPE_ENTRIES = ["xq_vit_rope_fwd", "xq_vit_rope_bwd"]
+# the class-token attention of a frozen teacher's last block (csrc/attn_kernel.cu), with an `_f16` twin in the same sense
+ATTN_CLS_ENTRIES = ["xq_vit_attn_fwd_cls"]
 
 
 def lib() -> ctypes.CDLL:
@@ -122,6 +124,8 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_gelu_bwd.argtypes = [vp, f32p, vp, vp, f32p, c_int, c_int, vp]
     L.xq_vit_attn_fwd.restype = c_int
     L.xq_vit_attn_fwd.argtypes = [vp, vp, f32p, c_int, c_int, c_int, c_int, c_float, vp]
+    L.xq_vit_attn_fwd_cls.restype = c_int
+    L.xq_vit_attn_fwd_cls.argtypes = [vp, vp, c_int, c_int, c_int, c_int, c_float, vp]
     L.xq_vit_attn_bwd_workspace_bytes.restype = c_size_t
     L.xq_vit_attn_bwd_workspace_bytes.argtypes = [c_int, c_int, c_int]
     L.xq_vit_attn_bwd.restype = c_int
@@ -149,7 +153,7 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_rope_bwd.restype = c_int
     L.xq_vit_rope_bwd.argtypes = [vp, vp, f32p, f32p] + [c_int] * 7 + [vp, f32p, f32p, f32p, vp, c_size_t, vp]
     # fp16 twins of the 16-bit ViT entry points: the same argument lists
-    for name in F16_TWINS + SWIGLU_ENTRIES + ROPE_ENTRIES:
+    for name in F16_TWINS + SWIGLU_ENTRIES + ROPE_ENTRIES + ATTN_CLS_ENTRIES:
         twin = getattr(L, name + "_f16")
         twin.restype = c_int
         twin.argtypes = getattr(L, name).argtypes
@@ -273,4 +277,4 @@ EXPORTED_SYMBOLS = [
     "xq_ema_update", "xq_adamw_step", "xq_grad_norm_workspace_bytes", "xq_grad_norm", "xq_grad_scale", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
     "xq_vit_rope_bwd_workspace_bytes",
 ] + [n + "_f16" for n in F16_TWINS] + SWIGLU_ENTRIES + [n + "_f16" for n in SWIGLU_ENTRIES] + ROPE_ENTRIES + [
-    n + "_f16" for n in ROPE_ENTRIES]
+    n + "_f16" for n in ROPE_ENTRIES] + ATTN_CLS_ENTRIES + [n + "_f16" for n in ATTN_CLS_ENTRIES]

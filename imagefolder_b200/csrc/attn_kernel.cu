@@ -719,6 +719,117 @@ static int attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
     return XQ_OK;
 }
 
+// ---- class-token attention (inference) ------------------------------------------------------------------------------
+// The last block of a frozen teacher whose output is the class token needs the attention output of query row 0 only, over
+// all N keys.  That is B*H*N*64 multiply-adds: CUDA cores, one CTA of AC_THREADS per (b, h), fp32 throughout, the scores of
+// the (b, h) row in shared memory.  Every sum has a fixed order (no atomics), so repeated calls agree bit for bit:
+//   scores   thread t owns keys t, t + AC_THREADS, ...: s_n = q . k_n summed over d = 0..63 in order
+//   max      per-thread, warp butterfly, then the AC_WARPS warp maxima in order
+//   sum      p_n = exp2(c (s_n - m)) written back over s_n; per-thread sums in key order, a warp butterfly, the warp sums
+//            in warp order
+//   P V      lane l owns dims 2l, 2l + 1, warp w keys w, w + AC_WARPS, ...; the AC_WARPS partial rows are added in warp order,
+//            divided by l and rounded once
+constexpr int AC_THREADS = 256, AC_WARPS = AC_THREADS / 32;
+constexpr int AC_MAX_N = 8192;              // scores in dynamic shared memory: 32 KB at the limit
+
+__device__ __forceinline__ float ac_warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ float ac_warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+template <typename E>
+__global__ void __launch_bounds__(AC_THREADS)
+attn_cls_kernel(const typename E::T *__restrict__ qkv, typename E::T *__restrict__ out, int N, int H, float c) {
+    using T = typename E::T;
+    using T2 = typename E::T2;
+    extern __shared__ float ac_s[];                       // [N] scores, then probabilities
+    __shared__ float q[AT_D];
+    __shared__ float red[AC_WARPS];
+    __shared__ float2 part[AC_WARPS][32];
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int b = blockIdx.x / H, h = blockIdx.x - b * H;
+    const size_t row = (size_t)3 * H * AT_D;              // elements per token of the packed [N,3,H,64] qkv
+    const T *base = qkv + (size_t)b * N * row + (size_t)h * AT_D;      // q of token 0; k at + H*64, v at + 2*H*64
+    if (tid < AT_D) q[tid] = E::to(base[tid]);
+    __syncthreads();
+
+    float m = -INFINITY;
+    for (int n = tid; n < N; n += AC_THREADS) {
+        const uint4 *k = reinterpret_cast<const uint4 *>(base + (size_t)n * row + (size_t)H * AT_D);
+        float s = 0.f;
+#pragma unroll
+        for (int i = 0; i < AT_D / 8; ++i) {
+            const uint4 u = k[i];
+            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                s += q[8 * i + 2 * j] * E::lo(w[j]);
+                s += q[8 * i + 2 * j + 1] * E::hi(w[j]);
+            }
+        }
+        ac_s[n] = s;
+        m = fmaxf(m, s);
+    }
+    m = ac_warp_max(m);
+    if (lane == 0) red[warp] = m;
+    __syncthreads();
+    m = red[0];
+#pragma unroll
+    for (int w = 1; w < AC_WARPS; ++w) m = fmaxf(m, red[w]);
+    __syncthreads();                                      // every thread has read red[] before it holds the sums
+
+    float l = 0.f;
+    for (int n = tid; n < N; n += AC_THREADS) {
+        const float p = exp2f(c * (ac_s[n] - m));
+        ac_s[n] = p;
+        l += p;
+    }
+    l = ac_warp_sum(l);
+    if (lane == 0) red[warp] = l;
+    __syncthreads();                                      // the probabilities and the warp sums are complete
+    l = red[0];
+#pragma unroll
+    for (int w = 1; w < AC_WARPS; ++w) l += red[w];
+
+    float2 o = make_float2(0.f, 0.f);
+    const T *v = base + (size_t)2 * H * AT_D + 2 * lane;
+    for (int n = warp; n < N; n += AC_WARPS) {
+        const float p = ac_s[n];
+        const float2 x = E::to2(*reinterpret_cast<const T2 *>(v + (size_t)n * row));
+        o.x += p * x.x;
+        o.y += p * x.y;
+    }
+    part[warp][lane] = o;
+    __syncthreads();
+    if (warp == 0) {
+        float2 a = part[0][lane];
+#pragma unroll
+        for (int w = 1; w < AC_WARPS; ++w) { a.x += part[w][lane].x; a.y += part[w][lane].y; }
+        *reinterpret_cast<T2 *>(out + (size_t)b * H * AT_D + (size_t)h * AT_D + 2 * lane) = E::from2(a.x / l, a.y / l);
+    }
+}
+
+template <typename E>
+static int attn_fwd_cls(const void *qkv, void *out, int B, int N, int H, int head_dim, float scale, void *stream) {
+    using T = typename E::T;
+    if (!qkv || !out || B <= 0 || N <= 0 || H <= 0) return XQ_ERR_ARG;
+    if (head_dim != AT_D) return XQ_ERR_UNSUPPORTED;
+    if (((uintptr_t)qkv & 15) || ((uintptr_t)out & 15)) return XQ_ERR_ARG;
+    if (N > AC_MAX_N) return XQ_ERR_UNSUPPORTED;
+    if ((long long)B * H > 0x7fffffffLL) return XQ_ERR_ARG;
+    const float c = scale * 1.4426950408889634f;
+    attn_cls_kernel<E><<<(unsigned)(B * H), AC_THREADS, (size_t)N * sizeof(float), (cudaStream_t)stream>>>(
+        (const T *)qkv, (T *)out, N, H, c);
+    XQ_LAUNCH_CHECK("attn_cls_kernel");
+    return XQ_OK;
+}
+
 }  // namespace xq
 
 extern "C" {
@@ -742,6 +853,13 @@ int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H
 }
 int xq_vit_attn_fwd_f16(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream) {
     return xq::attn_fwd<xqtc::F16>(qkv, out, lse2, B, N, H, head_dim, scale, stream);
+}
+
+int xq_vit_attn_fwd_cls(const void *qkv, void *out, int B, int N, int H, int head_dim, float scale, void *stream) {
+    return xq::attn_fwd_cls<xqtc::Bf16>(qkv, out, B, N, H, head_dim, scale, stream);
+}
+int xq_vit_attn_fwd_cls_f16(const void *qkv, void *out, int B, int N, int H, int head_dim, float scale, void *stream) {
+    return xq::attn_fwd_cls<xqtc::F16>(qkv, out, B, N, H, head_dim, scale, stream);
 }
 
 }  // extern "C"

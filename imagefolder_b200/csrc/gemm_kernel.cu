@@ -98,7 +98,8 @@ struct GmClock {
 };
 #endif
 
-// EPI 1: forward  -- the staged tile is the pre-activation: TMA-stored as it stands (tmP); GELU(pre + bias) -> tmO.
+// EPI 1: forward  -- the staged tile is the pre-activation: TMA-stored as it stands (tmP, only when store_pre: the inference
+//                    form leaves `pre` unwritten and tmP unbuilt); GELU(pre + bias) -> tmO.
 // EPI 3 / 4: the SwiGLU forms of EPI 1 / 2 (N is 2H in the forward, H in the backward; the column mapping is above).
 // EPI 2: backward -- the staged tile is d_act; the producer loads the stored pre-activation tile (tmP);
 //                    d_act * GELU'(pre + bias) -> tmO; column sums of the ROUNDED result -> dbias (fp32 atomics at the end).
@@ -113,7 +114,7 @@ __global__ void __launch_bounds__(GM_THREADS, 1)
 mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmO,
                 const __grid_constant__ CUtensorMap tmU, const __grid_constant__ CUtensorMap tmL, const float *__restrict__ bias,
-                float *__restrict__ dbias, int M, int N, int K, int R) {
+                float *__restrict__ dbias, int M, int N, int K, int R, bool store_pre) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *base = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t *stg = base + GM_STG_OFF;
@@ -205,7 +206,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         for (int mb = mb0; mb < nM; mb += mstep, ++t) {
             uint8_t *aux = base + GM_AUX_OFF + (t & 1) * GM_TILE_BYTES;
             mbar_wait(stg_full, t & 1);
-            if (te == 0) {
+            if (te == 0 && store_pre) {
                 tma_store_3d(&tmP, stg, j0, mb * GM_BM, 0);
                 tma_store_3d(&tmP, stg + GM_HALF_BYTES, H + j0, mb * GM_BM, 0);
                 bulk_commit();
@@ -237,7 +238,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             if (te == 0) {
                 tma_store_3d(&tmO, aux, j0, mb * GM_BM, 0);
                 bulk_commit();
-                bulk_wait_read<1>();                             // this tile's `pre` stores and the previous `act` store
+                bulk_wait_read<1>();                             // this tile's `pre` stores (if any) and the previous `act` store
                 mbar_arrive(stg_empty);
             }
         }
@@ -328,7 +329,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             uint8_t *aux = base + GM_AUX_OFF + (t & 1) * GM_TILE_BYTES;
             mbar_wait(stg_full, t & 1);
             if (EPI == 1) {
-                if (te == 0) {
+                if (te == 0 && store_pre) {
                     tma_store_3d(&tmP, stg, nb * GM_BN, mb * GM_BM, 0);
                     tma_store_3d(&tmP, stg + GM_HALF_BYTES, nb * GM_BN + 64, mb * GM_BM, 0);
                     bulk_commit();
@@ -407,8 +408,8 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 tma_store_3d(&tmO, aux, nb * GM_BN, mb * GM_BM, 0);
                 tma_store_3d(&tmO, aux + GM_HALF_BYTES, nb * GM_BN + 64, mb * GM_BM, 0);
                 bulk_commit();
-                // forward: every store but the one just issued has read its tile -- this tile's `pre` (the staging tile) and
-                // the previous tile's `act` (the auxiliary tile the next tile writes)
+                // forward: every store but the one just issued has read its tile -- this tile's `pre` (the staging tile), if
+                // stored, and the previous tile's `act` (the auxiliary tile the next tile writes)
                 if (EPI == 1) bulk_wait_read<1>();
                 mbar_arrive(stg_empty);
             }
@@ -492,7 +493,8 @@ static int gm_check_lora(const void *u, const void *l, int R) {
     return XQ_OK;
 }
 
-// `pre` is the pre-activation tensor (written by the forward, read by the backward), `out` the epilogue's result (act / d_pre)
+// `pre` is the pre-activation tensor (written by the forward, read by the backward), `out` the epilogue's result (act / d_pre).
+// A forward with pre == NULL stores only `out`: no tensor map is built for `pre` (the kernel gets a copy of tmO it never uses).
 template <typename E, int EPI>
 // R > 0 adds the rank-R stage u [M,R] . l [N,R]^T; R == 0 ignores u / l
 static int gm_launch(const void *a, const void *b, const void *u, const void *l, const void *pre, void *out, const float *bias,
@@ -507,8 +509,10 @@ static int gm_launch(const void *a, const void *b, const void *u, const void *l,
     CUtensorMap tmA, tmB, tmP, tmO;
     if (!tensor_map_16_3d(&tmA, E::TMAP, a, K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BM) ||
         !tensor_map_16_3d(&tmB, E::TMAP, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, EPI == 3 ? 64 : GM_BN) ||
-        !tensor_map_16_3d(&tmP, E::TMAP, pre, pre_cols, M, 1, pre_cols * 2, (uint64_t)M * pre_cols * 2, GM_BM) ||
         !tensor_map_16_3d(&tmO, E::TMAP, out, out_cols, M, 1, out_cols * 2, (uint64_t)M * out_cols * 2, GM_BM))
+        return XQ_ERR_UNSUPPORTED;
+    tmP = tmO;
+    if (pre && !tensor_map_16_3d(&tmP, E::TMAP, pre, pre_cols, M, 1, pre_cols * 2, (uint64_t)M * pre_cols * 2, GM_BM))
         return XQ_ERR_UNSUPPORTED;
     CUtensorMap tmU = tmA, tmL = tmB;
     if (R > 0 && (!tensor_map_16_3d(&tmU, E::TMAP, u, R, M, 1, (uint64_t)R * 2, (uint64_t)M * R * 2, GM_BM) ||
@@ -520,7 +524,8 @@ static int gm_launch(const void *a, const void *b, const void *u, const void *l,
     if (per_col > nM) per_col = nM;
     // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
     if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N * (EPI == 4 ? 2 : 1), st));
-    mlp_gemm_kernel<E, EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, tmU, tmL, bias, dbias, M, N, K, R);
+    mlp_gemm_kernel<E, EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, tmU, tmL, bias, dbias, M, N, K, R,
+                                                                        pre != nullptr);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
     return XQ_OK;
 }
@@ -531,7 +536,7 @@ namespace xq {
 
 template <typename E>
 static int fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream) {
-    if (int rc = gm_check(x, w, pre, act, bias, M, N, K)) return rc;
+    if (int rc = gm_check(x, w, act, pre ? pre : act, bias, M, N, K)) return rc;      // pre may be NULL (inference)
     return gm_launch<E, 1>(x, w, nullptr, nullptr, pre, act, bias, nullptr, M, N, K, 0, (cudaStream_t)stream);
 }
 
@@ -546,7 +551,7 @@ static int fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, co
 template <typename E>
 static int fc1_lora_gelu_fwd(const void *x, const void *w, const void *u, const void *b_lora, const float *bias, void *pre, void *act,
                              int M, int N, int K, int R, void *stream) {
-    if (int rc = gm_check(x, w, pre, act, bias, M, N, K)) return rc;
+    if (int rc = gm_check(x, w, act, pre ? pre : act, bias, M, N, K)) return rc;
     if (int rc = gm_check_lora(u, b_lora, R)) return rc;
     return gm_launch<E, 1>(x, w, u, b_lora, pre, act, bias, nullptr, M, N, K, R, (cudaStream_t)stream);
 }
@@ -565,7 +570,7 @@ static int fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v,
 template <typename E>
 static int fc1_swiglu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K, void *stream) {
     if (H <= 0 || H > (1 << 29)) return XQ_ERR_ARG;
-    if (int rc = gm_check(x, w, pre, act, bias, M, 2 * H, K)) return rc;
+    if (int rc = gm_check(x, w, act, pre ? pre : act, bias, M, 2 * H, K)) return rc;
     return gm_launch<E, 3>(x, w, nullptr, nullptr, pre, act, bias, nullptr, M, 2 * H, K, 0, (cudaStream_t)stream);
 }
 

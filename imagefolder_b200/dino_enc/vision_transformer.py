@@ -13,7 +13,10 @@ Parameter names (= checkpoint keys) are identical to timm's: patch_embed.proj, c
 pos_embed, blocks.{i}.{norm1,attn.qkv,attn.proj,ls1.gamma,norm2,mlp.fc1,mlp.fc2,ls2.gamma}, norm.
 
 GEMMs run on cuBLAS and attention on the fused SDPA library kernel (plain library calls); the
-elementwise / normalisation glue is what imagefolder_b200.vit_ops replaces with sm_90a kernels.
+elementwise / normalisation glue is what imagefolder_b200.vit_ops replaces with sm_90a kernels.  A frozen model (every
+parameter requires_grad=False: the semantic / detail guide teachers) called on a CUDA fp32 image that needs no gradient under
+bf16 / fp16 autocast runs `forward` / `forward_features` on those kernels too (vit_ops.frozen_forward); everything else
+runs the module path below.
 """
 from __future__ import annotations
 
@@ -23,6 +26,8 @@ from functools import partial
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from ..vit_ops import frozen_forward, frozen_path_ok
 
 
 def trunc_normal_(t, std=0.02):
@@ -359,6 +364,8 @@ class VisionTransformer(nn.Module):
         return self.pos_drop(x)
 
     def forward_features(self, x):
+        if frozen_path_ok(self, x):
+            return frozen_forward(self, x)      # a frozen teacher under bf16 / fp16 autocast: the fused kernels
         x = self.patch_embed(x)
         x = self._pos_embed(x)
         x = self.patch_drop(x)
@@ -376,6 +383,9 @@ class VisionTransformer(nn.Module):
         return x if pre_logits else self.head(x)
 
     def forward(self, x):
+        if self.global_pool == 'token' and frozen_path_ok(self, x):
+            # only row 0 of the final norm is read: the last block runs its attention, proj and MLP on the class rows
+            return self.head(self.head_drop(self.fc_norm(frozen_forward(self, x, cls_only=True))))
         return self.forward_head(self.forward_features(x))
 
 

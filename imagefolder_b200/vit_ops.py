@@ -10,7 +10,8 @@ than 64, attention dropout > 0 in training, qk_norm; no shipped config) run the 
 their attention.  The residual stream is fp32 and the GEMM operands are the autocast dtype, bf16 or fp16: the
 `_f16` twin of every entry point runs the same kernel instantiated for fp16.  That is what bf16 / fp16 autocast gives the
 reference, so the numerics are the reference's.  Without autocast (or under another autocast dtype) `run_blocks` takes the
-module path.
+module path.  `frozen_forward` runs a frozen VisionTransformer (the guide teachers) on the same block body (`block_forward`),
+without saved activations, and with a class-token-only last block for `forward`.
 """
 from __future__ import annotations
 
@@ -181,11 +182,19 @@ def mlp_tc_ok(y, fc1, fc2) -> bool:
             and fc1.weight.shape[0] // 128 <= _sm_count(y.device))
 
 
+def _keeps_pre(ctx) -> bool:
+    """whether a fused fc1 forward must store and save its pre-activation: only when some input needs a gradient.  A
+    forward whose inputs all do without one (a frozen teacher, a model with every parameter frozen) passes NULL for `pre`
+    -- the kernel then stores `act` only, the same bits -- and saves nothing for a backward that cannot run."""
+    return any(ctx.needs_input_grad)
+
+
 class _FusedMLP(torch.autograd.Function):
     """branch = fc2(GELU(fc1(y)))  WITHOUT the fc2 bias (folded into the next residual_ln), timm Mlp as called from Block.forward
     (dino_enc/vision_transformer.py:336-339).  The fc1 GEMM carries bias + GELU in its epilogue, the fc2 input-gradient GEMM carries
     GELU' and the fc1-bias gradient; the other GEMMs are library calls.  Same bits as F.linear + gelu_bias (the epilogues apply
-    the same device functions to the same rounded 16-bit values).  Operands, weights and outputs in y's dtype, bf16 or fp16."""
+    the same device functions to the same rounded 16-bit values).  Operands, weights and outputs in y's dtype, bf16 or fp16.
+    When no input needs a gradient (a frozen teacher) the fc1 GEMM writes no `pre` and nothing is saved (_keeps_pre)."""
 
     @staticmethod
     def forward(ctx, y, W1, b1, W2):
@@ -199,13 +208,15 @@ class _FusedMLP(torch.autograd.Function):
         W1b = W1.to(dt)
         W2b = W2.to(dt)
         b1f = b1.float()
-        pre = torch.empty(M, N, dtype=dt, device=y.device)
+        keep = _keeps_pre(ctx)
+        pre = torch.empty(M, N, dtype=dt, device=y.device) if keep else None
         act = torch.empty(M, N, dtype=dt, device=y.device)
         name, fn = _entry("xq_vit_fc1_gelu_fwd", dt)
         C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(b1f), C.ptr(pre), C.ptr(act), M, N, K,
-               C.stream_ptr(y.device), nbytes=M * K * 2 + N * K * 2 + M * N * 4, nflops=2.0 * M * N * K)
+               C.stream_ptr(y.device), nbytes=M * K * 2 + N * K * 2 + M * N * (4 if keep else 2), nflops=2.0 * M * N * K)
         branch = act @ W2b.t()
-        ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
+        if keep:
+            ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
         ctx.out_shape = y.shape[:-1] + (W2.shape[0],)
         ctx.in_shape = y.shape
         return branch.view(ctx.out_shape)
@@ -286,7 +297,8 @@ def swiglu_tc_ok(y, fc1, fc2) -> bool:
 class _FusedSwiGLU(torch.autograd.Function):
     """branch = fc2(silu(a) * c), [a | c] = fc1(y), WITHOUT the fc2 bias (folded into the next residual_ln): timm GluMlp as
     called from Block.forward.  The fc1 GEMM carries bias + SwiGLU in its epilogue, the fc2 input-gradient GEMM carries the
-    SwiGLU derivative and the fc1-bias gradient; the other GEMMs are library calls.  Same bits as F.linear + swiglu_bias."""
+    SwiGLU derivative and the fc1-bias gradient; the other GEMMs are library calls.  Same bits as F.linear + swiglu_bias.
+    No `pre` and nothing saved when no input needs a gradient (_keeps_pre)."""
 
     @staticmethod
     def forward(ctx, y, W1, b1, W2):
@@ -298,13 +310,16 @@ class _FusedSwiGLU(torch.autograd.Function):
         M = y2.shape[0]
         dt = y.dtype
         W1b, W2b, b1f = W1.to(dt), W2.to(dt), b1.float()
-        pre = torch.empty(M, N1, dtype=dt, device=y.device)
+        keep = _keeps_pre(ctx)
+        pre = torch.empty(M, N1, dtype=dt, device=y.device) if keep else None
         act = torch.empty(M, H, dtype=dt, device=y.device)
         name, fn = _entry("xq_vit_fc1_swiglu_fwd", dt)
         C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(b1f), C.ptr(pre), C.ptr(act), M, H, K,
-               C.stream_ptr(y.device), nbytes=M * K * 2 + N1 * K * 2 + M * N1 * 2 + M * H * 2, nflops=2.0 * M * N1 * K)
+               C.stream_ptr(y.device), nbytes=M * K * 2 + N1 * K * 2 + (M * N1 * 2 if keep else 0) + M * H * 2,
+               nflops=2.0 * M * N1 * K)
         branch = act @ W2b.t()
-        ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
+        if keep:
+            ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
         ctx.out_shape = y.shape[:-1] + (W2.shape[0],)
         ctx.in_shape = y.shape
         return branch.view(ctx.out_shape)
@@ -354,7 +369,8 @@ class _LoRAMLP(torch.autograd.Function):
       backward  d_pre = (g W2 + v A2) * GELU'(pre + b1), d_b1   xq_vit_fc2_lora_dgelu_bwd
                 dy = d_pre W1 + s1 (d_pre B1) A1, the four adapter gradients, and dW1 / dW2 / d_b1 only for parameters that
                 require grad (LoRA freezes them: their GEMMs are not run).
-    The base and rank-r products of `pre` / `d_act` share one fp32 accumulator and one rounding (DESIGN.md section 8)."""
+    The base and rank-r products of `pre` / `d_act` share one fp32 accumulator and one rounding (DESIGN.md section 8).
+    No `pre` and nothing saved when no input needs a gradient (_keeps_pre)."""
 
     @staticmethod
     def forward(ctx, y, W1, b1, W2, A1, B1, A2, B2, s1: float, s2: float):
@@ -370,15 +386,17 @@ class _LoRAMLP(torch.autograd.Function):
         A1b, B1b = _pad_rank(A1.to(bf), 0, R), _pad_rank(B1.to(bf), 1, R)           # [R, K], [N, R]
         A2b, B2b = _pad_rank(A2.to(bf), 0, R), _pad_rank(B2.to(bf), 1, R)           # [R, N], [Ko, R]
         u = _scaled_mm(y2, A1b.t(), s1)
-        pre = torch.empty(M, N, dtype=bf, device=y.device)
+        keep = _keeps_pre(ctx)
+        pre = torch.empty(M, N, dtype=bf, device=y.device) if keep else None
         act = torch.empty(M, N, dtype=bf, device=y.device)
         name, fn = _entry("xq_vit_fc1_lora_gelu_fwd", bf)
         C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(u), C.ptr(B1b), C.ptr(b1f),
                C.ptr(pre), C.ptr(act), M, N, K, R, C.stream_ptr(y.device),
-               nbytes=M * (K + R) * 2 + N * (K + R) * 2 + M * N * 4, nflops=2.0 * M * N * (K + R))
+               nbytes=M * (K + R) * 2 + N * (K + R) * 2 + M * N * (4 if keep else 2), nflops=2.0 * M * N * (K + R))
         h2 = _scaled_mm(act, A2b.t(), s2)
         branch = torch.addmm(act @ W2b.t(), h2, B2b.t())
-        ctx.save_for_backward(y2, pre, act, u, h2, W1b, W2b, b1f, A1b, B1b, A2b, B2b)
+        if keep:
+            ctx.save_for_backward(y2, pre, act, u, h2, W1b, W2b, b1f, A1b, B1b, A2b, B2b)
         ctx.cfg = (s1, s2, r)
         ctx.out_shape = y.shape[:-1] + (W2.shape[0],)
         ctx.in_shape = y.shape
@@ -479,6 +497,18 @@ def attn_tc_forward(qkv, num_heads: int):
           _stream(qkv.device), nbytes=qkv.numel() * 2 + out.numel() * 2 + lse2.numel() * 4,
           nflops=4.0 * B * num_heads * N * N * 64)
     return out, lse2
+
+
+def attn_cls_forward(qkv, num_heads: int):
+    """qkv bf16 or fp16 [B,N,3*H*64] -> the attention output of query row 0 only, [B,H*64] in qkv's dtype
+    (xq_vit_attn_fwd_cls: fp32 on CUDA cores, fixed summation order).  Inference only: there is no backward."""
+    B, N, C3 = qkv.shape
+    qkv = qkv.contiguous()
+    out = torch.empty(B, C3 // 3, dtype=qkv.dtype, device=qkv.device)
+    name, fn = _entry("xq_vit_attn_fwd_cls", qkv.dtype)
+    _call(name, 1, fn, _ptr(qkv), _ptr(out), B, N, num_heads, 64, 0.125, _stream(qkv.device),
+          nbytes=B * N * (C3 // 3) * 4 + out.numel() * 2)
+    return out
 
 
 _ATTN_WS = {}
@@ -768,6 +798,31 @@ def _droppath_scale(mod, batch: int, device):
     return t
 
 
+_NO_BRANCH = (None, None, None, None)
+
+
+def _mlp_tail(blk, x, y):
+    """the MLP half of Block.forward from norm2's output y: (branch, fc2 bias, ls2 gamma, drop-path scale) -- the residual add
+    that block_forward leaves to the next residual_ln"""
+    branch = mlp_forward(blk.mlp, y)              # fc1 bias in the GELU epilogue / kernel; fc2 bias folded into the next residual_ln
+    gamma = blk.ls2.gamma if hasattr(blk.ls2, "gamma") else None
+    return branch, blk.mlp.fc2.bias, gamma, _droppath_scale(blk.drop_path2, x.shape[0], x.device)
+
+
+def block_forward(blk, x, pending):
+    """Block.forward (vision_transformer.py:336-339) on the fused glue.  x: the fp32 residual stream [B,S,D] WITHOUT the
+    previous block's MLP branch, which arrives in `pending` = (branch, bias, ls gamma, drop-path scale) and is added by this
+    block's first residual_ln (_NO_BRANCH for the first block).  Returns (x, pending) in the same sense for the next block or
+    the final norm."""
+    Bn, dev = x.shape[0], x.device
+    x, y = residual_ln(x, *pending, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
+    a, a_bias = attention_forward(blk.attn, y)
+    g1 = blk.ls1.gamma if hasattr(blk.ls1, "gamma") else None
+    x, y = residual_ln(x, a, a_bias, g1,
+                       _droppath_scale(blk.drop_path1, Bn, dev), blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
+    return x, _mlp_tail(blk, x, y)
+
+
 def fused_path_ok(vit, x) -> bool:
     return (x.is_cuda and _autocast_half() is not None
             and vit.embed_dim in _SUPPORTED_D and isinstance(vit.norm_pre, nn.Identity))
@@ -785,20 +840,71 @@ def run_blocks(vit, x, attn_mask=None):
         else:
             x = vit.blocks(x)
         return vit.norm(x)
-    Bn = x.shape[0]
-    dev = x.device
     x = x.float()
-    branch = bias = gamma = rs = None
+    pending = _NO_BRANCH
     for blk in vit.blocks:
-        x, y = residual_ln(x, branch, bias, gamma, rs, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
-        a, a_bias = attention_forward(blk.attn, y)
-        g1 = blk.ls1.gamma if hasattr(blk.ls1, "gamma") else None
-        x, y = residual_ln(x, a, a_bias, g1,
-                           _droppath_scale(blk.drop_path1, Bn, dev), blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
-        branch = mlp_forward(blk.mlp, y)          # fc1 bias in the GELU epilogue / kernel; fc2 bias folded into the next residual_ln
-        bias = blk.mlp.fc2.bias
-        gamma = blk.ls2.gamma if hasattr(blk.ls2, "gamma") else None
-        rs = _droppath_scale(blk.drop_path2, Bn, dev)
+        x, pending = block_forward(blk, x, pending)
     norm = _live(vit.norm)
-    _, y = residual_ln(x, branch, bias, gamma, rs, norm.weight, norm.bias, norm.eps)
+    _, y = residual_ln(x, *pending, norm.weight, norm.bias, norm.eps)
     return y
+
+
+def frozen_path_ok(vit, x) -> bool:
+    """VisionTransformer.forward / forward_features take the frozen fused path (frozen_forward) when the model is a frozen
+    teacher under bf16 / fp16 autocast: x a CUDA fp32 image that needs no gradient, a supported width, and no parameter
+    that requires grad.  Anything else -- CPU, fp32 runs, a teacher a user has unfrozen -- runs the module path."""
+    return (x.is_cuda and x.dtype == torch.float32 and not x.requires_grad and _autocast_half() is not None
+            and vit.embed_dim in _SUPPORTED_D and not any(p.requires_grad for p in vit.parameters()))
+
+
+def _cls_tail_ok(vit, blk, y) -> bool:
+    """the class-token tail covers a plain Attention on the wgmma kernels with the class token in row 0"""
+    from .dino_enc.vision_transformer import RoPEAttention      # imported here: dino_enc imports this module
+    return (vit.has_class_token and not isinstance(blk.attn, RoPEAttention) and attn_tc_ok(blk.attn, y)
+            and y.shape[1] <= _ATTN_CLS_MAX_N)
+
+
+_ATTN_CLS_MAX_N = 8192         # sequence lengths xq_vit_attn_fwd_cls covers (include/xqb200.h)
+
+
+def frozen_forward(vit, x, cls_only: bool = False):
+    """VisionTransformer.forward_features of a frozen model (frozen_path_ok) on the fused kernels: image x fp32 [B,3,H,W] ->
+    norm(blocks(norm_pre(pos_embed(patch_embed(x))))) [B,S,D] in the autocast dtype, as run_blocks returns it.  Nothing is
+    saved for a backward and the fused MLP GEMMs write no pre-activation.
+
+    cls_only: row 0 only, [B,D] -- what forward() reads with global_pool 'token'.  The last block then computes its qkv GEMM
+    over every token (keys and values need them all), the attention of the class query alone (xq_vit_attn_fwd_cls), and the
+    proj GEMM, residual_ln, MLP and final norm on the B class rows."""
+    x = patch_embed(vit.patch_embed, x)
+    x = assemble_tokens(vit, vit._pos_embed, x, vit.num_prefix_tokens)
+    x = vit.patch_drop(x)
+    if isinstance(vit.norm_pre, nn.LayerNorm):
+        # the CLIP teacher: torch's layer_norm on the fp32 stream, the fp32 result autocast gives the module path
+        x = F.layer_norm(x.float(), vit.norm_pre.normalized_shape, vit.norm_pre.weight, vit.norm_pre.bias, vit.norm_pre.eps)
+    else:
+        x = vit.norm_pre(x)
+    x = x.float()
+    blocks = list(vit.blocks)
+    norm = _live(vit.norm)
+    pending = _NO_BRANCH
+    for blk in blocks[:-1] if cls_only else blocks:
+        x, pending = block_forward(blk, x, pending)
+    if cls_only:
+        blk = blocks[-1]
+        x_in = x
+        x, y = residual_ln(x_in, *pending, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
+        if not _cls_tail_ok(vit, blk, y):
+            x, pending = block_forward(blk, x_in, pending)       # the whole last block, then row 0 of the norm
+            _, y = residual_ln(x, *pending, norm.weight, norm.bias, norm.eps)
+            return y[:, 0]
+        attn = blk.attn
+        Bn, S, D = y.shape
+        Wb, y2 = attn.qkv.weight.to(y.dtype), y.reshape(Bn * S, D)
+        qkv = (torch.addmm(attn.qkv.bias.to(y.dtype), y2, Wb.t()) if attn.qkv.bias is not None else y2 @ Wb.t())
+        a = F.linear(attn_cls_forward(qkv.view(Bn, S, 3 * D), attn.num_heads), attn.proj.weight).view(Bn, 1, D)
+        g1 = blk.ls1.gamma if hasattr(blk.ls1, "gamma") else None
+        x, y = residual_ln(x[:, :1], a, attn.proj.bias, g1, _droppath_scale(blk.drop_path1, Bn, x.device),
+                           blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
+        pending = _mlp_tail(blk, x, y)
+    _, y = residual_ln(x, *pending, norm.weight, norm.bias, norm.eps)
+    return y[:, 0] if cls_only else y

@@ -321,6 +321,18 @@ int xq_vit_rope_bwd_f16(const void *qkv, const void *d_out, const float *freqs, 
 int xq_vit_attn_fwd(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream);
 int xq_vit_attn_fwd_f16(const void *qkv, void *out, float *lse2, int B, int N, int H, int head_dim, float scale, void *stream);
 
+/*   Class-token attention for inference: the output of xq_vit_attn_fwd's query row 0 only, over all N keys -- what the last
+ *   block of a frozen ViT needs when only its class token is read (VisionTransformer.forward with global_pool 'token').
+ *     qkv   bf16 [B,N,3,H,64]  the same packed projection xq_vit_attn_fwd reads
+ *     out   bf16 [B,H*64]      softmax(scale q_0 K^T) V per head, head-merged
+ *   fp32 throughout (q.k over the 64 dims, the max, exp2(scale*log2(e)*(s - m)), the sum, sum p v / l), rounded once at the
+ *   end.  CUDA cores, one CTA per (b, h); every sum has a fixed order (no atomics), so repeated calls agree bit for bit.
+ *   1 <= N <= 8192 (the scores of a row live in shared memory; else XQ_ERR_UNSUPPORTED).  NULL or non-16-byte-aligned
+ *   qkv / out, or B, N, H < 1, give XQ_ERR_ARG; head_dim != 64 gives XQ_ERR_UNSUPPORTED.  A refused call writes nothing.
+ *   The _f16 twin reads and writes fp16. */
+int xq_vit_attn_fwd_cls(const void *qkv, void *out, int B, int N, int H, int head_dim, float scale, void *stream);
+int xq_vit_attn_fwd_cls_f16(const void *qkv, void *out, int B, int N, int H, int head_dim, float scale, void *stream);
+
 /*   Backward of xq_vit_attn_fwd: d_out bf16 [B,N,H*64] -> dqkv bf16 [B,N,3,H,64] (the gradient of the packed projection,
  *   written in place of autograd's three permuted tensors + stack).  `out` and `lse2` are the forward's results.
  *   workspace (256-byte aligned, xq_vit_attn_bwd_workspace_bytes): fp32 dQ accumulator [B*H,N,64] (atomic adds across
@@ -372,6 +384,9 @@ int xq_diffaug_backward(const float *g, const float *rand01, int B, int C, int H
  * written by TMA stores (and pre read by TMA loads in the backward), so they must be 16-byte aligned like the operands.
  *   x [M,K], w [N,K] (fc1.weight as bf16)  ->  pre [M,N] = x w^T ,  act [M,N] = GELU(pre + bias)                               */
 int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream);
+/*   pre may be NULL (inference: no backward will read it): the kernel then stores act only, bit-identical to the call with
+ *   pre given.  The same holds for xq_vit_fc1_lora_gelu_fwd and xq_vit_fc1_swiglu_fwd and their _f16 twins; the backward
+ *   entry points still require pre.                                                                                      */
 /*  d_out [M,K] (gradient of the fc2 output), w2t [N,K] (fc2.weight TRANSPOSED, bf16), pre [M,N] (saved by the forward)
  *   ->  d_pre [M,N] = (d_out w2t^T) * GELU'(pre + bias) ,  d_bias [N] = column sums of the rounded d_pre                      */
 int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
