@@ -1022,45 +1022,51 @@ struct MsBwdSmem {
     float *My, *Mx;  // dense [H][P], [W][P]
     float *ratio;
     int *idx;
+    size_t floats;   // size of the whole carve
 };
-__host__ __device__ inline size_t ms_bwd_smem_floats(int C, int H, int W) {
-    size_t chw = (size_t)C * H * W, rp = (size_t)ms_rp(H, W);
-    size_t cpp = (size_t)C * ms_pp(H, W);
-    return 3 * chw /*F,S,du*/ + 2 * cpp /*u,dh padded*/ + (size_t)C * rp + chw /*tmp*/ + 8 * (size_t)(H + W) +
-           (size_t)H * H + (size_t)W * W + XQ_MAX_SCALES + rp + 16 + 8 + (size_t)C * C * 9 + C;
-}
-__device__ __forceinline__ MsBwdSmem ms_bwd_carve(float *base, int C, int H, int W) {
+// The one layout of the backward's shared memory: the launch sizes it with base = nullptr, the kernel carves it.
+// Buffers whose lifetimes within a scale do not overlap share storage:
+//   rows (gathered codes, pitch HW)  -> du : rows is dead once bicubic-up has written u; du is first written by the
+//                                            Phi^T pass, and read last by bicubic^T, before the next scale's gather
+//   tmp (bicubic^T intermediate)     -> dh : dh is dead once du and the dW / db partials are computed; tmp overwrites
+//                                            part of dh's zero border, which is re-zeroed after bicubic^T
+// At C = 32 and a 16 x 16 last scale that is 222,464 bytes (217.3 KiB) of the 227 KiB a CTA may have.
+__host__ __device__ inline MsBwdSmem ms_bwd_layout(float *base, int C, int H, int W) {
     MsBwdSmem s;
-    size_t chw = (size_t)C * H * W, rp = (size_t)ms_rp(H, W);
-    float *p = base;
-    size_t cpp = (size_t)C * ms_pp(H, W);
-    s.F = p; p += chw;
-    s.S = p; p += chw;
-    s.u = p; p += cpp;      // zero-padded planes
-    s.dh = p; p += cpp;     // zero-padded planes
-    s.du = p; p += chw;
-    s.tmp = p; p += chw;
-    s.rows = p; p += (size_t)C * rp;
-    s.wy = p; p += 4 * H;
-    s.wx = p; p += 4 * W;
-    s.iy = (int *)p; p += 4 * H;
-    s.ix = (int *)p; p += 4 * W;
-    s.My = p; p += (size_t)H * H;
-    s.Mx = p; p += (size_t)W * W;
-    s.ratio = p; p += XQ_MAX_SCALES;
-    s.idx = (int *)p; p += rp;
-    p = (float *)(((uintptr_t)p + 15) & ~(uintptr_t)15);    // 16-byte loads of the staged weights
-    s.w = p; p += (size_t)C * C * 9 + C;
+    const size_t chw = (size_t)C * H * W, rp = (size_t)ms_rp(H, W), cpp = (size_t)C * ms_pp(H, W);
+    size_t o = 0;   // offset in floats; base is 16-byte aligned
+    auto take = [&](size_t n) { float *q = base + o; o += n; return q; };
+    s.F = take(chw);
+    s.S = take(chw);
+    s.u = take(cpp);        // zero-padded planes
+    s.dh = take(cpp);       // zero-padded planes
+    s.tmp = s.dh;           // [C][H][P], P <= W: fits inside dh
+    s.du = take(chw);
+    s.rows = s.du;          // k-major [C][HW]
+    s.wy = take(4 * H);
+    s.wx = take(4 * W);
+    s.iy = (int *)take(4 * H);
+    s.ix = (int *)take(4 * W);
+    s.My = take((size_t)H * H);
+    s.Mx = take((size_t)W * W);
+    s.ratio = take(XQ_MAX_SCALES);
+    s.idx = (int *)take(rp);
+    o = (o + 3) & ~(size_t)3;    // 16-byte loads of the staged weights
+    s.w = take((size_t)C * C * 9 + C);
+    s.floats = o;
     return s;
+}
+__host__ __device__ inline size_t ms_bwd_smem_bytes(int C, int H, int W) {
+    return sizeof(float) * ms_bwd_layout(nullptr, C, H, W).floats;
 }
 
 __global__ void __launch_bounds__(MS_BWD_THREADS)
 ms_backward_kernel(const MsBwdArgs a) {
     extern __shared__ __align__(16) float smem[];
     const xq_ms_desc &d = a.d;
-    const int C = d.C, H = d.H, W = d.W, HW = H * W, CHW = C * HW, RP = ms_rp(H, W), SN = d.SN;
+    const int C = d.C, H = d.H, W = d.W, HW = H * W, CHW = C * HW, SN = d.SN;
     const bool bsq = ms_is_bsq(d.mode);
-    MsBwdSmem s = ms_bwd_carve(smem, C, H, W);
+    MsBwdSmem s = ms_bwd_layout(smem, C, H, W);
     // adapter so the forward primitives can be reused
     MsSmem fs;
     fs.rows = s.rows; fs.u = s.u; fs.idx = s.idx; fs.wy = s.wy; fs.wx = s.wx; fs.iy = s.iy; fs.ix = s.ix;
@@ -1075,7 +1081,6 @@ ms_backward_kernel(const MsBwdArgs a) {
     for (int i = tid; i < CHW; i += blockDim.x) {
         s.F[i] = a.F_last[(size_t)b * CHW + i];
         s.S[i] = 0.f;
-        s.tmp[i] = 0.f;
     }
     const int PW = ms_pw(W), PP = ms_pp(H, W);
     for (int i = tid; i < C * PP; i += blockDim.x) { s.u[i] = 0.f; s.dh[i] = 0.f; }
@@ -1103,7 +1108,7 @@ ms_backward_kernel(const MsBwdArgs a) {
             ms_cubic_tables(fs, P, H, W);
         }
         __syncthreads();
-        ms_gather(fs, a.E, C, R, RP, d.V, bsq, d.scaler[k]);
+        ms_gather(fs, a.E, C, R, HW, d.V, bsq, d.scaler[k]);     // rows shares du's storage: pitch HW
         if (P != H || P != W) {
             // dense transposes for the backward of the bicubic map
             for (int i = tid; i < H * P; i += blockDim.x) s.My[i] = 0.f;
@@ -1114,7 +1119,7 @@ ms_backward_kernel(const MsBwdArgs a) {
             for (int y = 0; y < H; ++y) for (int t = 0; t < 4; ++t) s.My[y * P + s.iy[y * 4 + t]] += s.wy[y * 4 + t];
             for (int x = 0; x < W; ++x) for (int t = 0; t < 4; ++t) s.Mx[x * P + s.ix[x * 4 + t]] += s.wx[x * 4 + t];
         }
-        ms_bicubic_up(fs, C, H, W, P, RP);
+        ms_bicubic_up(fs, C, H, W, P, HW);
         __syncthreads();
         const int kphi = d.K > 0 ? d.phi_map[k] : -1;
         if (kphi >= 0 && kphi != cur_phi) {   // stage this Phi's weights + bias in shared memory (4 times per image)
@@ -1228,6 +1233,9 @@ ms_backward_kernel(const MsBwdArgs a) {
                     for (int y = 0; y < H; ++y) acc = fmaf(s.My[y * P + pp], s.tmp[(size_t)c * H * P + y * P + q], acc);
                     atomicAdd(a.gE + (size_t)s.idx[rr] * C + c, acc);
                 }
+                __syncthreads();
+                // tmp lives in dh's storage: restore dh's zero border (its interior is rewritten by the next Phi pass)
+                for (int i = tid; i < C * H * P; i += blockDim.x) s.tmp[i] = 0.f;
             }
         }
         __syncthreads();
@@ -1464,9 +1472,9 @@ int xq_ms_forward(const xq_ms_desc *d, const float *f, const float *E, const flo
     const int C = d->C, H = d->H, W = d->W, HW = H * W;
     size_t smem = sizeof(float) * ms_fwd_smem_floats(C, H, W, d->SN, !bsq);
     if (smem > 227 * 1024) return XQ_ERR_UNSUPPORTED;
-    // a training forward is followed by xq_ms_backward, whose CTA holds more per image than the forward's: refuse the
-    // shape here rather than let loss.backward() fail after the forward has run
-    if (with_losses && saved && sizeof(float) * ms_bwd_smem_floats(C, H, W) > 227 * 1024) return XQ_ERR_UNSUPPORTED;
+    // a training forward is followed by xq_ms_backward, whose CTA may hold more per image than the forward's: refuse
+    // the shape here rather than let loss.backward() fail after the forward has run
+    if (with_losses && saved && ms_bwd_smem_bytes(C, H, W) > 227 * 1024) return XQ_ERR_UNSUPPORTED;
     MsSaved sv = {nullptr, nullptr, nullptr, nullptr, nullptr};
     if (saved) sv = ms_saved_layout(d, saved);
 
@@ -1538,7 +1546,7 @@ int xq_ms_backward(const xq_ms_desc *d, const float *f, const float *E, const fl
     cudaStream_t stream = (cudaStream_t)stream_;
     const int C = d->C, H = d->H, W = d->W;
     const size_t chw = (size_t)C * H * W;
-    size_t smem = sizeof(float) * ms_bwd_smem_floats(C, H, W);
+    const size_t smem = ms_bwd_smem_bytes(C, H, W);
     if (smem > 227 * 1024) return XQ_ERR_UNSUPPORTED;
     MsSaved sv = ms_saved_layout(d, const_cast<void *>(saved));
 
