@@ -45,14 +45,9 @@ _lib = None
 F16_TWINS = [
     "xq_vit_residual_ln_fwd", "xq_vit_residual_ln_bwd", "xq_vit_patchify", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd",
     "xq_vit_attn_fwd", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd",
-    "xq_vit_fc2_lora_dgelu_bwd",
+    "xq_vit_fc2_lora_dgelu_bwd", "xq_vit_swiglu_fwd", "xq_vit_swiglu_bwd", "xq_vit_rope_fwd", "xq_vit_rope_bwd",
+    "xq_vit_attn_fwd_cls",
 ]
-# the SwiGLU entry points of the giant backbones' MLP, with `_f16` twins in the same sense
-SWIGLU_ENTRIES = ["xq_vit_swiglu_fwd", "xq_vit_swiglu_bwd", "xq_vit_fc1_swiglu_fwd", "xq_vit_fc2_dswiglu_bwd"]
-# the RoPE decoder's q / k rotation (csrc/rope_kernel.cu), with `_f16` twins in the same sense
-ROPE_ENTRIES = ["xq_vit_rope_fwd", "xq_vit_rope_bwd"]
-# the class-token attention of a frozen teacher's last block (csrc/attn_kernel.cu), with an `_f16` twin in the same sense
-ATTN_CLS_ENTRIES = ["xq_vit_attn_fwd_cls"]
 
 
 def lib() -> ctypes.CDLL:
@@ -142,10 +137,6 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_swiglu_fwd.argtypes = [vp, f32p, vp, c_int, c_int, vp]
     L.xq_vit_swiglu_bwd.restype = c_int
     L.xq_vit_swiglu_bwd.argtypes = [vp, f32p, vp, vp, f32p, c_int, c_int, vp]
-    L.xq_vit_fc1_swiglu_fwd.restype = c_int
-    L.xq_vit_fc1_swiglu_fwd.argtypes = [vp, vp, f32p, vp, vp, c_int, c_int, c_int, vp]
-    L.xq_vit_fc2_dswiglu_bwd.restype = c_int
-    L.xq_vit_fc2_dswiglu_bwd.argtypes = [vp, vp, vp, f32p, vp, f32p, c_int, c_int, c_int, vp]
     L.xq_vit_rope_fwd.restype = c_int
     L.xq_vit_rope_fwd.argtypes = [vp, vp, f32p, f32p] + [c_int] * 7 + [vp]
     L.xq_vit_rope_bwd_workspace_bytes.restype = c_size_t
@@ -153,7 +144,7 @@ def lib() -> ctypes.CDLL:
     L.xq_vit_rope_bwd.restype = c_int
     L.xq_vit_rope_bwd.argtypes = [vp, vp, f32p, f32p] + [c_int] * 7 + [vp, f32p, f32p, f32p, vp, c_size_t, vp]
     # fp16 twins of the 16-bit ViT entry points: the same argument lists
-    for name in F16_TWINS + SWIGLU_ENTRIES + ROPE_ENTRIES + ATTN_CLS_ENTRIES:
+    for name in F16_TWINS:
         twin = getattr(L, name + "_f16")
         twin.restype = c_int
         twin.argtypes = getattr(L, name).argtypes
@@ -249,6 +240,19 @@ def workspace(nbytes: int, device) -> torch.Tensor:
     return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=device)
 
 
+_STREAM_WS = {}
+
+
+def stream_workspace(entry: str, nbytes: int, device) -> torch.Tensor:
+    """Workspace of entry point `entry` on the current stream of `device`: one grow-only buffer per (entry, device, stream),
+    reused across calls because calls on one stream are ordered."""
+    key = (entry, device.index, torch.cuda.current_stream(device).cuda_stream)
+    ws = _STREAM_WS.get(key)
+    if ws is None or ws.numel() < nbytes:
+        ws = _STREAM_WS[key] = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    return ws
+
+
 def make_ms_desc(B, C, H, W, V, K, patch_nums, phi_map, mode, scaler=None, resi_ratio=0.5, beta=0.25,
                  loss_div_sn_all=False, channel_norm=False, entropy_weight=0.0, w_sample=1.0, w_batch=1.0) -> XqMsDesc:
     SN = len(patch_nums)
@@ -270,11 +274,10 @@ EXPORTED_SYMBOLS = [
     "xq_strerror", "xq_abi_version", "xq_last_cuda_error", "xq_vq_workspace_bytes", "xq_vq_forward",
     "xq_vq_backward", "xq_perturb_workspace_bytes", "xq_perturb_forward", "xq_perturb_backward",
     "xq_ms_workspace_bytes", "xq_ms_saved_bytes", "xq_ms_total_tokens", "xq_ms_forward", "xq_ms_backward",
-    "xq_ms_decode", "xq_ms_embed", "xq_usage_ema_dev", "xq_vit_residual_ln_fwd", "xq_vit_ln_bwd_workspace_bytes",
-    "xq_vit_residual_ln_bwd", "xq_vit_gelu_fwd", "xq_vit_gelu_bwd", "xq_vit_patchify", "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_fwd", "xq_vit_attn_bwd_workspace_bytes", "xq_vit_attn_bwd", "xq_vit_fc1_gelu_fwd", "xq_vit_fc2_dgelu_bwd", "xq_vit_fc1_lora_gelu_fwd", "xq_vit_fc2_lora_dgelu_bwd",
+    "xq_ms_decode", "xq_ms_embed", "xq_usage_ema_dev", "xq_vit_ln_bwd_workspace_bytes",
+    "xq_vit_assemble_fwd", "xq_vit_assemble_bwd", "xq_vit_attn_bwd_workspace_bytes",
     "xq_lpips_workspace_bytes", "xq_lpips_layer_forward", "xq_lpips_layer_backward", "xq_diffaug_forward",
     "xq_diffaug_backward", "xq_img_workspace_bytes", "xq_img_box_halve", "xq_img_resize_crop_normalize",
     "xq_ema_update", "xq_adamw_step", "xq_grad_norm_workspace_bytes", "xq_grad_norm", "xq_grad_scale", "xq_recon_psnr_ssim_workspace_bytes", "xq_recon_psnr_ssim",
     "xq_vit_rope_bwd_workspace_bytes",
-] + [n + "_f16" for n in F16_TWINS] + SWIGLU_ENTRIES + [n + "_f16" for n in SWIGLU_ENTRIES] + ROPE_ENTRIES + [
-    n + "_f16" for n in ROPE_ENTRIES] + ATTN_CLS_ENTRIES + [n + "_f16" for n in ATTN_CLS_ENTRIES]
+] + F16_TWINS + [n + "_f16" for n in F16_TWINS]

@@ -13,15 +13,8 @@
 // are the same kernel with one more K stage: the producer loads the [128][64] tiles of u / v and of the K-major adapter
 // (B1 [N,R], A2^T [N,R]) after the main K loop, TMA zero-filling the columns >= R, and the MMA warps accumulate it into the
 // same fp32 accumulators before the single rounding to bf16.
-// The SwiGLU MLP of the giant backbones (timm GluMlp, gate_last=False: fc1 -> [gate | up] halves -> silu(gate) * up -> fc2,
-// vision_transformer.py:2925-2937) has the same two fused GEMMs, with the epilogue pairing each gate column j with its up
-// column H + j:
-//   xq_vit_fc1_swiglu_fwd   pre = y W1^T [M,2H] ; act = silu(pre[:, j] + b1[j]) * (pre[:, H+j] + b1[H+j])  [M,H]
-//   xq_vit_fc2_dswiglu_bwd  g = d_branch W2 [M,H] ; d_pre[:, j] = g c silu'(a), d_pre[:, H+j] = g silu(a) ; d_b1 = colsum(d_pre)
-// The forward's output tile is 64 gate columns [j0, j0+64) and the matching 64 up columns: the producer loads its B operand as
-// two 64-row boxes of W1, so the staging tile's two row tiles are the two halves of every pair.  The backward's output tile
-// is 128 columns of g; the producer stages the matching gate and up tiles of `pre` in the two auxiliary tiles (one tile's
-// worth, not double-buffered) and the epilogue overwrites them in place with the two halves of d_pre.
+// The giant backbones' SwiGLU MLP has no fused form: a library GEMM + the stand-alone xq_vit_swiglu_fwd / _bwd
+// (vit_kernels.cu) is faster at its shape (DESIGN.md).
 // Every entry point has an `_f16` twin: the same kernel instantiated for fp16 operands and outputs (fp16 autocast), wgmma
 // .f16 instead of .bf16, f16 tensor maps and conversions; shared memory, registers and schedule are the same.
 //
@@ -49,8 +42,6 @@ namespace xq {
 using namespace xqtc;
 using xqv::dgelu_f;
 using xqv::gelu_f;
-using xqv::dswiglu_f;
-using xqv::swiglu_f;
 
 constexpr int GM_BM = 128, GM_BN = 128, GM_BK = 64;
 constexpr int GM_THREADS = 13 * 32;                            // 2 MMA warpgroups + 1 epilogue warpgroup + 1 producer warp
@@ -100,7 +91,6 @@ struct GmClock {
 
 // EPI 1: forward  -- the staged tile is the pre-activation: TMA-stored as it stands (tmP, only when store_pre: the inference
 //                    form leaves `pre` unwritten and tmP unbuilt); GELU(pre + bias) -> tmO.
-// EPI 3 / 4: the SwiGLU forms of EPI 1 / 2 (N is 2H in the forward, H in the backward; the column mapping is above).
 // EPI 2: backward -- the staged tile is d_act; the producer loads the stored pre-activation tile (tmP);
 //                    d_act * GELU'(pre + bias) -> tmO; column sums of the ROUNDED result -> dbias (fp32 atomics at the end).
 // Both apply the element-wise function to the ROUNDED 16-bit value of the GEMM result, i.e. exactly what the stand-alone
@@ -140,7 +130,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (elect_one()) {
             tma_prefetch_desc(&tmA);
             tma_prefetch_desc(&tmB);
-            if (EPI == 2 || EPI == 4) tma_prefetch_desc(&tmP);
+            if (EPI == 2) tma_prefetch_desc(&tmP);
             if (R > 0) { tma_prefetch_desc(&tmU); tma_prefetch_desc(&tmL); }
         }
         __syncwarp();
@@ -156,164 +146,30 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                     mbar_expect_tx(&full[st], GM_ST_BYTES);
                     tma_load_3d(base + st * GM_ST_BYTES, tail ? &tmU : &tmA, tail ? 0 : kb * GM_BK, mb * GM_BM, 0,
                                 &full[st]);                                                        // rows >= M: zero-filled
-                    if (EPI == 3) {
-                        // gate rows [64 nb, 64 nb + 64) of W1 above the matching up rows, H = N / 2 further down
-                        uint8_t *bt = base + st * GM_ST_BYTES + GM_A_BYTES;
-                        tma_load_3d(bt, &tmB, kb * GM_BK, nb * 64, 0, &full[st]);
-                        tma_load_3d(bt + GM_BN * GM_BK, &tmB, kb * GM_BK, N / 2 + nb * 64, 0, &full[st]);
-                    } else {
-                        tma_load_3d(base + st * GM_ST_BYTES + GM_A_BYTES, tail ? &tmL : &tmB, tail ? 0 : kb * GM_BK, nb * GM_BN,
-                                    0, &full[st]);
-                    }
+                    tma_load_3d(base + st * GM_ST_BYTES + GM_A_BYTES, tail ? &tmL : &tmB, tail ? 0 : kb * GM_BK, nb * GM_BN, 0,
+                                &full[st]);
                 }
                 __syncwarp();
                 // backward: the stored pre-activation tile goes to the auxiliary tile as soon as the epilogue has released it
                 // (polled once per K step, so that the ring is not held up), at the latest with the tile's last K step;
                 // rows >= M are zero-filled
-                // (EPI 4: the gate tile to auxiliary tile 0, the up tile, H = N columns further, to tile 1; one pair in flight)
-                if ((EPI == 2 || EPI == 4) && !pre_sent) {
-                    const int ai = EPI == 2 ? (t & 1) : 0;
+                if (EPI == 2 && !pre_sent) {
+                    const int ai = t & 1;
                     uint64_t *e = &aux_empty[ai];
-                    const uint32_t par = EPI == 2 ? (((t >> 1) & 1) ^ 1) : ((t & 1) ^ 1);
+                    const uint32_t par = ((t >> 1) & 1) ^ 1;
                     if (kb == nks - 1) mbar_wait(e, par);
                     else if (!__any_sync(0xffffffffu, mbar_test(e, par))) continue;
                     uint8_t *aux = base + GM_AUX_OFF + ai * GM_TILE_BYTES;
                     if (elect_one()) {
-                        mbar_expect_tx(&aux_full[ai], EPI == 2 ? GM_TILE_BYTES : 2 * GM_TILE_BYTES);
+                        mbar_expect_tx(&aux_full[ai], GM_TILE_BYTES);
                         tma_load_3d(aux, &tmP, nb * GM_BN, mb * GM_BM, 0, &aux_full[ai]);
                         tma_load_3d(aux + GM_HALF_BYTES, &tmP, nb * GM_BN + 64, mb * GM_BM, 0, &aux_full[ai]);
-                        if (EPI == 4) {
-                            tma_load_3d(aux + GM_TILE_BYTES, &tmP, N + nb * GM_BN, mb * GM_BM, 0, &aux_full[ai]);
-                            tma_load_3d(aux + GM_TILE_BYTES + GM_HALF_BYTES, &tmP, N + nb * GM_BN + 64, mb * GM_BM, 0, &aux_full[ai]);
-                        }
                     }
                     __syncwarp();
                     pre_sent = true;
                 }
             }
         }
-        return;
-    }
-    if (warp >= 8 && EPI == 3) {
-        // ===== SwiGLU forward epilogue: thread te owns 16-byte unit uc of both row tiles (gate and up) in rows rg, rg + 16,
-        // ..., rg + 112, and writes that unit of the [128][64] act tile =====
-        const int te = tid - 8 * 32, uc = te & 7, rg = te >> 3;
-        const int H = N / 2, j0 = nb * 64;
-        float ba[8], bc[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { ba[e] = bias[j0 + 8 * uc + e]; bc[e] = bias[H + j0 + 8 * uc + e]; }
-        int t = 0;
-        for (int mb = mb0; mb < nM; mb += mstep, ++t) {
-            uint8_t *aux = base + GM_AUX_OFF + (t & 1) * GM_TILE_BYTES;
-            mbar_wait(stg_full, t & 1);
-            if (te == 0 && store_pre) {
-                tma_store_3d(&tmP, stg, j0, mb * GM_BM, 0);
-                tma_store_3d(&tmP, stg + GM_HALF_BYTES, H + j0, mb * GM_BM, 0);
-                bulk_commit();
-            }
-            constexpr int UB = 4;
-#pragma unroll
-            for (int ib = 0; ib < 8 / UB; ++ib) {
-                uint32_t off[UB];
-                uint4 qa[UB], qc[UB];
-#pragma unroll
-                for (int u = 0; u < UB; ++u) {
-                    off[u] = rowtile_unit(rg + 16 * (UB * ib + u), uc);
-                    qa[u] = lds128(smem_u32(stg) + off[u]);
-                    qc[u] = lds128(smem_u32(stg) + GM_HALF_BYTES + off[u]);
-                }
-#pragma unroll
-                for (int u = 0; u < UB; ++u) {
-                    const uint32_t a[4] = {qa[u].x, qa[u].y, qa[u].z, qa[u].w}, c[4] = {qc[u].x, qc[u].y, qc[u].z, qc[u].w};
-                    uint32_t o[4];
-#pragma unroll
-                    for (int w = 0; w < 4; ++w)
-                        o[w] = E::pack(swiglu_f(E::lo(a[w]) + ba[2 * w], E::lo(c[w]) + bc[2 * w]),
-                                       swiglu_f(E::hi(a[w]) + ba[2 * w + 1], E::hi(c[w]) + bc[2 * w + 1]));
-                    sts128(smem_u32(aux) + off[u], make_uint4(o[0], o[1], o[2], o[3]));
-                }
-            }
-            fence_async_smem();
-            asm volatile("bar.sync 1, 128;" ::: "memory");       // the act tile is complete, the staging tile read
-            if (te == 0) {
-                tma_store_3d(&tmO, aux, j0, mb * GM_BM, 0);
-                bulk_commit();
-                bulk_wait_read<1>();                             // this tile's `pre` stores (if any) and the previous `act` store
-                mbar_arrive(stg_empty);
-            }
-        }
-        if (te == 0) bulk_wait<0>();
-        return;
-    }
-    if (warp >= 8 && EPI == 4) {
-        // ===== SwiGLU backward epilogue: thread te owns 16-byte unit uc of the g tile in rows rg, rg + 8, ..., rg + 120 and
-        // the same unit of the gate (auxiliary tile 0) and up (auxiliary tile 1) pre-activation tiles =====
-        const int te = tid - 8 * 32, uc = te & 15, rg = te >> 4;
-        const uint32_t ubase = (uint32_t)((uc >> 3) * GM_HALF_BYTES);
-        const int H = N, j = nb * GM_BN + 8 * uc;
-        float ba[8], bc[8], sa[8], sc[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { ba[e] = bias[j + e]; bc[e] = bias[H + j + e]; sa[e] = sc[e] = 0.f; }
-        uint8_t *xa = base + GM_AUX_OFF, *xc = xa + GM_TILE_BYTES;
-        int t = 0;
-        for (int mb = mb0; mb < nM; mb += mstep, ++t) {
-            mbar_wait(stg_full, t & 1);
-            mbar_wait(&aux_full[0], t & 1);
-            // the tile's 16 rows summed here, then added to the running sums: a term passes through at most 16 + tiles adds
-            float ta[8], tc[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) ta[e] = tc[e] = 0.f;
-            constexpr int UB = 2;
-#pragma unroll
-            for (int ib = 0; ib < 16 / UB; ++ib) {
-                uint32_t off[UB];
-                uint4 qg[UB], qa[UB], qc[UB];
-#pragma unroll
-                for (int u = 0; u < UB; ++u) {
-                    off[u] = ubase + rowtile_unit(rg + 8 * (UB * ib + u), uc & 7);
-                    qg[u] = lds128(smem_u32(stg) + off[u]);
-                    qa[u] = lds128(smem_u32(xa) + off[u]);
-                    qc[u] = lds128(smem_u32(xc) + off[u]);
-                }
-#pragma unroll
-                for (int u = 0; u < UB; ++u) {
-                    // g rounded to 16 bits first: the stand-alone kernel reads the tensor a library GEMM wrote.  Rows >= M:
-                    // the zero-filled A rows give g = 0, so they add nothing to the bias gradient.
-                    const uint32_t g[4] = {qg[u].x, qg[u].y, qg[u].z, qg[u].w};
-                    const uint32_t a[4] = {qa[u].x, qa[u].y, qa[u].z, qa[u].w}, c[4] = {qc[u].x, qc[u].y, qc[u].z, qc[u].w};
-                    uint32_t oa[4], oc[4];
-#pragma unroll
-                    for (int w = 0; w < 4; ++w) {
-                        float da0, dc0, da1, dc1;
-                        dswiglu_f(E::lo(g[w]), E::lo(a[w]) + ba[2 * w], E::lo(c[w]) + bc[2 * w], da0, dc0);
-                        dswiglu_f(E::hi(g[w]), E::hi(a[w]) + ba[2 * w + 1], E::hi(c[w]) + bc[2 * w + 1], da1, dc1);
-                        oa[w] = E::pack(da0, da1);
-                        oc[w] = E::pack(dc0, dc1);
-                        ta[2 * w] += E::lo(oa[w]); ta[2 * w + 1] += E::hi(oa[w]);
-                        tc[2 * w] += E::lo(oc[w]); tc[2 * w + 1] += E::hi(oc[w]);
-                    }
-                    sts128(smem_u32(xa) + off[u], make_uint4(oa[0], oa[1], oa[2], oa[3]));
-                    sts128(smem_u32(xc) + off[u], make_uint4(oc[0], oc[1], oc[2], oc[3]));
-                }
-            }
-#pragma unroll
-            for (int e = 0; e < 8; ++e) { sa[e] += ta[e]; sc[e] += tc[e]; }
-            fence_async_smem();
-            asm volatile("bar.sync 1, 128;" ::: "memory");       // d_pre is complete in both tiles, the staging tile read
-            if (te == 0) {
-                tma_store_3d(&tmO, xa, nb * GM_BN, mb * GM_BM, 0);
-                tma_store_3d(&tmO, xa + GM_HALF_BYTES, nb * GM_BN + 64, mb * GM_BM, 0);
-                tma_store_3d(&tmO, xc, H + nb * GM_BN, mb * GM_BM, 0);
-                tma_store_3d(&tmO, xc + GM_HALF_BYTES, H + nb * GM_BN + 64, mb * GM_BM, 0);
-                bulk_commit();
-                mbar_arrive(stg_empty);
-                bulk_wait_read<0>();                             // the stores have read both tiles: the producer may refill
-                mbar_arrive(&aux_empty[0]);
-            }
-        }
-        if (te == 0) bulk_wait<0>();
-#pragma unroll
-        for (int e = 0; e < 8; ++e) { atomicAdd(dbias + j + e, sa[e]); atomicAdd(dbias + H + j + e, sc[e]); }
         return;
     }
     if (warp >= 8) {
@@ -475,7 +331,7 @@ mlp_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (lane == 0) mbar_arrive(stg_full);
         if (tid == 0) { clk.lap(GM_CLK_HANDOFF); clk.count(GM_CLK_TILES); }
     }
-    if (tid == 0 && EPI <= 2) clk.flush(EPI);               // the counters cover the GELU forms only
+    if (tid == 0) clk.flush(EPI);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------
@@ -503,16 +359,13 @@ static int gm_launch(const void *a, const void *b, const void *u, const void *l,
     if (int rc = sm_count(&sms)) return rc;
     const int nN = N / GM_BN;
     if (nN > sms) return XQ_ERR_UNSUPPORTED;
-    // SwiGLU: the forward (N = 2H) loads W1 in 64-row boxes and writes act [M, H]; the backward (N = H) reads and writes
-    // the [M, 2H] pre / d_pre and sums 2H bias-gradient columns
-    const uint64_t pre_cols = EPI == 4 ? 2 * (uint64_t)N : N, out_cols = EPI == 3 ? N / 2 : pre_cols;
     CUtensorMap tmA, tmB, tmP, tmO;
     if (!tensor_map_16_3d(&tmA, E::TMAP, a, K, M, 1, (uint64_t)K * 2, (uint64_t)M * K * 2, GM_BM) ||
-        !tensor_map_16_3d(&tmB, E::TMAP, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, EPI == 3 ? 64 : GM_BN) ||
-        !tensor_map_16_3d(&tmO, E::TMAP, out, out_cols, M, 1, out_cols * 2, (uint64_t)M * out_cols * 2, GM_BM))
+        !tensor_map_16_3d(&tmB, E::TMAP, b, K, N, 1, (uint64_t)K * 2, (uint64_t)N * K * 2, GM_BN) ||
+        !tensor_map_16_3d(&tmO, E::TMAP, out, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM))
         return XQ_ERR_UNSUPPORTED;
     tmP = tmO;
-    if (pre && !tensor_map_16_3d(&tmP, E::TMAP, pre, pre_cols, M, 1, pre_cols * 2, (uint64_t)M * pre_cols * 2, GM_BM))
+    if (pre && !tensor_map_16_3d(&tmP, E::TMAP, pre, N, M, 1, (uint64_t)N * 2, (uint64_t)M * N * 2, GM_BM))
         return XQ_ERR_UNSUPPORTED;
     CUtensorMap tmU = tmA, tmL = tmB;
     if (R > 0 && (!tensor_map_16_3d(&tmU, E::TMAP, u, R, M, 1, (uint64_t)R * 2, (uint64_t)M * R * 2, GM_BM) ||
@@ -523,7 +376,7 @@ static int gm_launch(const void *a, const void *b, const void *u, const void *l,
     int per_col = sms / nN;                               // CTAs per column block
     if (per_col > nM) per_col = nM;
     // the bias gradient is accumulated with atomics; zeroed here, after every check, so a refused call writes nothing
-    if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N * (EPI == 4 ? 2 : 1), st));
+    if (dbias) XQ_CUDA_TRY(cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)N, st));
     mlp_gemm_kernel<E, EPI><<<per_col * nN, GM_THREADS, GM_SMEM, st>>>(tmA, tmB, tmP, tmO, tmU, tmL, bias, dbias, M, N, K, R,
                                                                         pre != nullptr);
     XQ_LAUNCH_CHECK("mlp_gemm_kernel");
@@ -565,24 +418,6 @@ static int fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v,
     return gm_launch<E, 2>(d_out, w2t, v, a2t, pre, d_pre, bias, d_bias, M, N, K, R, (cudaStream_t)stream);
 }
 
-// SwiGLU: w [2H,K] = fc1.weight, pre / d_pre [M,2H], act / g [M,H], bias / d_bias [2H]; H % 64 == 0 for the forward (its
-// N = 2H is a multiple of 128), H % 128 == 0 for the backward
-template <typename E>
-static int fc1_swiglu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K, void *stream) {
-    if (H <= 0 || H > (1 << 29)) return XQ_ERR_ARG;
-    if (int rc = gm_check(x, w, act, pre ? pre : act, bias, M, 2 * H, K)) return rc;
-    return gm_launch<E, 3>(x, w, nullptr, nullptr, pre, act, bias, nullptr, M, 2 * H, K, 0, (cudaStream_t)stream);
-}
-
-template <typename E>
-static int fc2_dswiglu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias, int M,
-                           int H, int K, void *stream) {
-    if (H <= 0 || H > (1 << 29)) return XQ_ERR_ARG;
-    if (int rc = gm_check(d_out, w2t, d_pre, pre, bias, M, H, K)) return rc;
-    if (!d_bias) return XQ_ERR_ARG;
-    return gm_launch<E, 4>(d_out, w2t, nullptr, nullptr, pre, d_pre, bias, d_bias, M, H, K, 0, (cudaStream_t)stream);
-}
-
 }  // namespace xq
 
 extern "C" {
@@ -619,23 +454,6 @@ int xq_vit_fc2_lora_dgelu_bwd(const void *d_out, const void *w2t, const void *v,
 int xq_vit_fc2_lora_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre,
                                   const float *bias, void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream) {
     return xq::fc2_lora_dgelu_bwd<xqtc::F16>(d_out, w2t, v, a2t, pre, bias, d_pre, d_bias, M, N, K, R, stream);
-}
-
-int xq_vit_fc1_swiglu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K, void *stream) {
-    return xq::fc1_swiglu_fwd<xqtc::Bf16>(x, w, bias, pre, act, M, H, K, stream);
-}
-int xq_vit_fc1_swiglu_fwd_f16(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K,
-                              void *stream) {
-    return xq::fc1_swiglu_fwd<xqtc::F16>(x, w, bias, pre, act, M, H, K, stream);
-}
-
-int xq_vit_fc2_dswiglu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias, int M,
-                           int H, int K, void *stream) {
-    return xq::fc2_dswiglu_bwd<xqtc::Bf16>(d_out, w2t, pre, bias, d_pre, d_bias, M, H, K, stream);
-}
-int xq_vit_fc2_dswiglu_bwd_f16(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
-                               int M, int H, int K, void *stream) {
-    return xq::fc2_dswiglu_bwd<xqtc::F16>(d_out, w2t, pre, bias, d_pre, d_bias, M, H, K, stream);
 }
 
 #ifdef XQ_GM_CLOCKS

@@ -1,6 +1,6 @@
 // xq_gelu.cuh -- the exact-erf GELU, SiLU / SwiGLU and their derivatives as ONE set of device functions, shared by the
-// stand-alone element-wise kernels (vit_kernels.cu) and the fused GEMM epilogues (gemm_kernel.cu), so that both paths produce
-// the same bits.
+// stand-alone element-wise kernels (vit_kernels.cu) and the fused GELU GEMM epilogues (gemm_kernel.cu), so that both paths
+// produce the same bits.
 // Reference ops: nn.GELU() (erf form) inside timm's Mlp, tokenizer/tokenizer_image/dino_enc/vision_transformer.py:336-339, and
 // nn.SiLU inside timm's SwiGLUPacked (GluMlp, gate_last=False) of the giant backbones, vision_transformer.py:2925-2937.
 #pragma once

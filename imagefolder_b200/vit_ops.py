@@ -20,7 +20,6 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _capi as C
-from ._capi import call as _call, lib as _lib, ptr as _ptr, stream_ptr as _stream
 
 _SUPPORTED_D = (384, 768, 1024, 1536)
 _HALF = (torch.bfloat16, torch.float16)       # the GEMM operand dtypes the kernels are instantiated for
@@ -278,75 +277,6 @@ def swiglu_bias(x, bias=None):
     return _SwiGLUBias.apply(x, bias)
 
 
-# The wgmma GEMMs with fused SwiGLU / SwiGLU' epilogues (csrc/gemm_kernel.cu, EPI 3 / 4).  Off by default: at the giant
-# training shape they are slower than the library GEMM + stand-alone kernel (tools/bench_swiglu_mlp.py, DESIGN.md section 0).
-SWIGLU_TC_ENABLED = [False]
-
-
-def swiglu_tc_ok(y, fc1, fc2) -> bool:
-    """xq_vit_fc1_swiglu_fwd / xq_vit_fc2_dswiglu_bwd (and their _f16 twins) cover: bf16 or fp16 CUDA tokens, an fc1 bias,
-    H = fc1 width / 2 with H % 128 == 0 (the backward's 128-column tiles; the forward needs H % 64), embed % 64 == 0, out % 64
-    == 0 (the K of the backward GEMM) and H / 64 <= SM count (the forward's column blocks; the backward has half as many).
-    Mirrors every refusal of the C wrappers, so neither call fails inside forward or backward."""
-    N1, K = fc1.weight.shape
-    return (SWIGLU_TC_ENABLED[0] and y.is_cuda and y.dtype in _HALF and fc1.bias is not None
-            and N1 % 256 == 0 and K % 64 == 0 and fc2.weight.shape[1] == N1 // 2 and fc2.weight.shape[0] % 64 == 0
-            and (N1 // 2) // 64 <= _sm_count(y.device))
-
-
-class _FusedSwiGLU(torch.autograd.Function):
-    """branch = fc2(silu(a) * c), [a | c] = fc1(y), WITHOUT the fc2 bias (folded into the next residual_ln): timm GluMlp as
-    called from Block.forward.  The fc1 GEMM carries bias + SwiGLU in its epilogue, the fc2 input-gradient GEMM carries the
-    SwiGLU derivative and the fc1-bias gradient; the other GEMMs are library calls.  Same bits as F.linear + swiglu_bias.
-    No `pre` and nothing saved when no input needs a gradient (_keeps_pre)."""
-
-    @staticmethod
-    def forward(ctx, y, W1, b1, W2):
-        N1, K = W1.shape
-        H = N1 // 2
-        y2 = y.reshape(-1, K)
-        if not y2.is_contiguous():
-            y2 = y2.contiguous()
-        M = y2.shape[0]
-        dt = y.dtype
-        W1b, W2b, b1f = W1.to(dt), W2.to(dt), b1.float()
-        keep = _keeps_pre(ctx)
-        pre = torch.empty(M, N1, dtype=dt, device=y.device) if keep else None
-        act = torch.empty(M, H, dtype=dt, device=y.device)
-        name, fn = _entry("xq_vit_fc1_swiglu_fwd", dt)
-        C.call(name, 1, fn, C.ptr(y2), C.ptr(W1b), C.ptr(b1f), C.ptr(pre), C.ptr(act), M, H, K,
-               C.stream_ptr(y.device), nbytes=M * K * 2 + N1 * K * 2 + (M * N1 * 2 if keep else 0) + M * H * 2,
-               nflops=2.0 * M * N1 * K)
-        branch = act @ W2b.t()
-        if keep:
-            ctx.save_for_backward(y2, pre, act, W1b, W2b, b1f)
-        ctx.out_shape = y.shape[:-1] + (W2.shape[0],)
-        ctx.in_shape = y.shape
-        return branch.view(ctx.out_shape)
-
-    @staticmethod
-    def backward(ctx, g):
-        y2, pre, act, W1b, W2b, b1f = ctx.saved_tensors
-        M, N1 = pre.shape
-        H = N1 // 2
-        Ko = W2b.shape[0]
-        g2 = g.reshape(M, Ko)
-        if g2.dtype != pre.dtype:
-            g2 = g2.to(pre.dtype)
-        if not g2.is_contiguous():
-            g2 = g2.contiguous()
-        dW2 = (g2.t() @ act).float() if ctx.needs_input_grad[3] else None
-        W2t = W2b.t().contiguous()                      # [H, out]: the K-major B operand of g_act = g W2
-        dpre = torch.empty_like(pre)
-        db1 = torch.empty(N1, dtype=torch.float32, device=pre.device)
-        name, fn = _entry("xq_vit_fc2_dswiglu_bwd", pre.dtype)
-        C.call(name, 1, fn, C.ptr(g2), C.ptr(W2t), C.ptr(pre), C.ptr(b1f), C.ptr(dpre), C.ptr(db1),
-               M, H, Ko, C.stream_ptr(pre.device), nbytes=M * Ko * 2 + H * Ko * 2 + M * N1 * 4, nflops=2.0 * M * H * Ko)
-        dW1 = (dpre.t() @ y2).float() if ctx.needs_input_grad[1] else None
-        dy = (dpre @ W1b).view(ctx.in_shape) if ctx.needs_input_grad[0] else None
-        return dy, dW1, (db1 if ctx.needs_input_grad[2] else None), dW2
-
-
 def _scaled_mm(a, b, s: float):
     """16-bit(s * (a @ b)) in a's dtype: the scale applied to the fp32 accumulator, one rounding"""
     return torch.addmm(a.new_zeros(()), a, b, beta=0, alpha=s)
@@ -447,17 +377,15 @@ def _linear_no_bias(fc, x):
 
 
 def mlp_forward(mlp, y):
-    """timm Mlp (fc1 -> GELU -> fc2, drop = 0) or GluMlp (fc1 -> SwiGLU -> fc2) without the fc2 bias; fused wgmma path when the
-    shapes allow, else library GEMMs + the stand-alone bias / GELU (SwiGLU) kernel.  LoRA-wrapped fc1 and fc2 with inactive lora_dropout and r <= 64 take the LoRA form of
-    the fused path; any other LoRA Linear adds its `lora_delta` to a library GEMM."""
+    """timm Mlp (fc1 -> GELU -> fc2, drop = 0) or GluMlp (fc1 -> SwiGLU -> fc2) without the fc2 bias.  Mlp: fused wgmma path
+    when the shapes allow, else library GEMMs + the stand-alone bias / GELU kernel; LoRA-wrapped fc1 and fc2 with inactive
+    lora_dropout and r <= 64 take the LoRA form of the fused path.  GluMlp: library GEMMs + the stand-alone SwiGLU kernel.  Any
+    LoRA Linear off the fused path adds its `lora_delta` to a library GEMM."""
     fc1, fc2 = mlp.fc1, mlp.fc2
     lora = _lora()
     from .dino_enc.vision_transformer import GluMlp      # imported here: dino_enc imports this module
     if isinstance(mlp, GluMlp):
-        # timm GluMlp (the giant backbones): fused SwiGLU GEMMs for plain Linears, else library GEMMs + the stand-alone
-        # SwiGLU kernel (LoRA-wrapped fc1 / fc2 included: there is no fused LoRA form of the SwiGLU GEMMs)
-        if not (isinstance(fc1, lora.Linear) or isinstance(fc2, lora.Linear)) and swiglu_tc_ok(y, fc1, fc2):
-            return _FusedSwiGLU.apply(y, fc1.weight, fc1.bias, fc2.weight)
+        # timm GluMlp (the giant backbones), plain or LoRA-wrapped fc1 / fc2: library GEMMs + the stand-alone SwiGLU kernel
         return _linear_no_bias(fc2, swiglu_bias(_linear_no_bias(fc1, y), fc1.bias))
     if isinstance(fc1, lora.Linear) or isinstance(fc2, lora.Linear):
         if (isinstance(fc1, lora.Linear) and isinstance(fc2, lora.Linear) and _lora_off(fc1) and _lora_off(fc2)
@@ -493,9 +421,9 @@ def attn_tc_forward(qkv, num_heads: int):
     out = torch.empty(B, N, C3 // 3, dtype=qkv.dtype, device=qkv.device)
     lse2 = torch.empty(B, num_heads, N, dtype=torch.float32, device=qkv.device)
     name, fn = _entry("xq_vit_attn_fwd", qkv.dtype)
-    _call(name, 1, fn, _ptr(qkv), _ptr(out), _ptr(lse2), B, N, num_heads, 64, 0.125,
-          _stream(qkv.device), nbytes=qkv.numel() * 2 + out.numel() * 2 + lse2.numel() * 4,
-          nflops=4.0 * B * num_heads * N * N * 64)
+    C.call(name, 1, fn, C.ptr(qkv), C.ptr(out), C.ptr(lse2), B, N, num_heads, 64, 0.125,
+           C.stream_ptr(qkv.device), nbytes=qkv.numel() * 2 + out.numel() * 2 + lse2.numel() * 4,
+           nflops=4.0 * B * num_heads * N * N * 64)
     return out, lse2
 
 
@@ -506,12 +434,9 @@ def attn_cls_forward(qkv, num_heads: int):
     qkv = qkv.contiguous()
     out = torch.empty(B, C3 // 3, dtype=qkv.dtype, device=qkv.device)
     name, fn = _entry("xq_vit_attn_fwd_cls", qkv.dtype)
-    _call(name, 1, fn, _ptr(qkv), _ptr(out), B, N, num_heads, 64, 0.125, _stream(qkv.device),
-          nbytes=B * N * (C3 // 3) * 4 + out.numel() * 2)
+    C.call(name, 1, fn, C.ptr(qkv), C.ptr(out), B, N, num_heads, 64, 0.125, C.stream_ptr(qkv.device),
+           nbytes=B * N * (C3 // 3) * 4 + out.numel() * 2)
     return out
-
-
-_ATTN_WS = {}
 
 
 def attn_tc_backward(qkv, out, lse2, g, num_heads: int, want_bias_grad: bool = False):
@@ -523,18 +448,22 @@ def attn_tc_backward(qkv, out, lse2, g, num_heads: int, want_bias_grad: bool = F
         g = g.to(qkv.dtype)
     dqkv = torch.empty_like(qkv)
     db = torch.empty(C3, dtype=torch.float32, device=qkv.device) if want_bias_grad else None
-    L = _lib()
-    nbytes = int(L.xq_vit_attn_bwd_workspace_bytes(B, N, num_heads))
-    key = (qkv.device.index, torch.cuda.current_stream(qkv.device).cuda_stream)
-    ws = _ATTN_WS.get(key)                      # one workspace per (device, stream): calls on a stream are ordered
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=qkv.device)
-        _ATTN_WS[key] = ws
+    nbytes = int(C.lib().xq_vit_attn_bwd_workspace_bytes(B, N, num_heads))
+    ws = C.stream_workspace("xq_vit_attn_bwd", nbytes, qkv.device)
     name, fn = _entry("xq_vit_attn_bwd", qkv.dtype)
-    _call(name, 3, fn, _ptr(qkv), _ptr(out), _ptr(g), _ptr(lse2), _ptr(dqkv), _ptr(db), B, N, num_heads,
-          64, 0.125, _ptr(ws), ws.numel(), _stream(qkv.device), nbytes=qkv.numel() * 4 + out.numel() * 4 + lse2.numel() * 4,
-          nflops=10.0 * B * num_heads * N * N * 64)
+    C.call(name, 3, fn, C.ptr(qkv), C.ptr(out), C.ptr(g), C.ptr(lse2), C.ptr(dqkv), C.ptr(db), B, N, num_heads,
+           64, 0.125, C.ptr(ws), ws.numel(), C.stream_ptr(qkv.device),
+           nbytes=qkv.numel() * 4 + out.numel() * 4 + lse2.numel() * 4, nflops=10.0 * B * num_heads * N * N * 64)
     return (dqkv, db) if want_bias_grad else dqkv
+
+
+def _qkv_projection(y, W, b):
+    """(W in y's dtype, qkv = y W^T (+ b) [B,N,3D]) for y [B,N,D]: the packed qkv projection as one library GEMM in y's dtype
+    (autocast semantics)"""
+    B, N, D = y.shape
+    Wb = W.to(y.dtype)
+    y2 = y.reshape(B * N, D)
+    return Wb, (torch.addmm(b.to(y.dtype), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * D)
 
 
 class _QKVAttention(torch.autograd.Function):
@@ -545,10 +474,7 @@ class _QKVAttention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, y, W, b, num_heads: int):
-        B, N, C = y.shape
-        Wb = W.to(y.dtype)
-        y2 = y.reshape(B * N, C)
-        qkv = (torch.addmm(b.to(y.dtype), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * C)
+        Wb, qkv = _qkv_projection(y, W, b)
         out, lse2 = attn_tc_forward(qkv, num_heads)
         ctx.save_for_backward(y, Wb, qkv, out, lse2)
         ctx.heads = num_heads
@@ -569,7 +495,6 @@ class _QKVAttention(torch.autograd.Function):
 
 
 _ROPE_IMG = 256                # image tokens xq_vit_rope_fwd / _bwd cover (a 16 x 16 grid)
-_ROPE_WS = {}
 
 
 def rope_forward(qkv, freqs, freqs_1d_real, num_heads: int, P: int):
@@ -578,8 +503,8 @@ def rope_forward(qkv, freqs, freqs_1d_real, num_heads: int, P: int):
     B, N, _ = qkv.shape
     out = torch.empty_like(qkv)
     name, fn = _entry("xq_vit_rope_fwd", qkv.dtype)
-    _call(name, 1, fn, _ptr(qkv), _ptr(out), _ptr(freqs), _ptr(freqs_1d_real), B, N, num_heads, 64, P, _ROPE_IMG,
-          freqs_1d_real.shape[0], _stream(qkv.device), nbytes=qkv.numel() * 4)
+    C.call(name, 1, fn, C.ptr(qkv), C.ptr(out), C.ptr(freqs), C.ptr(freqs_1d_real), B, N, num_heads, 64, P, _ROPE_IMG,
+           freqs_1d_real.shape[0], C.stream_ptr(qkv.device), nbytes=qkv.numel() * 4)
     return out
 
 
@@ -593,16 +518,12 @@ def rope_backward(qkv, g, freqs, freqs_1d_real, num_heads: int, P: int):
     db = torch.empty(C3, dtype=torch.float32, device=qkv.device)
     dfreqs = torch.empty_like(freqs)
     d1 = torch.empty_like(freqs_1d_real)
-    nbytes = int(_lib().xq_vit_rope_bwd_workspace_bytes(B, N, num_heads, L))
-    key = (qkv.device.index, torch.cuda.current_stream(qkv.device).cuda_stream)
-    ws = _ROPE_WS.get(key)                      # one workspace per (device, stream): calls on a stream are ordered
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=qkv.device)
-        _ROPE_WS[key] = ws
+    nbytes = int(C.lib().xq_vit_rope_bwd_workspace_bytes(B, N, num_heads, L))
+    ws = C.stream_workspace("xq_vit_rope_bwd", nbytes, qkv.device)
     name, fn = _entry("xq_vit_rope_bwd", qkv.dtype)
-    _call(name, 2, fn, _ptr(qkv), _ptr(g), _ptr(freqs), _ptr(freqs_1d_real), B, N, num_heads, 64, P, _ROPE_IMG, L,
-          _ptr(dqkv), _ptr(db), _ptr(dfreqs), _ptr(d1), _ptr(ws), ws.numel(), _stream(qkv.device),
-          nbytes=qkv.numel() * 6 + ws.numel() * 2)
+    C.call(name, 2, fn, C.ptr(qkv), C.ptr(g), C.ptr(freqs), C.ptr(freqs_1d_real), B, N, num_heads, 64, P, _ROPE_IMG, L,
+           C.ptr(dqkv), C.ptr(db), C.ptr(dfreqs), C.ptr(d1), C.ptr(ws), ws.numel(), C.stream_ptr(qkv.device),
+           nbytes=qkv.numel() * 6 + ws.numel() * 2)
     return dqkv, db, dfreqs, d1
 
 
@@ -615,10 +536,7 @@ class _RoPEQKVAttention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, y, W, b, freqs, freqs_1d_real, num_heads: int, P: int):
-        B, N, C = y.shape
-        Wb = W.to(y.dtype)
-        y2 = y.reshape(B * N, C)
-        qkv = (torch.addmm(b.to(y.dtype), y2, Wb.t()) if b is not None else y2 @ Wb.t()).view(B, N, 3 * C)
+        Wb, qkv = _qkv_projection(y, W, b)
         freqs, freqs_1d_real = freqs.contiguous(), freqs_1d_real.contiguous()
         rot = rope_forward(qkv, freqs, freqs_1d_real, num_heads, P)
         out, lse2 = attn_tc_forward(rot, num_heads)
@@ -680,8 +598,8 @@ class _PatchEmbed(torch.autograd.Function):
         dt = _op_dtype()
         patches = torch.empty(M, K, dtype=dt, device=x.device)
         name, fn = _entry("xq_vit_patchify", dt)
-        _call(name, 1, fn, _ptr(x), _ptr(patches), Bn, Cin, H, Wd, p, _stream(x.device),
-              nbytes=x.numel() * 6)
+        C.call(name, 1, fn, C.ptr(x), C.ptr(patches), Bn, Cin, H, Wd, p, C.stream_ptr(x.device),
+               nbytes=x.numel() * 6)
         Wb = W.reshape(D, K).to(dt)
         if b is not None:
             y = torch.addmm(b.to(dt), patches, Wb.t())
@@ -737,9 +655,9 @@ class _Assemble(torch.autograd.Function):
         B, Ls, D = src.shape
         T = table.shape[-2]
         out = torch.empty(B, T, D, dtype=torch.float32, device=src.device)
-        L = _lib()
-        _call("xq_vit_assemble_fwd", 1, L.xq_vit_assemble_fwd, _ptr(src), _ASSEMBLE_TYPE[src.dtype], _ptr(table), B, Ls, T,
-              D, int(t0), _ptr(out), _stream(src.device), nbytes=out.numel() * 4 + src.numel() * src.element_size())
+        L = C.lib()
+        C.call("xq_vit_assemble_fwd", 1, L.xq_vit_assemble_fwd, C.ptr(src), _ASSEMBLE_TYPE[src.dtype], C.ptr(table), B, Ls, T,
+               D, int(t0), C.ptr(out), C.stream_ptr(src.device), nbytes=out.numel() * 4 + src.numel() * src.element_size())
         ctx.cfg = (B, Ls, T, D, int(t0), src.dtype, tuple(table.shape))
         return out
 
@@ -751,10 +669,10 @@ class _Assemble(torch.autograd.Function):
             g = g.float()
         d_src = torch.empty(B, Ls, D, dtype=sdt, device=g.device) if ctx.needs_input_grad[0] else None
         d_tab = torch.empty(tshape, dtype=torch.float32, device=g.device) if ctx.needs_input_grad[1] else None
-        L = _lib()
-        _call("xq_vit_assemble_bwd", 1, L.xq_vit_assemble_bwd, _ptr(g), B, Ls, T, D, t0, _ptr(d_src) if d_src is not None else None,
-              _ASSEMBLE_TYPE[sdt], _ptr(d_tab) if d_tab is not None else None, _stream(g.device),
-              nbytes=g.numel() * 4 + (d_src.numel() * d_src.element_size() if d_src is not None else 0))
+        L = C.lib()
+        C.call("xq_vit_assemble_bwd", 1, L.xq_vit_assemble_bwd, C.ptr(g), B, Ls, T, D, t0, C.ptr(d_src),
+               _ASSEMBLE_TYPE[sdt], C.ptr(d_tab), C.stream_ptr(g.device),
+               nbytes=g.numel() * 4 + (d_src.numel() * d_src.element_size() if d_src is not None else 0))
         return d_src, d_tab, None
 
 
@@ -898,10 +816,9 @@ def frozen_forward(vit, x, cls_only: bool = False):
             _, y = residual_ln(x, *pending, norm.weight, norm.bias, norm.eps)
             return y[:, 0]
         attn = blk.attn
-        Bn, S, D = y.shape
-        Wb, y2 = attn.qkv.weight.to(y.dtype), y.reshape(Bn * S, D)
-        qkv = (torch.addmm(attn.qkv.bias.to(y.dtype), y2, Wb.t()) if attn.qkv.bias is not None else y2 @ Wb.t())
-        a = F.linear(attn_cls_forward(qkv.view(Bn, S, 3 * D), attn.num_heads), attn.proj.weight).view(Bn, 1, D)
+        Bn, _, D = y.shape
+        _, qkv = _qkv_projection(y, attn.qkv.weight, attn.qkv.bias)
+        a = F.linear(attn_cls_forward(qkv, attn.num_heads), attn.proj.weight).view(Bn, 1, D)
         g1 = blk.ls1.gamma if hasattr(blk.ls1, "gamma") else None
         x, y = residual_ln(x[:, :1], a, attn.proj.bias, g1, _droppath_scale(blk.drop_path1, Bn, x.device),
                            blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)

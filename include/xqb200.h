@@ -385,8 +385,8 @@ int xq_diffaug_backward(const float *g, const float *rand01, int B, int C, int H
  *   x [M,K], w [N,K] (fc1.weight as bf16)  ->  pre [M,N] = x w^T ,  act [M,N] = GELU(pre + bias)                               */
 int xq_vit_fc1_gelu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int N, int K, void *stream);
 /*   pre may be NULL (inference: no backward will read it): the kernel then stores act only, bit-identical to the call with
- *   pre given.  The same holds for xq_vit_fc1_lora_gelu_fwd and xq_vit_fc1_swiglu_fwd and their _f16 twins; the backward
- *   entry points still require pre.                                                                                      */
+ *   pre given.  The same holds for xq_vit_fc1_lora_gelu_fwd and for the _f16 twins of both; the backward entry points
+ *   still require pre.                                                                                                    */
 /*  d_out [M,K] (gradient of the fc2 output), w2t [N,K] (fc2.weight TRANSPOSED, bf16), pre [M,N] (saved by the forward)
  *   ->  d_pre [M,N] = (d_out w2t^T) * GELU'(pre + bias) ,  d_bias [N] = column sums of the rounded d_pre                      */
 int xq_vit_fc2_dgelu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
@@ -415,24 +415,6 @@ int xq_vit_fc1_lora_gelu_fwd_f16(const void *x, const void *w, const void *u, co
                                  void *act, int M, int N, int K, int R, void *stream);
 int xq_vit_fc2_lora_dgelu_bwd_f16(const void *d_out, const void *w2t, const void *v, const void *a2t, const void *pre,
                                   const float *bias, void *d_pre, float *d_bias, int M, int N, int K, int R, void *stream);
-
-/* SwiGLU forms of xq_vit_fc1_gelu_fwd / xq_vit_fc2_dgelu_bwd for timm's GluMlp (vision_transformer.py:2925-2937):
- *   forward   F.linear(y, W1) [cuBLAS] + xq_vit_swiglu_fwd                       -> xq_vit_fc1_swiglu_fwd
- *   backward  g = d_out W2 [cuBLAS] + xq_vit_swiglu_bwd                          -> xq_vit_fc2_dswiglu_bwd
- *   x [M,K], w [2H,K] (fc1.weight), bias [2H]  ->  pre [M,2H] = x w^T ,  act [M,H] as xq_vit_swiglu_fwd computes it from pre
- *   d_out [M,K], w2t [H,K] (fc2.weight TRANSPOSED), pre [M,2H], bias [2H]
- *     ->  d_pre [M,2H] as xq_vit_swiglu_bwd computes it from g = 16-bit(d_out w2t^T),  d_bias [2H] (required)
- * Equal, bit for bit, to those two-call sequences up to the GEMM's fp32 accumulation order (d_bias: fp32 atomics, in no fixed
- * order).  The forward needs H % 64 == 0 and H / 64 <= SM count, the backward H % 128 == 0 and H / 128 <= SM count; both
- * K % 64 == 0 (else XQ_ERR_UNSUPPORTED); NULL or misaligned pointers give XQ_ERR_ARG.  A refused call writes nothing; no call
- * allocates. */
-int xq_vit_fc1_swiglu_fwd(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K, void *stream);
-int xq_vit_fc2_dswiglu_bwd(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre, float *d_bias,
-                           int M, int H, int K, void *stream);
-int xq_vit_fc1_swiglu_fwd_f16(const void *x, const void *w, const float *bias, void *pre, void *act, int M, int H, int K,
-                              void *stream);
-int xq_vit_fc2_dswiglu_bwd_f16(const void *d_out, const void *w2t, const void *pre, const float *bias, void *d_pre,
-                               float *d_bias, int M, int H, int K, void *stream);
 
 /* ---- input pipeline: the training / validation image transforms (SURVEY.md section 8 row f-4, csrc/img_kernels.cu) ---------
  * Replaces the per-image CPU transform of the reference's DataLoader workers:

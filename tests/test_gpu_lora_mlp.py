@@ -305,7 +305,7 @@ def test_lora_encoder_decoder_fused_path_matches_module_path():
             calls.append(name)
             return real_call(name, *a, **k)
 
-        _capi.call = vit_ops._call = spy
+        _capi.call = spy
         try:
             for m in (enc, dec):
                 m.zero_grad(set_to_none=True)
@@ -315,7 +315,7 @@ def test_lora_encoder_decoder_fused_path_matches_module_path():
             torch.manual_seed(13)
             (img.float() * torch.randn_like(img.float())).sum().backward()
         finally:
-            _capi.call = vit_ops._call = real_call
+            _capi.call = real_call
             vit_ops.MLP_TC_ENABLED[0] = True
         grads = {tag + n: p.grad.float().clone() for m, tag in ((enc, "enc."), (dec, "dec.")) for n, p in m.named_parameters()
                  if p.requires_grad}

@@ -1,14 +1,5 @@
-"""SwiGLU on the GPU: the fused GEMMs xq_vit_fc1_swiglu_fwd / xq_vit_fc2_dswiglu_bwd bit for bit against a library GEMM + the
-stand-alone xq_vit_swiglu_fwd / _bwd, the stand-alone kernels and the D = 1536 LayerNorm glue against fp64, and the giant /
-reg4 backbones end to end.
-
-Fused GEMMs: exact-grid operands as in test_gpu_mlp_gemm.py (A entries in {-1, 0, 1} * 2^-3, B entries in {-1, 0, 1} * 2^-2,
-K = 1536 < 2^11), so every GEMM result is exact in fp32 in any summation order and equals the 16-bit rounding of an fp64
-GEMM -- which is also what a library GEMM returns.  `pre`, `act` and `d_pre` are compared by equality (+0 / -0 aside where an
-exactly cancelling sum has no fixed sign).  d_b1 is summed with fp32 atomics whose order is not deterministic; it is checked
-against the fp64 column sums of the kernel's own d_pre within the fp32 summation depth.  Every output is NaN-filled and
-followed by guard rows holding a sentinel; the inputs carry extra nonzero rows after row M."""
-import math
+"""SwiGLU on the GPU: the stand-alone xq_vit_swiglu_fwd / _bwd and the D = 1536 LayerNorm glue against fp64, and the giant /
+reg4 backbones end to end (library GEMMs + the stand-alone SwiGLU kernel)."""
 import os
 import sys
 
@@ -21,8 +12,6 @@ pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-GUARD = 128
-SENTINEL = -12345
 DTYPES = {"bf16": (torch.bfloat16, ""), "f16": (torch.float16, "_f16")}
 EPS = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}       # one rounding to the 16-bit type, relative
 TINY = {torch.bfloat16: 2.0 ** -134, torch.float16: 2.0 ** -25}     # ... and absolute: half the subnormal spacing
@@ -37,78 +26,10 @@ def _nan(shape, dt):
     return torch.full(shape, float("nan"), dtype=dt, device="cuda")
 
 
-def _guarded(M, N, dt):
-    t = _nan((M + GUARD, N), dt)
-    t[M:].view(torch.int16).fill_(SENTINEL)
-    return t
-
-
-def _assert_guard(t, M, what):
-    bad = t[M:].view(torch.int16) != SENTINEL
-    assert not bool(bad.any()), f"{what}: {int(bad.sum())} guard elements after row {M} overwritten"
-
-
-def _assert_bits(a, b, what, zero_sign=False):
-    bad = a.view(torch.int16) != b.view(torch.int16)
-    if zero_sign:
-        bad &= ~((a == 0) & (b == 0))
-    assert not bool(bad.any()), f"{what}: {int(bad.sum())} of {bad.numel()} differ, first at {tuple(bad.nonzero()[0].tolist())}"
-
-
 def _assert_within(a, ref, tol, what):
     err = (a.double() - ref).abs()
     ok = err <= tol
     assert bool(ok.all()), f"{what}: {int((~ok).sum())} of {ok.numel()} out of tolerance, max err {err.max().item():.3e}"
-
-
-def _grid(rows, cols, scale, dt, gen):
-    return torch.randint(-1, 2, (rows, cols), device="cuda", generator=gen).to(dt) * scale
-
-
-# ---- fused GEMMs vs library GEMM + stand-alone kernel -----------------------------------------------------------------
-ROWS = [32 * 513, 32 * 517, 3 * 513, 3 * 517, 513, 517, 3 * 128 + 100]   # the last: a tail of 100 rows, into the 2nd warpgroup
-SMALL_H_ROWS = [513, 3 * 517, 3 * 128 + 100]
-
-
-@pytest.mark.parametrize("dtn", list(DTYPES))
-@pytest.mark.parametrize("H,M", [(4096, m) for m in ROWS] + [(384, m) for m in SMALL_H_ROWS])
-def test_fused_swiglu_gemms_bit_exact(H, M, dtn):
-    dt, sfx = DTYPES[dtn]
-    _capi, L = _lib()
-    p, s = _capi.ptr, _capi.stream_ptr()
-    K = 1536
-    gen = torch.Generator(device="cuda").manual_seed(H * 7 + M)
-    x = _grid(M + GUARD, K, 2.0 ** -3, dt, gen)
-    w1 = _grid(2 * H, K, 2.0 ** -2, dt, gen)
-    b1 = torch.randn(2 * H, device="cuda", generator=gen)
-    d_out = _grid(M + GUARD, K, 2.0 ** -3, dt, gen)
-    w2t = _grid(H, K, 2.0 ** -2, dt, gen)
-    pre, act, d_pre = _guarded(M, 2 * H, dt), _guarded(M, H, dt), _guarded(M, 2 * H, dt)
-    d_b1 = _nan((2 * H,), torch.float32)
-    _capi.check(getattr(L, "xq_vit_fc1_swiglu_fwd" + sfx)(p(x), p(w1), p(b1), p(pre), p(act), M, H, K, s), "fc1_swiglu_fwd")
-    _capi.check(getattr(L, "xq_vit_fc2_dswiglu_bwd" + sfx)(p(d_out), p(w2t), p(pre), p(b1), p(d_pre), p(d_b1), M, H, K, s),
-                "fc2_dswiglu_bwd")
-    # library path: the exact GEMM (= what the library GEMM returns on these operands) + the stand-alone kernels
-    pre_ref = (x[:M].double() @ w1.double().t()).to(dt)
-    _assert_bits(pre[:M], pre_ref, "pre vs library GEMM", zero_sign=True)
-    act_ref = _nan((M, H), dt)
-    _capi.check(getattr(L, "xq_vit_swiglu_fwd" + sfx)(p(pre_ref), p(b1), p(act_ref), M, H, s), "swiglu_fwd")
-    _assert_bits(act[:M], act_ref, "act vs library GEMM + xq_vit_swiglu_fwd")
-    g = (d_out[:M].double() @ w2t.double().t()).to(dt)
-    dp_ref, db_ref = _nan((M, 2 * H), dt), _nan((2 * H,), torch.float32)
-    _capi.check(getattr(L, "xq_vit_swiglu_bwd" + sfx)(p(pre_ref), p(b1), p(g), p(dp_ref), p(db_ref), M, H, s), "swiglu_bwd")
-    _assert_bits(d_pre[:M], dp_ref, "d_pre vs library GEMM + xq_vit_swiglu_bwd", zero_sign=True)
-    # d_b1: a column's terms pass through at most 16 + (tiles per CTA) fp32 adds in a thread and one atomic per CTA
-    t = d_pre[:M].double()
-    sums, abss = t.sum(0), t.abs().sum(0)
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    nM = (M + 127) // 128
-    per_col = min(sms // (H // 128), nM)
-    depth = 16 + -(-nM // per_col) + per_col + 2
-    _assert_within(d_b1, sums, depth * 2.0 ** -24 * abss, "d_b1 vs fp64 column sums of d_pre")
-    _assert_within(db_ref, sums, (M + 2) * 2.0 ** -24 * abss, "stand-alone d_b1 vs fp64 column sums")
-    for out, what in ((pre, "pre"), (act, "act"), (d_pre, "d_pre")):
-        _assert_guard(out, M, what)
 
 
 # ---- stand-alone SwiGLU against fp64 -----------------------------------------------------------------------------
@@ -171,8 +92,7 @@ def test_standalone_swiglu_exact_on_integer_inputs(dtn):
 
 @pytest.mark.parametrize("dtn", list(DTYPES))
 def test_silu_special_values_match_torch(dtn):
-    """silu at +-0, large +-x, where exp(-x) overflows, and at +-inf / NaN: the fused and stand-alone arithmetic (one device
-    function) against torch.nn.functional.silu on the same fp32 inputs, probed as act = silu(-0 + b) * (1 + 0) (-0 + b is b,
+    """silu at +-0, large +-x, where exp(-x) overflows, and at +-inf / NaN: the stand-alone kernel's arithmetic against torch.nn.functional.silu on the same fp32 inputs, probed as act = silu(-0 + b) * (1 + 0) (-0 + b is b,
     -0 included)"""
     dt, sfx = DTYPES[dtn]
     _capi, L = _lib()
@@ -249,18 +169,11 @@ def _build(cfg, depth, monkeypatch, det=True):
     return model
 
 
-@pytest.fixture
-def fused_on(monkeypatch):
-    """the fused SwiGLU GEMMs are opt-in (vit_ops.SWIGLU_TC_ENABLED, off by default: slower than the library path)"""
+def _count_swiglu(monkeypatch):
+    """counts the stand-alone SwiGLU nodes (vit_ops._SwiGLUBias) the model runs"""
     from imagefolder_b200 import vit_ops
-    monkeypatch.setattr(vit_ops, "SWIGLU_TC_ENABLED", [True])
-
-
-def _count_fused(monkeypatch):
-    from imagefolder_b200 import vit_ops
-    n = {"fused": 0, "swiglu": 0}
-    fused, lib = vit_ops._FusedSwiGLU.apply, vit_ops._SwiGLUBias.apply
-    monkeypatch.setattr(vit_ops._FusedSwiGLU, "apply", lambda *a: (n.__setitem__("fused", n["fused"] + 1), fused(*a))[1])
+    n = {"swiglu": 0}
+    lib = vit_ops._SwiGLUBias.apply
     monkeypatch.setattr(vit_ops._SwiGLUBias, "apply", lambda *a: (n.__setitem__("swiglu", n["swiglu"] + 1), lib(*a))[1])
     return n
 
@@ -271,24 +184,21 @@ def _giant_cfg(abs_pos_embed=True):
                 detail_guide="none", encoder_model=GIANT, decoder_model=GIANT)
 
 
-@pytest.mark.parametrize("fused", [True, False])
 @pytest.mark.parametrize("name", ["vit_giant_vq", "vit_giant_relpos", "vit_reg4_relpos"])
-def test_fused_path_matches_reference_golden(name, fused, monkeypatch):
+def test_fused_path_matches_reference_golden(name, monkeypatch):
     import ast
     g = np.load(os.path.join(HERE, "golden", name + ".npz"))
     cfg = ast.literal_eval(str(g["cfg_json"]))
     model = _build(cfg, int(g["giant_depth"]), monkeypatch).cuda().eval()
     from vit_det_init import golden_inputs
     x, q = golden_inputs(int(g["q_shape"][1]), int(g["q_shape"][2]))
-    from imagefolder_b200 import vit_ops
-    monkeypatch.setattr(vit_ops, "SWIGLU_TC_ENABLED", [fused])
-    n = _count_fused(monkeypatch)
+    n = _count_swiglu(monkeypatch)
     with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
         tok = model.encoder(x.cuda()).float().cpu().numpy()
         h = model.encode(x.cuda()).float().cpu().numpy()
         dec = model.decode(q.cuda()).float().cpu().numpy()
     if "giant" in name:
-        assert (n["fused"] > 0) == fused and (n["swiglu"] > 0) != fused
+        assert n["swiglu"] > 0
     st = int(g["token_stride"])
     for got, want in ((tok[:, ::st], g["tok_sub"]), (h.reshape(h.shape[0], h.shape[1], -1)[:, :, ::4], g["h_sub"]),
                       (dec[:, :, ::4, ::4], g["dec_sub"])):
@@ -301,9 +211,10 @@ def _enc_dec_loss(model, x, q, r1, r2):
 
 
 @pytest.mark.parametrize("dtn", list(DTYPES))
-def test_giant_parameter_gradients_against_fp64(dtn, fused_on, monkeypatch):
-    """every parameter gradient of the giant encoder + decoder (depth cut to 2, DropPath off) on the fused path against the
-    same modules run in fp64 (module path, no kernels of this library); fp16 through GradScaler"""
+def test_giant_parameter_gradients_against_fp64(dtn, monkeypatch):
+    """every parameter gradient of the giant encoder + decoder (depth cut to 2, DropPath off) on the fused ViT path (SwiGLU
+    MLP: library GEMMs + the stand-alone kernel) against the same modules run in fp64 (module path, no kernels of this
+    library); fp16 through GradScaler"""
     dt = DTYPES[dtn][0]
     model = _build(_giant_cfg(), 2, monkeypatch).cuda().train()
     for m in model.modules():
@@ -319,13 +230,13 @@ def test_giant_parameter_gradients_against_fp64(dtn, fused_on, monkeypatch):
     q = torch.randn(2, 32, 16, 16, device="cuda", generator=gen)
     r1 = torch.randn(2, 256, 1536, device="cuda", generator=gen) / 256
     r2 = torch.randn(2, 3, 256, 256, device="cuda", generator=gen) / 256
-    n = _count_fused(monkeypatch)
+    n = _count_swiglu(monkeypatch)
     scaler = torch.amp.GradScaler("cuda", init_scale=1024.0, enabled=dt == torch.float16)
     with torch.autocast("cuda", dtype=dt):
         loss = _enc_dec_loss(model, x, q, r1, r2)
     scaler.scale(loss).backward()
     inv = 1.0 / scaler.get_scale() if dt == torch.float16 else 1.0
-    assert n["fused"] == 4
+    assert n["swiglu"] == 4                                # the two blocks of the encoder and of the decoder
     loss64 = _enc_dec_loss(ref, x.double(), q.double(), r1.double(), r2.double())
     loss64.backward()
     ref_grads = dict(ref.named_parameters())
@@ -345,9 +256,8 @@ def test_giant_parameter_gradients_against_fp64(dtn, fused_on, monkeypatch):
 
 
 def test_full_depth_giant_fused_matches_library_path(monkeypatch):
-    """the 40-block giant encoder + decoder at batch 2, forward and backward: fused SwiGLU GEMMs against library GEMMs +
-    the stand-alone kernel (same modules, same bf16 autocast)"""
-    from imagefolder_b200 import vit_ops
+    """the 40-block giant encoder + decoder at batch 2, forward and backward under bf16 autocast on the fused ViT path (SwiGLU
+    MLP: library GEMMs + the stand-alone kernel): the tokens, the image and the picked gradients are finite"""
     model = _build(_giant_cfg(), 40, monkeypatch, det=False).cuda().train()
     with torch.no_grad():
         for name, p in model.named_parameters():
@@ -363,24 +273,16 @@ def test_full_depth_giant_fused_matches_library_path(monkeypatch):
     r2 = torch.randn(2, 3, 256, 256, device="cuda", generator=gen) / 256
     picks = ["encoder.model.blocks.0.mlp.fc1.weight", "encoder.model.blocks.39.mlp.fc2.weight",
              "decoder.model.blocks.20.mlp.fc1.bias", "decoder.model.blocks.0.attn.qkv.weight"]
-    runs = []
-    for fused in (True, False):
-        monkeypatch.setattr(vit_ops, "SWIGLU_TC_ENABLED", [fused])
-        model.zero_grad(set_to_none=True)
-        n = _count_fused(monkeypatch)
-        with torch.autocast("cuda", dtype=torch.bfloat16):
-            tok = model.encoder(x).float()
-            dec = model.decode(q).float()
-            loss = (tok * r1).sum() + (dec * r2).sum()
-        loss.backward()
-        assert (n["fused"] > 0) == fused and (n["swiglu"] > 0) != fused
-        params = dict(model.named_parameters())
-        runs.append((tok.detach(), dec.detach(), {k: params[k].grad.detach().clone() for k in picks}))
-    (t1, d1, g1), (t2, d2, g2) = runs
-    for a, b, what in [(t1, t2, "tokens"), (d1, d2, "image")] + [(g1[k], g2[k], k) for k in picks]:
+    n = _count_swiglu(monkeypatch)
+    with torch.autocast("cuda", dtype=torch.bfloat16):
+        tok = model.encoder(x).float()
+        dec = model.decode(q).float()
+        loss = (tok * r1).sum() + (dec * r2).sum()
+    loss.backward()
+    assert n["swiglu"] == 2 * 40
+    params = dict(model.named_parameters())
+    for a, what in [(tok, "tokens"), (dec, "image")] + [(params[k].grad, k) for k in picks]:
         assert bool(torch.isfinite(a).all()), what
-        rel = float((a - b).norm() / b.norm().clamp_min(1e-30))
-        assert rel < 5e-2, (what, rel)
 
 
 def test_reg4_model_training_step(monkeypatch):
@@ -413,10 +315,10 @@ def test_lora_giant_takes_library_path_and_matches(monkeypatch):
                 p.normal_(0, 0.02)                      # nonzero adapters: the LoRA term contributes
     gen = torch.Generator(device="cuda").manual_seed(8)
     x = torch.rand(2, 3, 256, 256, device="cuda", generator=gen) * 2 - 1
-    n = _count_fused(monkeypatch)
+    n = _count_swiglu(monkeypatch)
     with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
         tok = model.encoder(x).float()
-    assert n["fused"] == 0 and n["swiglu"] == 2
+    assert n["swiglu"] == 2
     with torch.no_grad():
         ref = model.encoder.double()(x.double())
     rel = float((tok.double() - ref).norm() / ref.norm())

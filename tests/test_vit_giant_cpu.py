@@ -112,26 +112,17 @@ def test_swiglu_entry_points_refuse_bad_arguments_without_writing():
         assert fwd(4096, f, 4096, 0, 64, None) == -1
         assert bwd(4096, f, None, 4096, f, 4, 64, None) == -1
         assert bwd(4096, f, 4096, 4096, f, 4, 12, None) == -1
-        ffwd, fbwd = getattr(L, "xq_vit_fc1_swiglu_fwd" + sfx), getattr(L, "xq_vit_fc2_dswiglu_bwd" + sfx)
-        assert ffwd(None, 4096, f, 4096, 4096, 128, 4096, 1536, None) == -1
-        assert ffwd(4096, 4096, f, 4096, 4096, 0, 4096, 1536, None) == -1  # M = 0
-        assert ffwd(4096, 4096, f, 4096, 4096, 128, 0, 1536, None) == -1   # H = 0
-        assert ffwd(4096, 4096, f, 4096, 4096, 128, 4000, 1536, None) == -4  # 2H % 128 != 0
-        assert ffwd(4096, 4096, f, 4096, 4096, 128, 4096, 100, None) == -4   # K % 64 != 0
-        assert ffwd(4100, 4096, f, 4096, 4096, 128, 4096, 1536, None) == -1  # x misaligned
-        assert fbwd(4096, 4096, 4096, f, 4096, None, 128, 4096, 1536, None) == -1   # no bias-gradient buffer
-        assert fbwd(4096, None, 4096, f, 4096, f, 128, 4096, 1536, None) == -1
-        assert fbwd(4096, 4096, 4096, f, 4096, f, 128, 4032, 1536, None) == -4      # H % 128 != 0
-        assert fbwd(4096, 4096, 4096, f, 4096, f, 128, 4096, 1000, None) == -4      # K % 64 != 0
     assert L.xq_vit_residual_ln_fwd(None, None, None, None, None, 1, None, None, 1e-6, 4, 1536, None, None, None, None,
                                     None) == -1
 
 
 def test_swiglu_dispatch_conditions():
-    from imagefolder_b200 import vit_ops
+    from imagefolder_b200 import _capi, vit_ops
     assert 1536 in vit_ops._SUPPORTED_D
-    mlp = vt.GluMlp(1536, hidden_features=8192)
-    assert not vit_ops.swiglu_tc_ok(torch.zeros(4, 1536, dtype=torch.bfloat16), mlp.fc1, mlp.fc2)   # CPU: never
+    # the giant MLP has no fused SwiGLU GEMMs: an export of one means a stale object file in the library
+    L = _capi.lib()
+    for name in ("xq_vit_fc1_swiglu_fwd", "xq_vit_fc2_dswiglu_bwd"):
+        assert not hasattr(L, name) and not hasattr(L, name + "_f16"), name
 
 
 # ---- goldens from the reference's own modules ---------------------------------------------------------------------
